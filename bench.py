@@ -4,10 +4,14 @@
 One "step" = one frame of the hot path: projection -> key duplication -> radix sort -> tile ranges ->
 alpha blend, on a synthetic splat cloud already resident in HBM.  Default workload = BASELINE.json
 configs[2] ("c3"): 6 M splats, 1920x1080, 1-degree-per-frame orbit (the configuration the north-star target
-">= 60 fps on a 6 M-splat scene @1080p on 1xB200" is quoted on).  N > 1 GPUs: screen-tile-row bands, one NCCL
+">= 60 fps on a 6 M-splat scene @1080p on 1xH100" is quoted on).  N > 1 GPUs: screen-tile-row bands, one NCCL
 gather of the framebuffer per frame (strong scaling: the frame is fixed, the GPUs split it).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4] [--impl gsr|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c2|c3|c4|c5] [--impl gsr|reference] [--dump-outputs DIR]
+
+--dump-outputs DIR writes what the timed path computed in its last timed step as DIR/<name>.npy (float32 / float64, at most
+64 MB in all): the RGBA32F frame (a fixed, seeded sample of its pixels when the frame is larger), or for c5 the sorted keys
+and values of the largest size (a fixed, seeded sample).  Inputs are seeded, so two builds can be compared output for output.
 
 `--impl reference` times the CPU restatement of the reference pipeline (oracle/, all host threads) -- the
 reference itself needs Godot 4.3 + a Vulkan device and cannot run on this box (BASELINE.md section 2).
@@ -56,7 +60,33 @@ def parse_args():
                          "NVLink peer memory + 4-byte NCCL sync; 'nccl' = NCCL gather of the band framebuffers")
     ap.add_argument("--overlap", type=int, default=-1, choices=[-1, 0, 1],
                     help="front/back overlap of consecutive frames (gsr_debug_pipeline): -1 = the library's default (off)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy (float32/float64, <= 64 MB)")
+    args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "gsr" or args.gpus != 1):
+        ap.error("--dump-outputs needs --impl gsr and --gpus 1")
+    return args
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes {name: array} as out_dir/<name>.npy.  An array past its share of DUMP_LIMIT_BYTES is replaced by a fixed, seeded
+    sample of its leading-axis rows (`<name>_sample`, rows in ascending order) plus those row indices (`<name>_sample_index`)."""
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // len(arrays) - 1024   # room for the .npy headers
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        if a.nbytes > share:
+            row = a.nbytes // a.shape[0]
+            keep = (share - 8) // (row + 8)   # float64 index per kept row
+            idx = np.sort(np.random.default_rng(12345).choice(a.shape[0], size=keep, replace=False))
+            np.save(os.path.join(out_dir, f"{name}_sample.npy"), np.ascontiguousarray(a[idx]))
+            np.save(os.path.join(out_dir, f"{name}_sample_index.npy"), idx.astype(np.float64))
+        else:
+            np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def frame_params(wl, n_frames, first=0):
@@ -112,15 +142,16 @@ def make_config(args, wl):
         par += "; e2e: every rank reads its own rows back into one shared page-locked host frame (device-resident leg: frame assembled in rank 0's HBM)"
     return {"workload": f"{args.workload}: {wl['desc']}", "splats": wl["n"], "width": wl["w"], "height": wl["h"], "sh_degree": 3,
             "parallelism": par, "reduced": bool(args.splats),
-            "l2": "inputs larger than L2 (SoA splats %.0f MB + records + pairs per frame >> 126 MB)" % (240 * wl["n"] / 1e6)}
+            "l2": "inputs larger than L2 (SoA splats %.0f MB + records + pairs per frame >> 50 MB)" % (240 * wl["n"] / 1e6)}
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
     def __init__(self, index):
+        self.index = index
         self.f = tempfile.NamedTemporaryFile("w+", suffix=".csv", delete=False)
         self.p = None
         try:
@@ -157,7 +188,16 @@ class ClockSampler:
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["no samples"]}
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "power_w_max": float(max(pw)), "samples": len(sm),
-                "reasons": sorted(reasons)}
+                "reasons": sorted(reasons), **self.device()}
+
+    def device(self):
+        """The card's name and power limit: part of every number measured on it."""
+        try:
+            out = subprocess.run(["nvidia-smi", "-i", str(self.index), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                                 capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+            return {"gpu": out[0], "power_limit_w": float(out[1])}
+        except (OSError, subprocess.SubprocessError, IndexError, ValueError):
+            return {"gpu": None, "power_limit_w": None}
 
 
 def measured_peak_gbs():
@@ -165,22 +205,7 @@ def measured_peak_gbs():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (copy, measured on this pool)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
-
-
-def profiled_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed ncu --set full
-    capture (profiles/rNN_traffic.json, written by profiles/summarize_ncu.py from the round's .ncu-rep)."""
-    import glob
-    for path in sorted(glob.glob(os.path.join(ROOT, "profiles", "r*_traffic.json")), reverse=True):
-        try:
-            with open(path) as f:
-                d = json.load(f)
-            if kernel_key in d:
-                return float(d[kernel_key]), os.path.relpath(path, ROOT)
-        except Exception:
-            continue
-    return None, None
+        return 3350.0, "fallback 3.35 TB/s (NVIDIA H100 SXM data sheet HBM3 bandwidth; not measured)"
 
 
 def tune_cpu_threads(wl, splat60, frame):
@@ -285,20 +310,25 @@ def run_c5(args):
     sizes = [20, 22, 24, 26, 28]
     res = {}
     for lg in sizes:
-        res[f"2^{lg}"] = radix_microbench(torch, 0, 1 << lg)
+        last = {} if (args.dump_outputs and lg == sizes[-1]) else None
+        res[f"2^{lg}"] = radix_microbench(torch, 0, 1 << lg, steps=args.steps, warmup=args.warmup, last=last)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"sorted_keys": last["keys"], "sorted_values": last["values"]})
     top = res[f"2^{sizes[-1]}"]
     peak, peak_src = measured_peak_gbs()
-    emit({"metric": "Gkeys/s", "value": top["pairs"]["gkeys_s"], "unit": "Gpairs/s (32-bit key + 32-bit value)", "n_gpus": 1, "steps": 3, "warmup": 1,
+    emit({"metric": "Gkeys/s", "value": top["pairs"]["gkeys_s"], "unit": "Gpairs/s (32-bit key + 32-bit value)", "n_gpus": 1, "steps": args.steps, "warmup": args.warmup,
           "ms_per_step": top["pairs"]["ms"], "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u32", "data": "synthetic",
           "config": {"workload": "c5: " + WORKLOADS["c5"]["desc"], "sizes": res, "l2": "2^26 and 2^28 exceed L2; smaller sizes are L2-resident"},
           "roofline": {"kernel": "sort_hist_kernel + 4x onesweep_kernel", "bound": "hbm", "achieved": top["pairs"]["hbm_frac_of_measured"] * peak, "peak": peak,
                        "unit": "GB/s", "frac": top["pairs"]["hbm_frac_of_measured"], "traffic": None, "peak_source": peak_src,
                        "algorithmic_bytes": "68 B per pair (36 B per key keys-only), SURVEY 8d"},
-          "keys_only_gkeys_s": top["keys"]["gkeys_s"], "gpu_launches": 5 * 4 * 2 * len(sizes), "e2e": None, "cpu_baseline": None})
+          "keys_only_gkeys_s": top["keys"]["gkeys_s"], "gpu_launches": 5 * (args.warmup + args.steps) * 2 * len(sizes), "e2e": None, "cpu_baseline": None})
 
 
-def radix_microbench(torch, device_index, n=1 << 26):
-    """config c5 point: n (tile<<16|depth16) keys + u32 values, device resident, CUDA events on the sort stream."""
+def radix_microbench(torch, device_index, n=1 << 26, steps=3, warmup=1, last=None):
+    """config c5 point: n (tile<<16|depth16) keys + u32 values, device resident, CUDA events on the sort stream; mean of `steps`
+    timed sorts after `warmup` untimed ones.  last: optional dict that receives the pairs sort's last output as float64 (the 32-bit
+    words are exact there)."""
     import ctypes as C
     from godotgaussiansplatting_b200 import _lib
     from godotgaussiansplatting_b200.synthetic import radix_keys
@@ -311,7 +341,7 @@ def radix_microbench(torch, device_index, n=1 << 26):
     try:
         for name, with_vals in (("pairs", True), ("keys", False)):
             best = []
-            for it in range(4):
+            for it in range(warmup + steps):
                 k = keys.clone()
                 v = vals.clone() if with_vals else None
                 torch.cuda.synchronize()
@@ -320,8 +350,11 @@ def radix_microbench(torch, device_index, n=1 << 26):
                 torch.cuda.synchronize()
                 ms = C.c_float()
                 _lib.check(L.gsr_sorter_last_ms(s, C.byref(ms)), "ms")
-                if it:
+                if it >= warmup:
                     best.append(ms.value)
+            if last is not None and with_vals:
+                last["keys"] = k.cpu().numpy().view(np.uint32).astype(np.float64)
+                last["values"] = v.cpu().numpy().view(np.uint32).astype(np.float64)
             t = float(np.mean(best))
             out[name] = {"n": n, "ms": t, "gkeys_s": n / t / 1e6, "hbm_frac_of_measured": (n * (68 if with_vals else 36) / (t * 1e-3)) / 1e9 / measured_peak_gbs()[0]}
     finally:
@@ -524,6 +557,9 @@ def main():
     sampler = ClockSampler(torch.cuda.current_device() if "CUDA_VISIBLE_DEVICES" not in os.environ else local_rank) if rank == 0 else None
     total_ms = timed(e2e=False)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs:   # the frame of the last timed step, as the caller of the device-resident path reads it
+        rast.sync()
+        dump_outputs(args.dump_outputs, {"rgba": rast.read_framebuffer().reshape(H * W, 4)})
     hist = rast.frame_history(min(args.steps, 512))
     st = rast.stats()
     e2e_ms = timed(e2e="rgba")
@@ -559,14 +595,11 @@ def main():
     dominant = max(("Projection", "Sort", "Render"), key=lambda k: stage[k])
     dom_bytes = {"Projection": bytes_proj, "Sort": bytes_sort, "Render": bytes_comp}[dominant]
     proj_name = "projection_scatter_kernel + segment wait + gather_segments_kernel" if group else "projection_kernel"
-    traffic, traffic_src = profiled_traffic({"Projection": "projection_kernel", "Sort": "onesweep_kernel", "Render": "composite_kernel"}[dominant])
-    if group and dominant == "Projection":
-        traffic, traffic_src = None, "no single-GPU ncu capture of the scatter projection (its stores go to peer memory)"
     roofline = {"kernel": {"Projection": proj_name, "Sort": "sort_hist_kernel + 4x onesweep_kernel", "Render": "composite_kernel"}[dominant],
                 "bound": "hbm", "achieved": gbs(dom_bytes, stage[dominant]), "peak": peak, "unit": "GB/s",
-                "frac": gbs(dom_bytes, stage[dominant]) / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-                "note": ("the compositor is FP32-issue/FMA-pipe bound, not HBM bound (ncu: FMA pipe ~55-70 % of active cycles, DRAM 4 %); its HBM "
-                         "fraction is reported because the contract asks for it; see per_stage for the HBM-bound kernels") if dominant == "Render" else None,
+                "frac": gbs(dom_bytes, stage[dominant]) / peak, "traffic": None, "peak_source": peak_src,
+                "note": ("the compositor is bound by FP32 issue and its sequential per-tile chains, not by HBM; its HBM fraction is "
+                         "reported because the contract asks for it; see per_stage for the HBM-bound kernels") if dominant == "Render" else None,
                 "algorithmic_bytes_per_launch": dom_bytes, "avg_launch_ms": stage[dominant],
                 "timing": "CUDA events recorded by libgsr on the render stream around every stage of every timed frame (gsr_get_frame_history)",
                 "per_stage": {

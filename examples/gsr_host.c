@@ -13,7 +13,7 @@
  *                                      frame statistics main.gd:93-119 shows (M, overflow flag, stage times).
  *
  * Exit codes: 0 ok; 2 usage / unreadable request; 3 a libgsr call failed (message on stderr) -- in particular
- * GSR_ERR_CUDA without an sm_100 device: there is no CPU fallback.
+ * GSR_ERR_CUDA without an sm_90 device: there is no CPU fallback.
  *
  * Build: gcc -std=c99 -O2 -Iinclude examples/gsr_host.c -Lgodotgaussiansplatting_b200 -lgsr -Wl,-rpath,... -o gsr_host
  */

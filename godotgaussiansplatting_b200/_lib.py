@@ -1,7 +1,7 @@
 """ctypes binding of the in-tree `libgsr.so` (include/gsr.h).
 
 There is NO fallback: if the shared library is missing or does not load, importing a symbol raises, and
-every entry point fails with GSR_ERR_CUDA when no sm_100 device is present.
+every entry point fails with GSR_ERR_CUDA when no sm_90 device is present.
 """
 from __future__ import annotations
 
@@ -65,7 +65,7 @@ def lib():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(f"{LIB_PATH} is missing: build it with `python -m godotgaussiansplatting_b200.build` "
-                              "(nvcc, sm_100a). There is no CPU fallback.")
+                              "(nvcc, sm_90a). There is no CPU fallback.")
         L = C.CDLL(LIB_PATH)
         vp, fp, u32 = C.c_void_p, C.POINTER(C.c_float), C.c_uint32
         L.gsr_create.argtypes = [C.POINTER(GsrConfig), C.POINTER(vp)]

@@ -1,4 +1,4 @@
-"""Builds godotgaussiansplatting_b200/csrc/*.cu into the in-tree shared library `libgsr.so` for sm_100a.
+"""Builds godotgaussiansplatting_b200/csrc/*.cu into the in-tree shared library `libgsr.so` for sm_90a (H100).
 
 nvcc cross-compiles without a GPU; the .so travels to the GPU box with the repo snapshot.
 -fmad=false is part of the numerical contract ("gsr deterministic math", DESIGN.md section 4): every
@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libgsr.so")
 
 NVCC_FLAGS = [
-    "-std=c++17", "-O3", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+    "-std=c++17", "-O3", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
     "-Xcompiler", "-fPIC,-fvisibility=hidden", "-shared", "-cudart", "shared",
 ]

@@ -1,4 +1,4 @@
-// common.cuh -- shared declarations of libgsr (sm_100a).  Product code: never includes anything from oracle/.
+// common.cuh -- shared declarations of libgsr (sm_90a).  Product code: never includes anything from oracle/.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,31 +1,29 @@
 // compositor.cu -- stage 4: per-tile front-to-back alpha blend.  Replaces gsplat_render.glsl:50-111.
 //
 // One CTA per 16x16 tile like the reference's workgroup, 256-splat chunks staged in shared memory, the same per-pixel
-// arithmetic and the same tile-stop vote.  What is Blackwell-specific is how the blend is issued and scheduled:
-//   * the kernel is FMA-pipe bound (113 FMA-pipe instructions per 4 splats and pixel pair; measured on B200, ubench/f32x2_latency.cu:
-//     FFMA2 and scalar FFMA both retire 128 lane-FMAs/clk/SM, FFMA2 at half the issue slots, dependent-issue latency 4 cycles), so
-//     every thread owns TWO horizontally adjacent pixels and the blend runs on packed fp32x2 instructions
-//     (PTX add/sub/mul/fma.rn.f32x2 -> SASS FADD2/FMUL2/FFMA2).  Each lane of a packed op is an ordinary IEEE binary32 operation,
-//     so results stay bit-identical to the oracle;
+// arithmetic and the same tile-stop vote.  How the blend is issued and scheduled on sm_90:
+//   * the blend is almost all FP32 arithmetic, so every thread owns TWO horizontally adjacent pixels: the per-splat shared-memory loads
+//     and broadcasts are paid once for two pixels, and the two pixels' dependency chains interleave (Hopper has no packed
+//     fp32x2 instructions; each F2 operation below is two scalar IEEE binary32 operations with explicit rounding, so results
+//     stay bit-identical to the oracle);
 //   * per-splat control flow is gone: dead pixels (t <= 1/255, gsplat_render.glsl:79) keep their state by select, the warp-level
 //     "all dead" test runs once per 4 splats on the transmittance of half a group earlier (off the loop-carried path), and the
 //     last chunk is padded with null splats (opacity 0);
 //   * the transmittance chain is two instructions per splat: alpha and 1 - alpha are formed off the critical path, the update is
-//     FMUL2 + select (`t = alive ? t * (1 - alpha) : t`, bit-identical to multiplying by 1 - 0);
+//     FMUL + select per pixel (`t = alive ? t * (1 - alpha) : t`, bit-identical to multiplying by 1 - 0);
 //   * the conic is pre-scaled at staging time (-0.5*cx, -0.5*cz, -cy: exact power-of-two/sign changes) so the `-0.5 * (...)`
 //     multiply of :84 disappears from the inner loop without changing any rounding;
 //   * the gather `culled_buffer[sort_buffer[...]]` (:72) for chunk i+1 is issued into registers before the blend loop of chunk i
 //     (software prefetch), and the (a, b) words of splat group g+1 are read from shared memory while group g is blended;
 //   * the tile-stop vote `atomicAdd(shared_t, uint(t*255))` (:97) is a warp reduction + 4 shared words;
-//   * scheduling (measured, profiles/r02_compositor_*): a tile is a sequential chain of up to ~19 chunks, a frame has ~1250 such
-//     chains of very different length, and the SM's warp scheduler favours its oldest warps -- so the persistent grid takes tiles
-//     LONGEST-FIRST (tile_order_kernel: the previous frame's consumed chunk count of the tile, else its list length), keeps few
-//     CTAs per SM and never migrates a tile (the round-1 re-queue mechanism cost a spill + restore per hand-back and made long
-//     chains young again; measured slower than this order).
+//   * scheduling: a tile is a sequential chain of up to ~19 chunks, a c3 frame has ~1250 such chains of very different length,
+//     and the SM's warp scheduler favours its oldest warps -- so the persistent grid takes tiles LONGEST-FIRST (tile_order_kernel:
+//     the previous frame's consumed chunk count of the tile, else its list length), keeps few CTAs per SM and never migrates a
+//     tile (handing a tile back costs a spill + restore and makes long chains young again).
 // Arithmetic contract: "gsr deterministic math" (common.cuh): the GLSL-legal contractions of :84 and :89 are explicit fma
 // (CONTRACT = true, the default); CONTRACT = false (GSR_FLAG_UNCONTRACTED_BLEND) evaluates :84-90 with no contraction at all,
 // which is bit-identical to the reference's own shader text executed by oracle/glsl_cpu.  exp() is the det_exp() polynomial,
-// evaluated here two lanes at a time.
+// evaluated here for both pixels side by side.
 #include <stdlib.h>
 #include <string.h>
 
@@ -39,35 +37,17 @@ constexpr int CHUNK = 256;    // gsplat_render.glsl:9 WORKGROUP_SIZE: splats per
 constexpr int THREADS = 128;  // 2 pixels per thread
 constexpr float MIN_ALPHA = 1.0f / 255.0f;
 
-typedef unsigned long long u64;
-
-#ifndef GSR_CPU_EMU
-__device__ __forceinline__ u64 pk(float lo, float hi) { u64 r; asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void upk(u64 v, float &lo, float &hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ u64 fma2(u64 a, u64 b, u64 c) { u64 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ u64 mul2(u64 a, u64 b) { u64 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 add2(u64 a, u64 b) { u64 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ u64 sub2(u64 a, u64 b) { u64 d; asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-// a*b + c with TWO roundings per lane, for the uncontracted evaluation.  ptxas (12.9, sm_100a) contracts a mul.rn.f32x2 whose only use
-// is an add.rn.f32x2 into one FFMA2 -- in spite of the .rn qualifiers and of -fmad=false (cuobjdump: 44 FFMA2 where the PTX has 24
-// fma.rn.f32x2; tests/test_gpu_pipeline.py::test_uncontracted_blend_flag_... caught it on silicon).  It honours the scalar .rn pair.
-__device__ __forceinline__ u64 mul_add2_unfused(u64 a, u64 b, u64 c) {
-    float al, ah, bl, bh, cl, ch;
-    asm volatile("mov.b64 {%0, %1}, %2;" : "=f"(al), "=f"(ah) : "l"(a));
-    upk(b, bl, bh); upk(c, cl, ch);
-    return pk(__fadd_rn(__fmul_rn(al, bl), cl), __fadd_rn(__fmul_rn(ah, bh), ch));
-}
-#else  // tests/kernel_emu: the kernels of this file compiled for the CPU (test infrastructure; libgsr never defines GSR_CPU_EMU).
-       // A packed op is two independent IEEE binary32 operations -- exactly what the PTX f32x2 instructions are.
-inline u64 pk(float lo, float hi) { uint32_t a, b; memcpy(&a, &lo, 4); memcpy(&b, &hi, 4); return (u64)a | ((u64)b << 32); }
-inline void upk(u64 v, float &lo, float &hi) { const uint32_t a = (uint32_t)v, b = (uint32_t)(v >> 32); memcpy(&lo, &a, 4); memcpy(&hi, &b, 4); }
-inline u64 fma2(u64 a, u64 b, u64 c) { float al, ah, bl, bh, cl, ch; upk(a, al, ah); upk(b, bl, bh); upk(c, cl, ch); return pk(fmaf(al, bl, cl), fmaf(ah, bh, ch)); }
-inline u64 mul2(u64 a, u64 b) { float al, ah, bl, bh; upk(a, al, ah); upk(b, bl, bh); return pk(al * bl, ah * bh); }
-inline u64 add2(u64 a, u64 b) { float al, ah, bl, bh; upk(a, al, ah); upk(b, bl, bh); return pk(al + bl, ah + bh); }
-inline u64 sub2(u64 a, u64 b) { float al, ah, bl, bh; upk(a, al, ah); upk(b, bl, bh); return pk(al - bl, ah - bh); }
-inline u64 mul_add2_unfused(u64 a, u64 b, u64 c) { return add2(mul2(a, b), c); }
-#endif
-__device__ __forceinline__ u64 bc(float x) { return pk(x, x); }
+// The two pixels of a thread.  __f*_rn are never contracted (nvcc, and -ffp-contract=off in tests/kernel_emu).
+struct F2 { float lo, hi; };
+__device__ __forceinline__ F2 pk(float lo, float hi) { F2 r; r.lo = lo; r.hi = hi; return r; }
+__device__ __forceinline__ void upk(F2 v, float &lo, float &hi) { lo = v.lo; hi = v.hi; }
+__device__ __forceinline__ F2 fma2(F2 a, F2 b, F2 c) { return pk(__fmaf_rn(a.lo, b.lo, c.lo), __fmaf_rn(a.hi, b.hi, c.hi)); }
+__device__ __forceinline__ F2 mul2(F2 a, F2 b) { return pk(__fmul_rn(a.lo, b.lo), __fmul_rn(a.hi, b.hi)); }
+__device__ __forceinline__ F2 add2(F2 a, F2 b) { return pk(__fadd_rn(a.lo, b.lo), __fadd_rn(a.hi, b.hi)); }
+__device__ __forceinline__ F2 sub2(F2 a, F2 b) { return pk(__fsub_rn(a.lo, b.lo), __fsub_rn(a.hi, b.hi)); }
+// a*b + c with TWO roundings per lane, for the uncontracted evaluation
+__device__ __forceinline__ F2 mul_add2_unfused(F2 a, F2 b, F2 c) { return add2(mul2(a, b), c); }
+__device__ __forceinline__ F2 bc(float x) { return pk(x, x); }
 
 struct Staged {  // one gathered record, pre-scaled for the inner loop
     float4 a;    // image_pos.x, image_pos.y, -0.5*conic.x, -0.5*conic.z
@@ -108,8 +88,8 @@ inline unsigned long long globaltimer_ns() { return 0ull; }
 inline uint32_t smid() { return 0u; }
 #endif
 
-struct BlendK {  // broadcast constants of det_exp() for the packed lanes
-    u64 L2E2, MAGIC2, ONE2, C6, C5, C4, C3, C2, C1;
+struct BlendK {  // broadcast constants of det_exp() for the two pixels
+    F2 L2E2, MAGIC2, ONE2, C6, C5, C4, C3, C2, C1;
 };
 __device__ __forceinline__ BlendK make_blend_k() {
     BlendK k;
@@ -123,9 +103,9 @@ __device__ __forceinline__ BlendK make_blend_k() {
 //      two pixels, written stage by stage so that the GU dependency chains can be interleaved.  No dependence on the transmittance:
 //      this part of gsplat_render.glsl:84-88 runs ahead of the sequential blend.
 template <bool CONTRACT>
-__device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], u64 npx2, float fpy, const BlendK &K, u64 al2[GU], u64 om2[GU]) {
+__device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], F2 npx2, float fpy, const BlendK &K, F2 al2[GU], F2 om2[GU]) {
     float oy[GU];
-    u64 ox2[GU], pw2[GU], tm2[GU], e2[GU];
+    F2 ox2[GU], pw2[GU], tm2[GU], e2[GU];
 #pragma unroll
     for (int u = 0; u < GU; ++u) { ox2[u] = add2(bc(A[u].x), npx2); oy[u] = A[u].y - fpy; }
     // power = -0.5*(cx*ox*ox + cz*oy*oy) - cy*ox*oy (:84) on the pre-scaled conic:
@@ -143,7 +123,7 @@ __device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], 
     for (int u = 0; u < GU; ++u) e2[u] = mul2(bc(B[u].x), ox2[u]);
 #pragma unroll
     for (int u = 0; u < GU; ++u) pw2[u] = CONTRACT ? fma2(e2[u], bc(oy[u]), pw2[u]) : mul_add2_unfused(e2[u], bc(oy[u]), pw2[u]);
-    // exp(power): det_exp(), two lanes at a time
+    // exp(power): det_exp() of both pixels
 #pragma unroll
     for (int u = 0; u < GU; ++u) pw2[u] = mul2(pw2[u], K.L2E2);
 #pragma unroll
@@ -189,7 +169,7 @@ __device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], 
 // ---- phase B: the sequential part (gsplat_render.glsl:89-90).  A dead pixel has left the reference's loop: its colour and
 //      transmittance are kept by select.  `alive_mid` = "a pixel of this thread was alive after the first half of the group".
 template <bool CONTRACT>
-__device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, int j, const u64 al2[GU], const u64 om2[GU], u64 &cr2, u64 &cg2, u64 &cb2,
+__device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, int j, const F2 al2[GU], const F2 om2[GU], F2 &cr2, F2 &cg2, F2 &cb2,
                                         float &t0, float &t1, bool &alive_mid) {
 #pragma unroll
     for (int u = 0; u < GU; ++u) {
@@ -198,9 +178,9 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, in
         const bool a0 = t0 > MIN_ALPHA, a1 = t1 > MIN_ALPHA;
         float al, ah, pl, ph;
         upk(al2[u], al, ah);
-        const u64 t2 = pk(t0, t1);
+        const F2 t2 = pk(t0, t1);
         upk(mul2(t2, om2[u]), pl, ph);
-        const u64 m2 = pk(a0 ? al : 0.0f, a1 ? ah : 0.0f);   // alpha = 0: an exact no-op on the colour
+        const F2 m2 = pk(a0 ? al : 0.0f, a1 ? ah : 0.0f);   // alpha = 0: an exact no-op on the colour
         if (CONTRACT) {
             cr2 = fma2(mul2(bc(B[u].z), m2), t2, cr2);
             cg2 = fma2(mul2(bc(B[u].w), m2), t2, cg2);
@@ -216,7 +196,7 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, in
 }
 
 #ifndef GSR_COMP_MIN_BLOCKS
-#define GSR_COMP_MIN_BLOCKS 3  // resident CTAs per SM the register allocation targets (profiles/r02_compositor_sweep.txt: 2-3 is best)
+#define GSR_COMP_MIN_BLOCKS 3  // resident CTAs per SM the register allocation targets
 #endif
 
 // Persistent CTAs.  Ticket k of the launch renders owned tile order[k] (longest chains first) or k itself; every tile is blended
@@ -252,7 +232,7 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
 
         const uint32_t tx = tile_id % (uint32_t)p.tiles_x, ty = tile_id / (uint32_t)p.tiles_x;
         const int px0 = (int)(tx * TILE + 2u * (tid & 7u)), py = (int)(ty * TILE + (tid >> 3));
-        const u64 npx2 = pk(-(float)px0, -(float)(px0 + 1));  // ox = image_pos.x - pixel.x  ==  image_pos.x + (-pixel.x)
+        const F2 npx2 = pk(-(float)px0, -(float)(px0 + 1));  // ox = image_pos.x - pixel.x  ==  image_pos.x + (-pixel.x)
         const float fpy = (float)py;
 
         const uint2 bounds = p.bounds[tile_id];
@@ -260,7 +240,7 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         const int num_splats = diff > 0 ? diff : 0;                              // :61
         const int num_iterations = (int)ceilf((float)num_splats / (float)CHUNK);  // :62
 
-        u64 cr2 = pk(0.f, 0.f), cg2 = cr2, cb2 = cr2;  // blended colour of the two pixels
+        F2 cr2 = pk(0.f, 0.f), cg2 = cr2, cb2 = cr2;  // blended colour of the two pixels
         float t0 = 1.0f, t1 = 1.0f;                    // transmittance of the two pixels
 
         Staged n0 = null_splat(), n1 = null_splat();
@@ -295,7 +275,7 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
             for (int u = 0; u < GU; ++u) { A[u] = s_a[u]; B[u] = s_b[u]; }
             bool go = __any_sync(0xffffffffu, (t0 > MIN_ALPHA) || (t1 > MIN_ALPHA));
             for (int j = 0; j < chunkg && go; j += GU) {
-                u64 al2[GU], om2[GU];
+                F2 al2[GU], om2[GU];
                 phase_a<CONTRACT>(A, B, npx2, fpy, K, al2, om2);
                 float4 Bc[GU];
 #pragma unroll

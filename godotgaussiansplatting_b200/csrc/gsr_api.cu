@@ -48,7 +48,7 @@ struct gsr_ctx {
     // (back: FMA-pipe / chain bound) when the host enqueues frames back to back (gsr_render_async).  gsr_debug_pipeline(ctx, 0) = serial.
     cudaStream_t front_stream = nullptr;
     cudaEvent_t front_gate = nullptr;    // recorded after the tile ranges of the most recent frame (nullptr: nothing to wait for)
-    int overlap = -1;                    // -1 = default = off (measured: DESIGN.md section 6; on helps c3 on 4 GPUs by 10 %, not one GPU, and hurt c4's read-back leg)
+    int overlap = -1;                    // -1 = default = off (DESIGN.md section 6)
     SortWorkspace sort;
     FrameState *ring = nullptr;  // GSR_HISTORY_FRAMES slots; slot = frame_counter % GSR_HISTORY_FRAMES
     FrameState *frame = nullptr; // slot of the most recent frame
@@ -139,8 +139,8 @@ int check_device(int device) {
     }
     cudaDeviceProp prop;
     GSR_CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) {
-        set_last_error("device %d is sm_%d%d; libgsr is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        set_last_error("device %d is sm_%d%d; libgsr is built for sm_90a only", device, prop.major, prop.minor);
         return GSR_ERR_CUDA;
     }
     return GSR_OK;
@@ -197,7 +197,7 @@ GSR_API const char *gsr_error_string(int code) {
     switch (code) {
         case GSR_OK: return "ok";
         case GSR_ERR_INVALID: return "invalid argument";
-        case GSR_ERR_CUDA: return "CUDA failure or no usable sm_100 device (no CPU fallback exists)";
+        case GSR_ERR_CUDA: return "CUDA failure or no usable sm_90 device (no CPU fallback exists)";
         case GSR_ERR_OOM: return "device out of memory";
         case GSR_ERR_STATE: return "call order violated";
         case GSR_ERR_OVERFLOW: return "duplicate list exceeded capacity";
@@ -205,7 +205,7 @@ GSR_API const char *gsr_error_string(int code) {
     }
 }
 GSR_API const char *gsr_last_error(void) { return g_last_error; }
-GSR_API const char *gsr_version(void) { return "gsr 0.1.0 (sm_100a)"; }
+GSR_API const char *gsr_version(void) { return "gsr 0.1.0 (sm_90a)"; }
 GSR_API int gsr_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;
@@ -595,14 +595,14 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     const bool fast = c->row_mod > 1 && !gf;   // group mode is exact: the frame-global last tile travels with the pairs
     pa.band_y0 = c->band_y0; pa.band_y1 = c->band_y1;
     pa.row_mod = c->row_mod; pa.row_rem = c->row_rem;
-    // Conservative early reject + compaction of the survivors over 1024-splat CTAs (projection_sharded_kernel): exact, and
-    // measured on B200 (c3, one rank of G emulated): G=8 0.39 vs 0.46 ms, G=4 equal, G=2 slower (with two ranks nearly every
-    // splat's conservative extent touches both).  So: on by default from 6 ranks, or on request (GSR_FLAG_FAST_REJECT).
+    // Conservative early reject + compaction of the survivors over 1024-splat CTAs (projection_sharded_kernel): exact, but it only
+    // pays when a rank owns a small share of the rows (with two ranks nearly every splat's conservative extent touches both).
+    // So: on by default from 6 ranks, or on request (GSR_FLAG_FAST_REJECT).
     const bool want_reject = (c->flags & GSR_FLAG_FAST_REJECT) != 0 || c->row_mod >= 6;
     pa.fast_reject = (want_reject && fast) ? 1 : 0;
     pa.fast_mode = fast ? 1 : 0;
     // full frame: 12 of 32 lanes (below that, per-lane 128-bit gathers move fewer bytes); sharded: few lanes of a warp land in
-    // this rank's rows and the latency-bound gather path was measured slower than fetching the whole 6 KB slice (0.60 vs 0.46 ms)
+    // this rank's rows and the latency-bound gather path is slower than fetching the whole 6 KB slice
     pa.sh_bulk_min = (fast || c->row_mod > 1) ? 1 : 12;
     pa.records = records; pa.keys = keys_in; pa.values = vals_in; pa.capacity = (uint32_t)c->capacity;
     pa.lookback = c->lookback; pa.frame = c->frame;

@@ -939,8 +939,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     //      source and the largest tile this source touched (the frame-global Q10 bookkeeping travels with the data) ----
     // The CTA barrier orders every thread's stores before thread 0's fence (cumulativity), and the ticket is a device-scope
     // synchronisation between this CTA and the one that finishes last; only that last CTA talks to other GPUs, behind ONE
-    // system-scope fence.  (A system-scope fence in every CTA was measured to stretch the kernel by up to the duration of a frame
-    // read-back in flight: profiles/r02_group_e2e_probe.txt.)
+    // system-scope fence.  (A system-scope fence in every CTA can stall for up to the duration of a frame read-back in flight.)
     __syncthreads();
 #ifdef GSR_SCATTER_FENCE_PER_CTA_SYS
     if (tid == 0) __threadfence_system();

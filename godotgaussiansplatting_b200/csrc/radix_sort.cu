@@ -15,8 +15,8 @@
 // forward-progress guarantee.
 #include "common.cuh"
 
-// Digit matching inside a warp: 8 ballots (1) or match.any (0).  Measured on B200: ballots are ~20 % faster and
-// insensitive to digit skew (MATCH.ANY cost grows with the number of distinct digits in the warp).
+// Digit matching inside a warp: 8 ballots (1) or match.any (0).  Ballots cost the same for any digit skew; MATCH.ANY's cost
+// grows with the number of distinct digits in the warp.
 #ifndef GSR_SORT_BALLOT
 #define GSR_SORT_BALLOT 1
 #endif
@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) onesweep_kernel(const
 
         // ---- rank inside the warp: lanes with the same digit are matched, the lowest of them (the leader) bumps the
         //      warp-private counter.  The counter update is a RETURNING shared atomic whose result is not consumed
-        //      in this loop, so the 12 match + 12 atomic operations of a thread pipeline instead of forming a
+        //      in this loop, so the ITEMS match + ITEMS atomic operations of a thread pipeline instead of forming a
         //      load->add->store chain per row; __syncwarp() keeps row i's update ordered before row i+1's.
         uint32_t *wh = s_whist + warp * RADIX;
         const uint32_t lt_mask = (1u << lane) - 1u;
@@ -302,7 +302,7 @@ struct SweepConfig { int threads, items; };
 #define GSR_SORT_THREADS 512
 #endif
 #ifndef GSR_SORT_ITEMS
-#define GSR_SORT_ITEMS 12
+#define GSR_SORT_ITEMS 10  // sm_90a: 12 keys per thread spill the pairs kernel at the 64 registers two CTAs/SM allow
 #endif
 constexpr int SWEEP_THREADS = GSR_SORT_THREADS;
 constexpr int SWEEP_ITEMS = GSR_SORT_ITEMS;

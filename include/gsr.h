@@ -1,5 +1,5 @@
 /*
- * gsr.h -- C-ABI of libgsr.so: the B200-native (sm_100a) forward 3D-Gaussian-splatting rasterizer that
+ * gsr.h -- C-ABI of libgsr.so: the H100-native (sm_90a) forward 3D-Gaussian-splatting rasterizer that
  * replaces the body of 2Retr0/GodotGaussianSplatting's `GaussianSplattingRasterizer`
  * (util/gaussian_splatting_rasterizer.gd) plus the six compute shaders it dispatches
  * (the .glsl files of resources/shaders/compute) and the RenderingDevice wrapper (util/render_context.gd).
@@ -13,7 +13,7 @@
  * boundary, no torch/CUDA types in signatures (device pointers and streams travel as void*).
  * All calls on one handle must be serialised by the caller (the reference calls everything from the
  * render thread: main.gd:122,152,156).  There is NO CPU fallback: every entry point fails with
- * GSR_ERR_CUDA when no sm_100 device is usable.
+ * GSR_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef GSR_H_
 #define GSR_H_
@@ -262,9 +262,9 @@ GSR_API int gsr_debug_enable_trace(gsr_ctx *ctx, uint32_t max_items);
 GSR_API int gsr_debug_compositor_config(gsr_ctx *ctx, int32_t ctas_per_sm, int32_t longest_first, int32_t sparse_tiles_per_sm);
 /* Front / back overlap of consecutive frames (results never depend on it): 1 = a frame's clear + projection run on a second
  * stream, released when the previous frame's tile ranges are done, i.e. beside that frame's compositor; 0 or -1 (default) = every
- * kernel of a frame on the render stream, frames strictly one after the other.  Measured on B200 (DESIGN.md section 6): one GPU,
- * c3: neutral (the two kernels compete for the same issue slots); shard group of 4, c3: +10 % device-resident and end to end;
- * shard group of 4, c4: +10 % device-resident but -35 % with the rows-local read-back -- hence off by default. */
+ * kernel of a frame on the render stream, frames strictly one after the other.  Off by default: on one GPU the projection and
+ * the compositor compete for the same issue slots, and beside a rows-local read-back the overlap can slow a shard group down
+ * (DESIGN.md section 6). */
 GSR_API int gsr_debug_pipeline(gsr_ctx *ctx, int32_t overlap);
 /* Keep an unsorted copy of the emitted pairs each frame (costs 8*M bytes of traffic; off by default). */
 GSR_API int gsr_debug_keep_unsorted(gsr_ctx *ctx, int enable);

@@ -1,6 +1,6 @@
 """The C-ABI from C: include/gsr.h is a strict C99 / C++17 header, and examples/gsr_host.c -- a minimal C host that plays
-GaussianSplattingRasterizer.rasterize() for one frame -- links against libgsr.so, fails loudly without a GPU, and (on a
-B200) produces the oracle's frame."""
+GaussianSplattingRasterizer.rasterize() for one frame -- links against libgsr.so, fails loudly without a GPU, and (on an
+H100) produces the oracle's frame."""
 import os
 import shutil
 import struct

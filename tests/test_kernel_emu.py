@@ -3,7 +3,7 @@ against the oracle -- bit for bit.
 
 This is NOT a CPU path of the product (libgsr has none; see tests/test_abi.py): it is a pre-flight check of kernel LOGIC.
 the five kernel files of csrc/ are compiled by g++ under a thin shim of the CUDA execution model (threads = fibers,
-__syncthreads / warp collectives real, __shared__ = block-shared, packed f32x2 PTX = two IEEE binary32 operations), and one
+__syncthreads / warp collectives real, __shared__ = block-shared, __f*_rn intrinsics = one IEEE binary32 operation each), and one
 persistent block works through every tile: staging, blend, tile-stop vote, quantum, spill, re-queue, resume.
 It lets a kernel that has not seen a GPU yet prove its indexing and buffering before GPU minutes are spent.
 What it cannot show: memory-model behaviour (fences, races between blocks) and timing.
@@ -167,10 +167,10 @@ def test_band_fixup_kernel_blanks_only_the_owned_last_tile():
     assert (img == 1).all()
 
 
-@pytest.mark.parametrize("n", [1, 31, 100, 6143, 6144, 6145, 20000, 100000])
+@pytest.mark.parametrize("n", [1, 31, 100, 5119, 5120, 5121, 6143, 6144, 6145, 20000, 100000])
 @pytest.mark.parametrize("pairs", [True, False], ids=["pairs", "keys"])
 def test_onesweep_kernels_are_a_stable_sort(n, pairs):
-    """sort_hist_kernel + 4 x onesweep_kernel<512, 12>: tile = 6144 keys, ragged last tile, padding keys, look-back chain."""
+    """sort_hist_kernel + 4 x onesweep_kernel<512, 10>: tile = 5120 keys, ragged last tile, padding keys, look-back chain."""
     rng = np.random.default_rng(n)
     keys = rng.integers(0, 2**32, n, dtype=np.uint64).astype(np.uint32)
     if n > 1000:

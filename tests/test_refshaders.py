@@ -243,27 +243,6 @@ def test_render_fuzz():
     np.testing.assert_array_equal(bits(tex), bits(want))
 
 
-REF_PLY = "/root/reference/resources/demo.ply"
-
-
-@pytest.mark.skipif(not __import__("os").path.exists(REF_PLY), reason="reference tree not mounted (GPU box)")
-def test_reference_demo_asset_through_the_reference_shaders():
-    """The reference's own demo.ply, 640x480, default camera: every stage of the shaders == the oracle (271 123 splats,
-    M = 428 272, Q10 fires on tile 1198 -- SURVEY Appendix B)."""
-    from godotgaussiansplatting_b200 import camera as cam
-    from godotgaussiansplatting_b200.ply_file import PlyFile
-
-    ply = PlyFile(REF_PLY)
-    s = orc.preprocess_ply(ply.table, 0.0)
-    c = cam.default_camera(aspect=640 / 480)
-    vp = cam.pack_camera_push_constants(c.get_camera_transform(), c.get_camera_projection())
-    from tests.scenes import uniforms_bytes
-    ub = uniforms_bytes([0.0, 0.0, 0.0], 1.0, 640, 480, 10.0)
-    ref, spec = check_scene(s, vp, ub, 640, 480)
-    assert ref.duplicates == 428272 and spec.visible == 226063
-    assert ref.bounds[1198, 1] == 0          # Q10: the last occupied tile never gets its end
-
-
 def test_boundaries_uninitialised_shared_word():
     """Q20: invocation 0 of workgroup 0 returns before storing local[1]; invocation 1 reads it as its left neighbour."""
     splat60, vp, ub, w, h, heat = build("orbit_ragged_size")

@@ -1,6 +1,6 @@
 // cub_sort.cu -- CALIBRATION ONLY (never linked into libgsr): cub::DeviceRadixSort::SortPairs / SortKeys on the c5 key
 // distribution, timed with CUDA events, so that the hand-written Onesweep of csrc/radix_sort.cu can be read against what the
-// vendor library reaches on the same box.  Build: nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o ubench/cub_sort ubench/cub_sort.cu
+// vendor library reaches on the same box.  Build: nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o ubench/cub_sort ubench/cub_sort.cu
 #include <cub/cub.cuh>
 #include <cstdio>
 #include <cstdlib>

@@ -1,5 +1,5 @@
 import os, sys, time
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 from tests.gsr_direct import Ctx
 from tests.scenes import make_scene
