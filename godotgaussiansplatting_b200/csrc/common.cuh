@@ -244,6 +244,10 @@ struct CompositeArgs {
     ulonglong4 *trace;       // optional schedule trace (debug): {tile<<32|smid, t0_ns, t1_ns, consumed<<32|list_chunks<<1|1}
     uint32_t *trace_count;
     uint32_t trace_cap;
+    // depth compositing (gsr_set_depth_compositing); depth_out == nullptr: off, the reference's opaque frame
+    float view_z[4];           // V[2], V[6], V[10], V[14] of view_proj: the splat's view depth is -(((V2*x + V6*y) + V10*z) + V14)
+    const float *scene_depth;  // optional W*H linear scene depth; a pixel stops at the first splat not in front of it (nullptr: +inf)
+    float *depth_out;          // W*H: D / (1 - t) of the blended splats, +inf where nothing was blended
 };
 int launch_composite(const CompositeArgs &a, cudaStream_t stream);
 int composite_max_ctas_per_sm(int *out);

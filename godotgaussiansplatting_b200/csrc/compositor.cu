@@ -24,6 +24,11 @@
 // (CONTRACT = true, the default); CONTRACT = false (GSR_FLAG_UNCONTRACTED_BLEND) evaluates :84-90 with no contraction at all,
 // which is bit-identical to the reference's own shader text executed by oracle/glsl_cpu.  exp() is the det_exp() polynomial,
 // evaluated here for both pixels side by side.
+// Depth compositing (DEPTH = true, gsr_set_depth_compositing): the staged chunk also carries each splat's view depth
+// d = -view[2] (the projection's expression on the record's position), a pixel STOPS at the first splat with !(d < Z) for its
+// scene depth Z (nothing after it contributes, as if the pixel had died), the depth is accumulated like a fourth colour channel,
+// and the outputs are premultiplied rgb, alpha = 1 - t and depth = D / (1 - t) (+inf where nothing was blended).  DEPTH = false
+// is the reference's frame and compiles to the same code as before the mode existed.
 #include <stdlib.h>
 #include <string.h>
 
@@ -53,6 +58,7 @@ struct Staged {  // one gathered record, pre-scaled for the inner loop
     float4 a;    // image_pos.x, image_pos.y, -0.5*conic.x, -0.5*conic.z
     float4 b;    // -conic.y, opacity, color.r, color.g
     float c;     // color.b
+    float d;     // DEPTH only: view depth -(((V2*x + V6*y) + V10*z) + V14) of the record's position
 };
 
 __device__ __forceinline__ Staged null_splat() {
@@ -60,10 +66,13 @@ __device__ __forceinline__ Staged null_splat() {
     s.a = make_float4(0.f, 0.f, 0.f, 0.f);
     s.b = make_float4(0.f, 0.f, 0.f, 0.f);
     s.c = 0.f;
+    s.d = 0.f;   // padding of the last chunk: alpha 0, and a stop it may cause is never seen (the tile ends with that chunk)
     return s;
 }
 
-__device__ __forceinline__ Staged gather(const float4 *__restrict__ records, const uint32_t *__restrict__ values, uint32_t idx) {
+// vz = (V[2], V[6], V[10], V[14]): the view-matrix row of the depth (DEPTH only)
+template <bool DEPTH>
+__device__ __forceinline__ Staged gather(const float4 *__restrict__ records, const uint32_t *__restrict__ values, uint32_t idx, float4 vz) {
     const uint32_t v = __ldg(values + idx);
     const float4 *r = records + (uint64_t)v * 3u;
     const float4 r0 = __ldg(r + 0), r1 = __ldg(r + 1), r2 = __ldg(r + 2);
@@ -71,6 +80,7 @@ __device__ __forceinline__ Staged gather(const float4 *__restrict__ records, con
     s.a = make_float4(r0.x, r0.y, -0.5f * r1.x, -0.5f * r1.z);
     s.b = make_float4(-r1.y, r2.w, r2.x, r2.y);
     s.c = r2.z;
+    s.d = DEPTH ? -(((vz.x * r0.z + vz.y * r0.w) + vz.z * r1.w) + vz.w * 1.0f) : 0.f;   // == -view[2] of the projection
     return s;
 }
 
@@ -168,14 +178,27 @@ __device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], 
 
 // ---- phase B: the sequential part (gsplat_render.glsl:89-90).  A dead pixel has left the reference's loop: its colour and
 //      transmittance are kept by select.  `alive_mid` = "a pixel of this thread was alive after the first half of the group".
-template <bool CONTRACT>
-__device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, int j, const F2 al2[GU], const F2 om2[GU], F2 &cr2, F2 &cg2, F2 &cb2,
-                                        float &t0, float &t1, bool &alive_mid) {
+//      DEPTH: o0/o1 = "not stopped by the scene depth" (z0/z1); a live pixel stops at the first splat with !(d < z), before blending
+//      it; a stopped pixel is dead from then on.  dd2 accumulates d * alpha * t exactly like a colour channel.
+template <bool CONTRACT, bool DEPTH>
+__device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, const float *s_d, int j, const F2 al2[GU], const F2 om2[GU], F2 &cr2,
+                                        F2 &cg2, F2 &cb2, float &t0, float &t1, bool &alive_mid, float z0, float z1, bool &o0, bool &o1, F2 &dd2) {
 #pragma unroll
     for (int u = 0; u < GU; ++u) {
         const float cbl = s_c[j + u];
-        if (u == GU / 2) alive_mid = (t0 > MIN_ALPHA) || (t1 > MIN_ALPHA);
-        const bool a0 = t0 > MIN_ALPHA, a1 = t1 > MIN_ALPHA;
+        float dj = 0.f;
+        bool a0, a1;
+        if constexpr (DEPTH) {
+            dj = s_d[j + u];
+            if (u == GU / 2) alive_mid = (t0 > MIN_ALPHA && o0) || (t1 > MIN_ALPHA && o1);
+            a0 = t0 > MIN_ALPHA && o0; a1 = t1 > MIN_ALPHA && o1;
+            const bool v0 = dj < z0, v1 = dj < z1;   // false for NaN: stops
+            o0 = a0 ? v0 : o0; o1 = a1 ? v1 : o1;
+            a0 = a0 && v0; a1 = a1 && v1;
+        } else {
+            if (u == GU / 2) alive_mid = (t0 > MIN_ALPHA) || (t1 > MIN_ALPHA);
+            a0 = t0 > MIN_ALPHA; a1 = t1 > MIN_ALPHA;
+        }
         float al, ah, pl, ph;
         upk(al2[u], al, ah);
         const F2 t2 = pk(t0, t1);
@@ -185,10 +208,12 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, in
             cr2 = fma2(mul2(bc(B[u].z), m2), t2, cr2);
             cg2 = fma2(mul2(bc(B[u].w), m2), t2, cg2);
             cb2 = fma2(mul2(bc(cbl), m2), t2, cb2);
+            if constexpr (DEPTH) dd2 = fma2(mul2(bc(dj), m2), t2, dd2);
         } else {
             cr2 = mul_add2_unfused(mul2(bc(B[u].z), m2), t2, cr2);
             cg2 = mul_add2_unfused(mul2(bc(B[u].w), m2), t2, cg2);
             cb2 = mul_add2_unfused(mul2(bc(cbl), m2), t2, cb2);
+            if constexpr (DEPTH) dd2 = mul_add2_unfused(mul2(bc(dj), m2), t2, dd2);
         }
         t0 = a0 ? pl : t0;
         t1 = a1 ? ph : t1;
@@ -201,11 +226,12 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, in
 
 // Persistent CTAs.  Ticket k of the launch renders owned tile order[k] (longest chains first) or k itself; every tile is blended
 // from its first chunk to its stop by the CTA that took it.
-template <bool CONTRACT>
+template <bool CONTRACT, bool DEPTH = false>
 __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel(const __grid_constant__ CompositeArgs p) {
     __shared__ float4 s_a[CHUNK];
     __shared__ float4 s_b[CHUNK];
     __shared__ float s_c[CHUNK];
+    __shared__ float s_d[DEPTH ? CHUNK : 1];   // view depth of the staged splats
     __shared__ uint32_t s_vote[THREADS / 32];
     __shared__ uint32_t s_tile;
 
@@ -215,6 +241,7 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         if (limit && blockIdx.x >= limit) return;
     }
     const BlendK K = make_blend_k();
+    const float4 vz = DEPTH ? make_float4(p.view_z[0], p.view_z[1], p.view_z[2], p.view_z[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
     uint32_t staged = 0;  // SURVEY 8 symbol C, summed over the tiles this CTA processed (uniform across the CTA)
     unsigned long long t_start = 0;  // trace only
 
@@ -242,11 +269,19 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
 
         F2 cr2 = pk(0.f, 0.f), cg2 = cr2, cb2 = cr2;  // blended colour of the two pixels
         float t0 = 1.0f, t1 = 1.0f;                    // transmittance of the two pixels
+        bool o0 = true, o1 = true;                     // DEPTH: not stopped by the scene depth
+        F2 dd2 = pk(0.f, 0.f);                         // DEPTH: accumulated depth
+        float z0 = __uint_as_float(0x7f800000u), z1 = z0; // DEPTH: scene depth (+inf: nothing occludes; also outside the image)
+        if (DEPTH && p.scene_depth && py < p.height) {
+            const float *zrow = p.scene_depth + (uint64_t)py * (uint64_t)p.width;
+            if (px0 < p.width) z0 = zrow[px0];
+            if (px0 + 1 < p.width) z1 = zrow[px0 + 1];
+        }
 
         Staged n0 = null_splat(), n1 = null_splat();
         if (num_iterations > 0) {
-            if ((int)tid < num_splats) n0 = gather(p.records, p.values, bounds.x + tid);
-            if ((int)tid + THREADS < num_splats) n1 = gather(p.records, p.values, bounds.x + tid + THREADS);
+            if ((int)tid < num_splats) n0 = gather<DEPTH>(p.records, p.values, bounds.x + tid, vz);
+            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH>(p.records, p.values, bounds.x + tid + THREADS, vz);
         }
 
         int consumed = 0;  // chunks blended before the stop rule fired (next frame's scheduling hint)
@@ -257,13 +292,14 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
             consumed = i + 1;
             s_a[tid] = n0.a; s_b[tid] = n0.b; s_c[tid] = n0.c;
             s_a[tid + THREADS] = n1.a; s_b[tid + THREADS] = n1.b; s_c[tid + THREADS] = n1.c;
+            if constexpr (DEPTH) { s_d[tid] = n0.d; s_d[tid + THREADS] = n1.d; }
             __syncthreads();
             // prefetch the next chunk's records while this one is blended (slots past the list end become null splats)
             n0 = null_splat(); n1 = null_splat();
             if (i + 1 < num_iterations) {
                 const int nb = sort_offset + CHUNK;
-                if (nb + (int)tid < num_splats) n0 = gather(p.records, p.values, bounds.x + (uint32_t)nb + tid);
-                if (nb + (int)tid + THREADS < num_splats) n1 = gather(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS);
+                if (nb + (int)tid < num_splats) n0 = gather<DEPTH>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz);
+                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz);
             }
 
             // :79-91, GU splats per iteration; `chunk` rounded up to GU reads null splats (opacity 0 => exact no-op).  Software-pipelined:
@@ -273,7 +309,9 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
             float4 A[GU], B[GU];
 #pragma unroll
             for (int u = 0; u < GU; ++u) { A[u] = s_a[u]; B[u] = s_b[u]; }
-            bool go = __any_sync(0xffffffffu, (t0 > MIN_ALPHA) || (t1 > MIN_ALPHA));
+            bool go;
+            if constexpr (DEPTH) go = __any_sync(0xffffffffu, (t0 > MIN_ALPHA && o0) || (t1 > MIN_ALPHA && o1));
+            else go = __any_sync(0xffffffffu, (t0 > MIN_ALPHA) || (t1 > MIN_ALPHA));
             for (int j = 0; j < chunkg && go; j += GU) {
                 F2 al2[GU], om2[GU];
                 phase_a<CONTRACT>(A, B, npx2, fpy, K, al2, om2);
@@ -284,12 +322,14 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
 #pragma unroll
                 for (int u = 0; u < GU; ++u) { A[u] = s_a[jn + u]; B[u] = s_b[jn + u]; }
                 bool alive_mid = true;
-                phase_b<CONTRACT>(Bc, s_c, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid);
+                phase_b<CONTRACT, DEPTH>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2);
                 go = __any_sync(0xffffffffu, alive_mid);
             }
 
-            // :97 tile-stop vote: continue only if the sum over the tile's 256 pixels of uint(t*255) exceeds 255
-            const uint32_t wsum = __reduce_add_sync(0xffffffffu, (uint32_t)(t0 * 255.0f) + (uint32_t)(t1 * 255.0f));
+            // :97 tile-stop vote: continue only if the sum over the tile's 256 pixels of uint(t*255) exceeds 255 (a stopped pixel adds 0)
+            uint32_t wsum;
+            if constexpr (DEPTH) wsum = __reduce_add_sync(0xffffffffu, (o0 ? (uint32_t)(t0 * 255.0f) : 0u) + (o1 ? (uint32_t)(t1 * 255.0f) : 0u));
+            else wsum = __reduce_add_sync(0xffffffffu, (uint32_t)(t0 * 255.0f) + (uint32_t)(t1 * 255.0f));
             if (lane == 0) s_vote[warp] = wsum;
             __syncthreads();
             uint32_t shared_t = 0;
@@ -306,10 +346,19 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         if (py < p.height) {
             float4 *row = p.out + (uint64_t)py * (uint64_t)p.width;
             const float k0 = 1.0f - t0, k1 = 1.0f - t1;
+            const float al0 = DEPTH ? k0 : 1.0f, al1 = DEPTH ? k1 : 1.0f;   // DEPTH: coverage; colour is premultiplied by construction
             if (px0 < p.width)
-                row[px0] = make_float4(r0 + h0 * k0 * p.heatmap_factor, g0 + h1 * k0 * p.heatmap_factor, b0 + h2c * k0 * p.heatmap_factor, 1.0f);
+                row[px0] = make_float4(r0 + h0 * k0 * p.heatmap_factor, g0 + h1 * k0 * p.heatmap_factor, b0 + h2c * k0 * p.heatmap_factor, al0);
             if (px0 + 1 < p.width)
-                row[px0 + 1] = make_float4(r1 + h0 * k1 * p.heatmap_factor, g1 + h1 * k1 * p.heatmap_factor, b1 + h2c * k1 * p.heatmap_factor, 1.0f);
+                row[px0 + 1] = make_float4(r1 + h0 * k1 * p.heatmap_factor, g1 + h1 * k1 * p.heatmap_factor, b1 + h2c * k1 * p.heatmap_factor, al1);
+            if (DEPTH) {
+                float d0, d1;
+                upk(dd2, d0, d1);
+                const float inf = __uint_as_float(0x7f800000u);
+                float *drow = p.depth_out + (uint64_t)py * (uint64_t)p.width;
+                if (px0 < p.width) drow[px0] = k0 > 0.0f ? __fdiv_rn(d0, k0) : inf;
+                if (px0 + 1 < p.width) drow[px0 + 1] = k1 > 0.0f ? __fdiv_rn(d1, k1) : inf;
+            }
         }
         // :105-110 pick: the elected (first) lane of each 32-wide subgroup of the reference's 16x16 workgroup is local
         // index 32*s = pixel (0, 2*s) of the tile = first pixel of thread 16*s here
@@ -338,13 +387,19 @@ int preload_composite_kernels() {
     cudaFuncAttributes fa;
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<true, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false, true>));
     return GSR_OK;
 }
 
 int composite_max_ctas_per_sm(int *out) {
-    int a = 0, b = 0;
+    int a = 0, b = 0, c = 0, d = 0;
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, composite_kernel<true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, composite_kernel<false>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, composite_kernel<true, true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d, composite_kernel<false, true>, THREADS, 0));
+    if (c < a) a = c;
+    if (d < b) b = d;
     *out = a < b ? a : b;
     if (*out < 1) *out = 1;
     return GSR_OK;
@@ -354,8 +409,14 @@ int launch_composite(const CompositeArgs &a, cudaStream_t stream) {
     if (a.num_tiles <= 0) return GSR_OK;
     const int per_sm = a.ctas_per_sm > 0 ? a.ctas_per_sm : 1;
     const int grid = a.num_tiles < a.sm_count * per_sm ? a.num_tiles : a.sm_count * per_sm;
-    if (a.contract) composite_kernel<true><<<grid, THREADS, 0, stream>>>(a);
-    else composite_kernel<false><<<grid, THREADS, 0, stream>>>(a);
+    if (a.depth_out) {   // depth compositing (gsr_set_depth_compositing)
+        if (a.contract) composite_kernel<true, true><<<grid, THREADS, 0, stream>>>(a);
+        else composite_kernel<false, true><<<grid, THREADS, 0, stream>>>(a);
+    } else if (a.contract) {
+        composite_kernel<true><<<grid, THREADS, 0, stream>>>(a);
+    } else {
+        composite_kernel<false><<<grid, THREADS, 0, stream>>>(a);
+    }
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }

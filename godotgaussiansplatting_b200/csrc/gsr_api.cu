@@ -64,6 +64,10 @@ struct gsr_ctx {
     uint32_t *trace_count = nullptr;
     uint32_t trace_cap = 0;
     float4 *fb = nullptr, *fb_ext = nullptr;
+    // depth compositing (gsr_set_depth_compositing): caller-owned W*H float planes; depth_out == nullptr = off
+    const float *scene_depth = nullptr;
+    float *depth_out = nullptr;
+    float4 *pick_strip = nullptr;   // 16 pixel rows: where gsr_pick's default-path re-dispatch writes while depth compositing is on
     float4 *fb2 = nullptr;                       // second frame for pipelined read-back (gsr_render_async)
     void *stage[2] = {nullptr, nullptr};         // converted copies of the two frames (GSR_OUT_* other than RGBA32F), lazily allocated (16 B/pixel)
     float4 *fb_last = nullptr;                   // frame written by the most recent render
@@ -169,7 +173,7 @@ void free_ctx(gsr_ctx *c) {
     if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
     if (c->peer_opened) { cudaIpcCloseMemHandle(c->peer_fb[0]); cudaIpcCloseMemHandle(c->peer_fb[1]); }
     cudaFree(c->stage[0]); cudaFree(c->stage[1]);
-    cudaFree(c->ring); cudaFree(c->lookback); cudaFree(c->bounds); cudaFree(c->comp_order); cudaFree(c->comp_hint); cudaFree(c->pick_frame); cudaFree(c->fb); cudaFree(c->fb2); cudaFree(c->pick); cudaFree(c->staging);
+    cudaFree(c->ring); cudaFree(c->lookback); cudaFree(c->bounds); cudaFree(c->comp_order); cudaFree(c->comp_hint); cudaFree(c->pick_frame); cudaFree(c->fb); cudaFree(c->fb2); cudaFree(c->pick); cudaFree(c->staging); cudaFree(c->pick_strip);
     for (int i = 0; i < 2; ++i) { if (c->ev_done[i]) cudaEventDestroy(c->ev_done[i]); if (c->ev_copied[i]) cudaEventDestroy(c->ev_copied[i]); }
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     cudaFree(c->sync_word);
@@ -392,6 +396,8 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
     if (c->peer_opened) { cudaIpcCloseMemHandle(c->peer_fb[0]); cudaIpcCloseMemHandle(c->peer_fb[1]); c->peer_opened = false; }
     c->peer_mode = false; c->peer_fb[0] = c->peer_fb[1] = nullptr; c->peer_counter = 0; c->async_counter = 0;
     group_detach(c);   // same for a shard group: every rank resizes, exports and attaches again
+    c->scene_depth = nullptr; c->depth_out = nullptr;   // the caller's depth planes have the old size: depth compositing is off
+    cudaFree(c->pick_strip); c->pick_strip = nullptr;
     GSR_CUDA_TRY(cudaMalloc((void **)&c->bounds, sizeof(uint2) * (size_t)tx * ty));
     GSR_CUDA_TRY(cudaMalloc((void **)&c->comp_order, sizeof(uint32_t) * (size_t)tx * ty));
     GSR_CUDA_TRY(cudaMalloc((void **)&c->comp_hint, sizeof(uint32_t) * (size_t)tx * ty));
@@ -411,6 +417,7 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
 
 GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod) {
     if (!c || row_mod < 1 || row_rem < 0 || row_rem >= row_mod) { set_last_error("gsr_set_row_interleave: need 0 <= rem < mod"); return GSR_ERR_INVALID; }
+    if (c->depth_out && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -430,6 +437,7 @@ GSR_API int gsr_band_fixup(gsr_ctx *c) {
 GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (!c || c->tiles_y == 0) { set_last_error("gsr_set_band before gsr_resize"); return GSR_ERR_STATE; }
     if (row_begin < 0 || row_end > c->tiles_y || row_begin > row_end) { set_last_error("band [%d,%d) outside [0,%d]", row_begin, row_end, c->tiles_y); return GSR_ERR_INVALID; }
+    if (c->depth_out && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
     c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
     return GSR_OK;
@@ -706,6 +714,8 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         launches += 1;
     }
     ca.trace = c->trace; ca.trace_count = c->trace_count; ca.trace_cap = c->trace_cap;
+    ca.view_z[0] = view_proj[2]; ca.view_z[1] = view_proj[6]; ca.view_z[2] = view_proj[10]; ca.view_z[3] = view_proj[14];
+    ca.scene_depth = c->scene_depth; ca.depth_out = c->depth_out;
     if (c->trace) GSR_CUDA_TRY(cudaMemsetAsync(c->trace_count, 0, sizeof(uint32_t), s));
     if (gf && !gf->rows_local && c->grp.rank != 0 && gf->seq >= 3u) {   // the presenting rank must have consumed the frame that used this slot
         if ((rc = launch_group_wait_released(c->grp.flags[c->grp.rank], gf->seq - 2u, s))) return rc;
@@ -908,6 +918,7 @@ GSR_API int gsr_readback_rows_async(gsr_ctx *c, void *host_frame) {
 
 GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
+    if (c->depth_out) { set_last_error("gsr_peer_export_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -922,6 +933,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
 
 GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
+    if (c->depth_out) { set_last_error("gsr_peer_import_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -979,6 +991,7 @@ GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
 GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void *blobs) {
     if (!c || !blobs || world < 1 || world > GROUP_MAX || rank < 0 || rank >= world) { set_last_error("gsr_group_attach: need 0 <= rank < world <= %d", GROUP_MAX); return GSR_ERR_INVALID; }
     if (!c->grp.arena || !c->fb) { set_last_error("gsr_group_attach before gsr_group_export"); return GSR_ERR_STATE; }
+    if (c->depth_out && world > 1) { set_last_error("gsr_group_attach: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1082,6 +1095,22 @@ GSR_API int gsr_set_framebuffer_external(gsr_ctx *c, void *device_ptr) {
     return GSR_OK;
 }
 
+GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_device, float *depth_out_device) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!depth_out_device) {
+        if (scene_depth_device) { set_last_error("gsr_set_depth_compositing: a scene depth needs a depth output"); return GSR_ERR_INVALID; }
+        c->scene_depth = nullptr; c->depth_out = nullptr;
+        return GSR_OK;
+    }
+    if (c->width == 0) { set_last_error("gsr_set_depth_compositing before gsr_resize"); return GSR_ERR_STATE; }
+    if (c->grp.world > 1 || c->peer_mode || c->row_mod > 1 || !(c->band_y0 == 0 && c->band_y1 == c->tiles_y)) {
+        set_last_error("gsr_set_depth_compositing: single-context only (no group, peer framebuffers, partial band or row interleave)");
+        return GSR_ERR_STATE;
+    }
+    c->scene_depth = scene_depth_device; c->depth_out = depth_out_device;
+    return GSR_OK;
+}
+
 GSR_API int gsr_pick(gsr_ctx *c, uint32_t tile_id, float heatmap_factor, float out_xyzn[4]) {
     if (!c || !out_xyzn) return GSR_ERR_INVALID;
     if (c->width == 0) { set_last_error("gsr_pick before gsr_resize"); return GSR_ERR_STATE; }
@@ -1100,6 +1129,14 @@ GSR_API int gsr_pick(gsr_ctx *c, uint32_t tile_id, float heatmap_factor, float o
         ca.order = nullptr; ca.consumed = nullptr; ca.ctas_per_sm = 1; ca.sm_count = c->sm_count;
         ca.contract = (c->flags & GSR_FLAG_UNCONTRACTED_BLEND) ? 0 : 1;
         ca.trace = nullptr; ca.trace_count = nullptr; ca.trace_cap = 0;
+        ca.view_z[0] = ca.view_z[1] = ca.view_z[2] = ca.view_z[3] = 0.0f;
+        ca.scene_depth = nullptr; ca.depth_out = nullptr;   // the pick re-dispatch is always the default compositor
+        if (c->depth_out) {
+            // ... whose opaque pixels must not replace the depth-composited tile: they go to a 16-row strip instead (the kernel
+            // stores pixel (x, y) at out[y * width + x], y in the tile's 16 rows)
+            if (!c->pick_strip) GSR_CUDA_TRY(cudaMalloc((void **)&c->pick_strip, sizeof(float4) * (size_t)TILE * c->width));
+            ca.out = c->pick_strip - (size_t)(tile_id / (uint32_t)c->tiles_x) * TILE * (size_t)c->width;
+        }
         for (int i = 0; i < 2; ++i)   // the re-dispatch rewrites the tile's pixels: not under a read-back in flight
             if (c->copied_valid[i]) GSR_CUDA_TRY(cudaStreamWaitEvent(c->stream, c->ev_copied[i], 0));
         GSR_CUDA_TRY(cudaMemsetAsync(c->pick_frame, 0, sizeof(FrameState), c->stream));

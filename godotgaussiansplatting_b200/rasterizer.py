@@ -152,6 +152,13 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_set_framebuffer_external(self._ctx, C.c_void_p(device_ptr)), "gsr_set_framebuffer_external")
         self._bind_texture()
 
+    def set_depth_compositing(self, scene_depth_ptr: int | None, depth_out_ptr: int | None) -> None:
+        """Composite into the host's 3D scene (include/gsr.h gsr_set_depth_compositing): depth_out_ptr = device float[h*w] that receives
+        the splats' linear view depth (None switches the mode off), scene_depth_ptr = optional device float[h*w] linear scene depth
+        that hides the splats behind it.  The frame's alpha becomes the coverage."""
+        _lib.check(_lib.lib().gsr_set_depth_compositing(self._ctx, C.c_void_p(scene_depth_ptr or None), C.c_void_p(depth_out_ptr or None)),
+                   "gsr_set_depth_compositing")
+
     def render_raw(self, vp32: np.ndarray, uniforms32: bytes, heatmap: float = 0.0, host_ptr: int | None = None,
                    asynchronous: bool = True, rgb_only: bool = False, out_format: int | None = None) -> None:
         """rasterize() with pre-packed push constants / uniform block (bench hot loop).  out_format: GSR_OUT_* of the host frame

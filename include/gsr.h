@@ -238,6 +238,24 @@ GSR_API void *gsr_framebuffer_device_ptr(gsr_ctx *ctx);
 /* Render into caller-owned device memory instead (>= width*height*16 bytes; NULL restores the internal one). */
 GSR_API int gsr_set_framebuffer_external(gsr_ctx *ctx, void *device_ptr);
 
+/* ---- Depth compositing: splats composited into the host's 3D scene (no reference counterpart: the reference shows an opaque
+ *      frame on a full-screen quad).  Both pointers are caller-owned device float[width*height], row-major like the frame.
+ *      depth_out_device != NULL switches the mode on, NULL switches it off (scene_depth_device must then be NULL too).
+ *      scene_depth_device (optional, NULL = nothing occludes) holds the scene's LINEAR view depth per pixel: the distance along
+ *      the camera's viewing axis, positive in front of the camera (Godot: -(VIEW_MATRIX * world position).z), in the world units
+ *      of view_proj; +inf = nothing.  Per pixel, in the tile's sorted order, the compositor stops before the first splat whose
+ *      view depth d = -(view_matrix * splat position).z is not in front of the scene depth (!(d < Z), NaN included): that splat and
+ *      every later one contribute nothing.  The frame then carries:
+ *        rgb   = the same blend as the default frame (bit-identical to it without a scene depth), i.e. premultiplied colour;
+ *        alpha = 1 - t, the splats' coverage (the default frame's alpha is the constant 1.0);
+ *      and depth_out the coverage-weighted linear view depth of the blended splats, +inf where nothing was blended.
+ *      depth_out is written by every frame's compositor on the render stream; the caller orders its reads like those of an
+ *      external framebuffer.  GSR_OUT_RGB32F drops the coverage; GSR_OUT_SRGB_TO_LINEAR converts the premultiplied values as
+ *      they are.  Single-context only: GSR_ERR_STATE on a context with an attached group, peer framebuffers, a partial band
+ *      or row_mod > 1, and those calls fail with GSR_ERR_STATE while the mode is on.  gsr_resize switches the mode off;
+ *      gsr_pick keeps the default path (and leaves the depth-composited frame as it is).  GSR_ERR_STATE before gsr_resize. ---- */
+GSR_API int gsr_set_depth_compositing(gsr_ctx *ctx, const float *scene_depth_device, float *depth_out_device);
+
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
  *      num_tile_splats -- persistent across calls exactly like the reference's storage buffer.
