@@ -158,6 +158,28 @@ struct ProjectionArgs {
 int launch_projection(const ProjectionArgs &a, cudaStream_t stream);
 
 // ---------------------------------------------------------------------------------------------
+// splat instances (gsr_set_instances): ranges of the splat buffer drawn with their own affine transform into frame space
+// ---------------------------------------------------------------------------------------------
+// Per instance and frame (instance_prepare_kernel): V_k = V * [A|t] (16), cam_k = B * camera_pos + u (3), A (9), t (3), pad.
+constexpr int INSTANCE_FRAME_FLOATS = 32;
+constexpr int INSTANCE_XFORM_FLOATS = 24;   // what the host hands the prepare kernel per instance: A|t as given, then B|u = its inverse
+struct InstanceDesc {                       // static per layout
+    uint64_t first;                         // first source splat
+    uint32_t count;                         // source splats
+    uint32_t warp0;                         // first drawn warp: drawn ids [32 warp0, 32 warp0 + count)
+};
+struct InstanceArgs {
+    const float *frame;                     // INSTANCE_FRAME_FLOATS per instance: this frame's constants
+    const InstanceDesc *desc;
+    const uint32_t *warp_inst;              // instance of every drawn warp of the grid; 0xFFFFFFFF = padding warp
+};
+// a.num_splats = D (drawn ids), a.records indexed by drawn id
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream);
+// one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
+// (mapped page-locked host memory on the frame path)
+int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream);
+
+// ---------------------------------------------------------------------------------------------
 // multi-GPU shard group (group.cu, gsr_group_attach): flag words + receive segments + record tables in every rank's arena
 // ---------------------------------------------------------------------------------------------
 constexpr int GROUP_MAX = 16;                                   // ranks per group (one NVSwitch domain)

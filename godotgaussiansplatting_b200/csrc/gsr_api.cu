@@ -4,6 +4,7 @@
 // cleanup_gpu (util/gaussian_splatting_rasterizer.gd:65-171) and of RenderingContext
 // (util/render_context.gd).  Fifteen compute dispatches with full barriers per frame in the reference
 // become 1 + 5 + 1 + 1 kernel launches on one CUDA stream, with no host synchronisation on the frame path.
+#include <math.h>
 #include <stdarg.h>
 #include <stdlib.h>
 #include <stddef.h>
@@ -114,6 +115,25 @@ struct gsr_ctx {
     bool ev_valid = false;
     uint32_t last_launches = 0;
     int sm_count = 0;
+    uint64_t dup_factor = 10;
+    uint64_t rec_entries = 0;    // ids each record table holds: max(max_splats, D of the largest instance layout so far)
+    uint32_t lookback_cap = 0;   // projection links the look-back words cover (scatter links come on top)
+    // splat instances (gsr_set_instances); inst_n == 0: off
+    struct Instances {
+        uint32_t n = 0;                  // instances of the current layout
+        uint64_t drawn = 0;              // D
+        uint64_t *range = nullptr;       // [2n] first, count (the layout)
+        float *xf = nullptr;             // [24n] A|t as given, B|u = the inverse (host copy; GSR_BUF_INSTANCES)
+        InstanceDesc *desc = nullptr;    // device [n]
+        uint32_t *warps = nullptr;       // device: instance of every drawn warp of the projection grid
+        float *frame = nullptr;          // device [2][n][INSTANCE_FRAME_FLOATS]: this frame's constants, by frame parity
+        uint32_t cap = 0;                // instances the device tables and the ring are sized for
+        float *ring = nullptr;           // mapped page-locked [GSR_INSTANCE_RING][cap][24]: the transforms of one frame per slot
+        float *ring_dev = nullptr;
+        cudaEvent_t ev[GSR_INSTANCE_RING] = {};   // recorded after the prepare kernel that read the slot
+        bool ev_used[GSR_INSTANCE_RING] = {};
+        uint64_t seq = 0;                // instanced frames enqueued
+    } inst;
 };
 
 struct gsr_sorter {
@@ -180,6 +200,10 @@ void free_ctx(gsr_ctx *c) {
     for (int i = 0; i < c->grp.n_opened; ++i) cudaIpcCloseMemHandle(c->grp.opened[i]);
     cudaFree(c->grp.arena);
     cudaFree(c->unsorted_keys); cudaFree(c->unsorted_vals); cudaFree(c->trace); cudaFree(c->trace_count);
+    cudaFree(c->inst.desc); cudaFree(c->inst.warps); cudaFree(c->inst.frame);
+    if (c->inst.ring) cudaFreeHost(c->inst.ring);
+    for (int i = 0; i < GSR_INSTANCE_RING; ++i) if (c->inst.ev[i]) cudaEventDestroy(c->inst.ev[i]);
+    delete[] c->inst.range; delete[] c->inst.xf;
     if (c->ev) {
         for (int i = 0; i < GSR_HISTORY_FRAMES * EV_PER_FRAME; ++i) if (c->ev[i]) cudaEventDestroy(c->ev[i]);
         delete[] c->ev;
@@ -230,6 +254,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     if (!(c->flags & (GSR_FLAG_REFERENCE_QUIRKS | GSR_FLAG_FIXED_RANGES))) c->flags |= GSR_FLAG_REFERENCE_QUIRKS;
     c->max_splats = cfg->max_splats;
     const uint64_t factor = cfg->dup_capacity_factor ? cfg->dup_capacity_factor : 10;  // rasterizer.gd:79
+    c->dup_factor = factor;
     c->capacity_max = (1ull << 30) - 1;  // look-back words carry 30-bit counts
     c->capacity = c->max_splats * factor;
     if (c->capacity > c->capacity_max) c->capacity = c->capacity_max;
@@ -273,7 +298,9 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     TRY_ALLOC(c->keys, sizeof(uint32_t) * 3ull * c->cap_stride);
     TRY_ALLOC(c->vals, sizeof(uint32_t) * 3ull * c->cap_stride);
     c->keys_cur = c->keys; c->vals_cur = c->vals; c->records_cur = c->records;
+    c->rec_entries = c->max_splats;
     c->lookback_blocks = projection_num_blocks((uint32_t)c->max_splats);  // one scan link per CTA
+    c->lookback_cap = c->lookback_blocks;
     TRY_ALLOC(c->ring, sizeof(FrameState) * GSR_HISTORY_FRAMES);
     TRY_ALLOC(c->lookback, sizeof(unsigned long long) * ((size_t)c->lookback_blocks + 2u * GROUP_MAX * GROUP_MAX));  // scatter mode: (N/G/256 + 1) x G links
     c->frame = c->ring;
@@ -418,6 +445,7 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
 GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod) {
     if (!c || row_mod < 1 || row_rem < 0 || row_rem >= row_mod) { set_last_error("gsr_set_row_interleave: need 0 <= rem < mod"); return GSR_ERR_INVALID; }
     if (c->depth_out && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (c->inst.n && row_mod > 1) { set_last_error("gsr_set_row_interleave: instances are set (single-context only)"); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -438,6 +466,7 @@ GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (!c || c->tiles_y == 0) { set_last_error("gsr_set_band before gsr_resize"); return GSR_ERR_STATE; }
     if (row_begin < 0 || row_end > c->tiles_y || row_begin > row_end) { set_last_error("band [%d,%d) outside [0,%d]", row_begin, row_end, c->tiles_y); return GSR_ERR_INVALID; }
     if (c->depth_out && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (c->inst.n && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: instances are set (single-context only)"); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
     c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
     return GSR_OK;
@@ -579,8 +608,9 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
 
     // ---- front: rasterizer.gd:127-128 (clear M = this frame's history slot + the scan links), then the projection ----
     if (overlap && c->front_gate) GSR_CUDA_TRY(cudaStreamWaitEvent(fs, c->front_gate, 0));
+    const bool inst = c->inst.n > 0 && !gf;   // (a context with instances cannot attach a group)
     {
-        uint32_t links = projection_num_blocks((uint32_t)c->max_splats);
+        uint32_t links = projection_num_blocks((uint32_t)(inst ? c->inst.drawn : c->max_splats));
         if (gf) {
             const uint64_t first = (uint64_t)c->grp.rank * c->grp.slice;
             const uint64_t count = first < c->max_splats ? ((c->max_splats - first) < c->grp.slice ? (c->max_splats - first) : c->grp.slice) : 0;
@@ -592,11 +622,28 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         launches += 1;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[0], fs));  // 'Start'
+    if (inst) {
+        // this frame's transforms -> a slot of the mapped ring (no copy engine, no host sync while the host is fewer than
+        // GSR_INSTANCE_RING frames ahead), then one small kernel composes every instance's V_k / cam_k into this parity's table
+        const uint32_t rs = (uint32_t)(c->inst.seq % GSR_INSTANCE_RING);
+        if (c->inst.ev_used[rs] && cudaEventQuery(c->inst.ev[rs]) != cudaSuccess) {
+            cudaGetLastError();
+            GSR_CUDA_TRY(cudaEventSynchronize(c->inst.ev[rs]));
+        }
+        const size_t per = (size_t)c->inst.cap * INSTANCE_XFORM_FLOATS;
+        memcpy(c->inst.ring + rs * per, c->inst.xf, sizeof(float) * INSTANCE_XFORM_FLOATS * c->inst.n);
+        if ((rc = launch_instance_prepare(c->inst.ring_dev + rs * per, view_proj, u.camera_pos, c->inst.n,
+                                          c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS, fs))) return rc;
+        GSR_CUDA_TRY(cudaEventRecord(c->inst.ev[rs], fs));
+        c->inst.ev_used[rs] = true;
+        c->inst.seq += 1;
+        launches += 1;
+    }
 
     ProjectionArgs pa;
     // the reference dispatches over splat_buffer.length() = point_cloud.size every frame (rasterizer.gd:83,134), i.e. also over the
     // zero-initialised structs of splats the loader has not delivered yet: so does libgsr (the SoA planes start zeroed)
-    pa.soa = c->soa; pa.plane_stride = c->plane_stride; pa.num_splats = (uint32_t)c->max_splats;
+    pa.soa = c->soa; pa.plane_stride = c->plane_stride; pa.num_splats = (uint32_t)(inst ? c->inst.drawn : c->max_splats);
     memcpy(pa.vp, view_proj, sizeof pa.vp);
     pa.u = u;
     frame_constants(view_proj, u, pa);
@@ -636,6 +683,12 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         sp.lookback = c->lookback;
         if ((rc = launch_projection_scatter(pa, sp, fs))) return rc;
         launches += 1;
+    } else if (inst) {
+        InstanceArgs ia;
+        ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
+        ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
+        if ((rc = launch_projection_instanced(pa, ia, fs))) return rc;
+        launches += pa.num_splats ? 1 : 0;
     } else {
         if ((rc = launch_projection(pa, fs))) return rc;
         launches += pa.num_splats ? 1 : 0;
@@ -919,6 +972,7 @@ GSR_API int gsr_readback_rows_async(gsr_ctx *c, void *host_frame) {
 GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
     if (c->depth_out) { set_last_error("gsr_peer_export_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (c->inst.n) { set_last_error("gsr_peer_export_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -934,6 +988,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
 GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
     if (c->depth_out) { set_last_error("gsr_peer_import_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (c->inst.n) { set_last_error("gsr_peer_import_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -992,6 +1047,7 @@ GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void
     if (!c || !blobs || world < 1 || world > GROUP_MAX || rank < 0 || rank >= world) { set_last_error("gsr_group_attach: need 0 <= rank < world <= %d", GROUP_MAX); return GSR_ERR_INVALID; }
     if (!c->grp.arena || !c->fb) { set_last_error("gsr_group_attach before gsr_group_export"); return GSR_ERR_STATE; }
     if (c->depth_out && world > 1) { set_last_error("gsr_group_attach: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (c->inst.n && world > 1) { set_last_error("gsr_group_attach: instances are set (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1108,6 +1164,149 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_devic
         return GSR_ERR_STATE;
     }
     c->scene_depth = scene_depth_device; c->depth_out = depth_out_device;
+    return GSR_OK;
+}
+
+// [A | t] -> [A | t, B | u] with B = A^-1, u = -A^-1 t in double precision, rounded to float.  False: non-finite or singular.
+static bool instance_inverse(const float m[12], float out[24]) {
+    double A[3][3], t[3];   // A[c][r]
+    for (int e = 0; e < 12; ++e) if (!isfinite(m[e])) return false;
+    for (int c = 0; c < 3; ++c) for (int r = 0; r < 3; ++r) A[c][r] = m[3 * c + r];
+    for (int r = 0; r < 3; ++r) t[r] = m[9 + r];
+    auto a = [&](int r, int col) { return A[col][r]; };   // row r, column col
+    const double c00 = a(1, 1) * a(2, 2) - a(1, 2) * a(2, 1), c01 = a(1, 2) * a(2, 0) - a(1, 0) * a(2, 2), c02 = a(1, 0) * a(2, 1) - a(1, 1) * a(2, 0);
+    const double det = a(0, 0) * c00 + a(0, 1) * c01 + a(0, 2) * c02;
+    if (!(det != 0.0) || !isfinite(det)) return false;
+    double inv[3][3];   // inv[r][col] = (A^-1) row r, column col = adj / det
+    inv[0][0] = c00 / det; inv[0][1] = (a(0, 2) * a(2, 1) - a(0, 1) * a(2, 2)) / det; inv[0][2] = (a(0, 1) * a(1, 2) - a(0, 2) * a(1, 1)) / det;
+    inv[1][0] = c01 / det; inv[1][1] = (a(0, 0) * a(2, 2) - a(0, 2) * a(2, 0)) / det; inv[1][2] = (a(0, 2) * a(1, 0) - a(0, 0) * a(1, 2)) / det;
+    inv[2][0] = c02 / det; inv[2][1] = (a(0, 1) * a(2, 0) - a(0, 0) * a(2, 1)) / det; inv[2][2] = (a(0, 0) * a(1, 1) - a(0, 1) * a(1, 0)) / det;
+    memcpy(out, m, sizeof(float) * 12);
+    for (int col = 0; col < 3; ++col)
+        for (int r = 0; r < 3; ++r) out[12 + 3 * col + r] = (float)inv[r][col];
+    for (int r = 0; r < 3; ++r) out[21 + r] = (float)-(inv[r][0] * t[0] + inv[r][1] * t[1] + inv[r][2] * t[2]);
+    for (int e = 12; e < 24; ++e) if (!isfinite(out[e])) return false;
+    return true;
+}
+
+// New drawn-id layout: device tables, ring and record / look-back / sort capacity for n instances drawing D ids.  The caller synchronised.
+static int instance_layout(gsr_ctx *c, const uint64_t *range, uint32_t n, uint64_t drawn) {
+    auto &I = c->inst;
+    const uint32_t blocks = projection_num_blocks((uint32_t)drawn);
+    if (drawn > c->rec_entries) {   // record tables for max(max_splats, D) drawn ids
+        float4 *r1 = nullptr, *r2 = nullptr;
+        GSR_CUDA_TRY(cudaMalloc((void **)&r1, sizeof(float4) * 3ull * drawn));
+        cudaError_t e = cudaMalloc((void **)&r2, sizeof(float4) * 3ull * drawn);
+        if (e != cudaSuccess) { cudaFree(r1); set_last_error("cudaMalloc(records, D = %llu) -> %s", (unsigned long long)drawn, cudaGetErrorString(e)); return GSR_ERR_OOM; }
+        GSR_CUDA_TRY(cudaMemset(r1, 0, sizeof(float4) * 3ull * drawn));
+        GSR_CUDA_TRY(cudaMemset(r2, 0, sizeof(float4) * 3ull * drawn));
+        cudaFree(c->records); cudaFree(c->records2);
+        c->records = r1; c->records2 = r2; c->records_cur = r1; c->rec_entries = drawn;
+    }
+    if (blocks > c->lookback_cap) {
+        unsigned long long *lb = nullptr;
+        GSR_CUDA_TRY(cudaMalloc((void **)&lb, sizeof(unsigned long long) * ((size_t)blocks + 2u * GROUP_MAX * GROUP_MAX)));
+        cudaFree(c->lookback);
+        c->lookback = lb; c->lookback_cap = blocks;
+    }
+    if (n > I.cap) {
+        cudaFree(I.desc); cudaFree(I.frame); I.desc = nullptr; I.frame = nullptr;
+        if (I.ring) cudaFreeHost(I.ring);
+        I.ring = I.ring_dev = nullptr; I.cap = 0;
+        GSR_CUDA_TRY(cudaMalloc((void **)&I.desc, sizeof(InstanceDesc) * n));
+        GSR_CUDA_TRY(cudaMalloc((void **)&I.frame, sizeof(float) * 2ull * INSTANCE_FRAME_FLOATS * n));
+        if (cudaHostAlloc((void **)&I.ring, sizeof(float) * GSR_INSTANCE_RING * INSTANCE_XFORM_FLOATS * (size_t)n, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
+            cudaGetLastError(); I.ring = nullptr; set_last_error("cudaHostAlloc(instance ring) failed"); return GSR_ERR_OOM;
+        }
+        GSR_CUDA_TRY(cudaHostGetDevicePointer((void **)&I.ring_dev, I.ring, 0));
+        I.cap = n;
+    }
+    for (int i = 0; i < GSR_INSTANCE_RING; ++i) {
+        if (!I.ev[i]) GSR_CUDA_TRY(cudaEventCreateWithFlags(&I.ev[i], cudaEventDisableTiming));
+        I.ev_used[i] = false;
+    }
+    // static tables: descriptors and the instance of every warp of the grid (padding warps of the last CTA: none)
+    InstanceDesc *desc = new (std::nothrow) InstanceDesc[n ? n : 1];
+    const size_t nwarps = (size_t)blocks * (PROJ_THREADS / 32);
+    uint32_t *warps = new (std::nothrow) uint32_t[nwarps ? nwarps : 1];
+    if (!desc || !warps) { delete[] desc; delete[] warps; return GSR_ERR_OOM; }
+    uint32_t w = 0;
+    for (uint32_t k = 0; k < n; ++k) {
+        desc[k].first = range[2 * k]; desc[k].count = (uint32_t)range[2 * k + 1]; desc[k].warp0 = w;
+        const uint32_t nw = (uint32_t)((range[2 * k + 1] + 31ull) / 32ull);
+        for (uint32_t j = 0; j < nw; ++j) warps[w + j] = k;
+        w += nw;
+    }
+    for (size_t j = w; j < nwarps; ++j) warps[j] = 0xFFFFFFFFu;
+    cudaFree(I.warps); I.warps = nullptr;
+    cudaError_t e = cudaMalloc((void **)&I.warps, sizeof(uint32_t) * (nwarps ? nwarps : 1));
+    if (e == cudaSuccess && n) e = cudaMemcpy(I.desc, desc, sizeof(InstanceDesc) * n, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess && nwarps) e = cudaMemcpy(I.warps, warps, sizeof(uint32_t) * nwarps, cudaMemcpyHostToDevice);
+    delete[] desc; delete[] warps;
+    if (e != cudaSuccess) { set_last_error("instance tables -> %s", cudaGetErrorString(e)); return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA; }
+    // the first instanced frame must not overflow: the initial capacity rule (factor x splats) applied to the drawn ids
+    if (drawn > c->max_splats) {
+        int rc = grow_capacity(c, c->dup_factor * drawn);
+        if (rc) return rc;
+    }
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_instances(gsr_ctx *c, const gsr_instance *instances, uint32_t n) {
+    if (!c) return GSR_ERR_INVALID;
+    if (n == 0) { c->inst.n = 0; c->inst.drawn = 0; return GSR_OK; }   // tables stay allocated; frames in flight keep reading them
+    if (!instances) { set_last_error("gsr_set_instances: NULL array with n = %u", n); return GSR_ERR_INVALID; }
+    if (n > GSR_MAX_INSTANCES) { set_last_error("gsr_set_instances: %u instances exceed GSR_MAX_INSTANCES (%d)", n, GSR_MAX_INSTANCES); return GSR_ERR_INVALID; }
+    if (c->grp.world > 1 || c->peer_mode || c->row_mod > 1 || !(c->band_y0 == 0 && c->band_y1 == c->tiles_y)) {
+        set_last_error("gsr_set_instances: single-context only (no group, peer framebuffers, partial band or row interleave)");
+        return GSR_ERR_STATE;
+    }
+    float *xf = new (std::nothrow) float[(size_t)INSTANCE_XFORM_FLOATS * n];
+    uint64_t *range = new (std::nothrow) uint64_t[2ull * n];
+    if (!xf || !range) { delete[] xf; delete[] range; return GSR_ERR_OOM; }
+    uint64_t warps = 0;
+    for (uint32_t k = 0; k < n; ++k) {
+        const gsr_instance &g = instances[k];
+        const char *bad = nullptr;
+        if (g.count > c->max_splats || g.first > c->max_splats - g.count) bad = "range beyond max_splats";
+        else if (!instance_inverse(g.to_frame, xf + (size_t)INSTANCE_XFORM_FLOATS * k)) bad = "non-finite or singular transform";
+        if (bad) {
+            set_last_error("gsr_set_instances: instance %u [%llu, +%llu): %s", k, (unsigned long long)g.first, (unsigned long long)g.count, bad);
+            delete[] xf; delete[] range;
+            return GSR_ERR_INVALID;
+        }
+        range[2 * k] = g.first; range[2 * k + 1] = g.count;
+        warps += (g.count + 31ull) / 32ull;
+    }
+    const uint64_t drawn = 32ull * warps;
+    if (drawn >= (1ull << 32) - 256ull) {
+        set_last_error("gsr_set_instances: %llu drawn ids (padded to whole warps) must be < 2^32 - 256", (unsigned long long)drawn);
+        delete[] xf; delete[] range;
+        return GSR_ERR_INVALID;
+    }
+    auto &I = c->inst;
+    const bool same_layout = I.n == n && I.range && memcmp(I.range, range, sizeof(uint64_t) * 2ull * n) == 0;
+    if (!same_layout) {   // new drawn-id layout: may synchronise and reallocate
+        int rc = use_device(c->device);
+        if (!rc) {
+            cudaError_t e = cudaStreamSynchronize(c->front_stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(c->copy_stream);
+            if (e != cudaSuccess) { set_last_error("gsr_set_instances: sync -> %s", cudaGetErrorString(e)); rc = GSR_ERR_CUDA; }
+        }
+        c->front_gate = nullptr;
+        I.n = 0; I.drawn = 0;   // a failure below leaves instancing off
+        if (!rc) rc = instance_layout(c, range, n, drawn);
+        if (rc) { delete[] xf; delete[] range; return rc; }
+        delete[] I.range;
+        I.range = range;
+    } else {
+        delete[] range;
+    }
+    // transforms: the host copy the next frames hand to the ring
+    delete[] I.xf;
+    I.xf = xf;
+    I.n = n; I.drawn = drawn;
     return GSR_OK;
 }
 
@@ -1247,7 +1446,7 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
     const void *src = nullptr;
     size_t avail = 0;
     switch (which) {
-        case GSR_BUF_RECORDS: src = c->records_cur; avail = sizeof(float4) * 3ull * c->max_splats; break;
+        case GSR_BUF_RECORDS: src = c->records_cur; avail = sizeof(float4) * 3ull * (c->inst.n ? c->inst.drawn : c->max_splats); break;
         case GSR_BUF_KEYS: src = c->keys_cur; avail = sizeof(uint32_t) * c->capacity; break;
         case GSR_BUF_VALUES: src = c->vals_cur; avail = sizeof(uint32_t) * c->capacity; break;
         case GSR_BUF_BOUNDS: src = c->bounds; avail = sizeof(uint2) * (size_t)c->tiles_x * c->tiles_y; break;
@@ -1256,6 +1455,12 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
         case GSR_BUF_FRAMEBUFFER: src = framebuffer(c); avail = sizeof(float4) * (size_t)c->width * c->height; break;
         case GSR_BUF_COMPOSITOR_TRACE: src = c->trace; avail = c->trace ? sizeof(ulonglong4) * (size_t)c->trace_cap : 0; break;
         case GSR_BUF_COMPOSITOR_TRACE_COUNT: src = c->trace_count; avail = c->trace_count ? sizeof(uint32_t) : 0; break;
+        case GSR_BUF_INSTANCES: {   // host copy: no device involved
+            avail = sizeof(float) * INSTANCE_XFORM_FLOATS * c->inst.n;
+            if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }
+            memcpy(dst, c->inst.xf, bytes);
+            return GSR_OK;
+        }
         default: set_last_error("gsr_debug_copy: unknown buffer %d", which); return GSR_ERR_INVALID;
     }
     if (!src || bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }

@@ -175,9 +175,13 @@ struct LaneOut {  // what one splat contributes (valid when n > 0)
 
 // gsplat_projection.glsl:158-218 for one splat given its plane-0..2 values.  Returns false when the splat is culled (or,
 // in fast sharded mode, provably outside this context's rows).  QUICK: stop after the cull + conservative reject.
-template <bool QUICK>
-__device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const float4 pt, const float4 ca, const float4 cb, LaneOut &o) {
-    const float *V = a.vp, *P = a.vp + 16;  // X[c][r] = X[4*c + r]
+// V (16 floats) and cam (3) stand for the view matrix and uniforms.camera_pos: the frame's own (a.vp, a.u.camera_pos), or an
+// instance's V_k = V * M_k and cam_k = M_k^-1 * camera_pos (instance_prepare_kernel).  INST: `At` is the instance's A|t (12 floats,
+// column-major) and the record's position words hold the FRAME-space position A * sp + t instead of sp.
+template <bool QUICK, bool INST = false>
+__device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const float *V, const float *cam, const float *At, const float4 pt,
+                                             const float4 ca, const float4 cb, LaneOut &o) {
+    const float *P = a.vp + 16;  // X[c][r] = X[4*c + r]
     const int W = a.u.dims[0], H = a.u.dims[1];
     const uint32_t gx = (uint32_t)((W + TILE - 1) / TILE), gy = (uint32_t)((H + TILE - 1) / TILE);
     const float ms = a.u.model_scale;
@@ -295,11 +299,22 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             if (nt == 0u) return false;
 
             // :198-206 everything of the record except the colour
+            if constexpr (INST) {   // frame-space position w = A * sp + t (what gsr_pick and depth compositing read)
+                const float d0 = sp0 - cam[0], d1 = sp1 - cam[1], d2 = sp2 - cam[2];
+                const float inv_len = 1.0f / sqrtf((d0 * d0 + d1 * d1) + d2 * d2);
+                o.vx = d0 * inv_len; o.vy = d1 * inv_len; o.vz = d2 * inv_len; o.opacity = splat_opacity;
+                const float w0 = ((At[0] * sp0 + At[3] * sp1) + At[6] * sp2) + At[9];
+                const float w1 = ((At[1] * sp0 + At[4] * sp1) + At[7] * sp2) + At[10];
+                const float w2 = ((At[2] * sp0 + At[5] * sp1) + At[8] * sp2) + At[11];
+                o.r0.x = ipx; o.r0.y = ipy; o.r0.z = w0; o.r0.w = w1;
+                o.r1.x = cz / det; o.r1.y = -cy / det; o.r1.z = cx / det; o.r1.w = w2;
+            } else {   // (the frame's camera_pos is read from the grid constants as written here: the default SASS stays as it was)
             const float d0 = sp0 - a.u.camera_pos[0], d1 = sp1 - a.u.camera_pos[1], d2 = sp2 - a.u.camera_pos[2];
             const float inv_len = 1.0f / sqrtf((d0 * d0 + d1 * d1) + d2 * d2);
             o.vx = d0 * inv_len; o.vy = d1 * inv_len; o.vz = d2 * inv_len; o.opacity = splat_opacity;
             o.r0.x = ipx; o.r0.y = ipy; o.r0.z = sp0; o.r0.w = sp1;                        // image_pos, pos_xy
             o.r1.x = cz / det; o.r1.y = -cy / det; o.r1.z = cx / det; o.r1.w = sp2;        // conic, pos_z
+            }
             // :218
             o.depth = ((uint32_t)(ndc2 * ndc2 * ndc2 * 65535.0f)) & 0xFFFFu;
             o.n = nt; o.x0 = (uint32_t)x0; o.y0 = (uint32_t)y0; o.w = (uint32_t)(x1 - x0);
@@ -324,7 +339,30 @@ constexpr int PROJ_WARPS = PROJ_THREADS / 32;
 constexpr size_t PROJ_SLAB_BYTES = sizeof(float4) * NUM_PLANES * 32;             // 7680 B per warp
 constexpr size_t PROJ_SMEM_BYTES = PROJ_SLAB_BYTES * PROJ_WARPS;                // 61440 B per CTA
 
-__global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a) {
+// Instanced warp: its instance k, first source splat, live lanes and the bytes of one plane slice (0 for a padding warp of the last CTA).
+struct InstanceWarp { uint32_t k; uint64_t src0; uint32_t live, slice_bytes; };
+__device__ __forceinline__ InstanceWarp instance_warp(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t vwarp) {
+    InstanceWarp w{0xFFFFFFFFu, 0ull, 0u, 0u};
+    const uint32_t k = __ldg(ia.warp_inst + vwarp);
+    if (k == 0xFFFFFFFFu) return w;
+    const InstanceDesc d = ia.desc[k];
+    const uint32_t j = vwarp - d.warp0;
+    w.k = k;
+    w.src0 = d.first + 32ull * j;
+    w.live = d.count - 32u * j < 32u ? d.count - 32u * j : 32u;
+    // no plane slice is read past plane_stride: a range that ends at max_splats with an unaligned first copies fewer bytes
+    const uint64_t room = a.plane_stride - w.src0;
+    w.slice_bytes = (uint32_t)(room < 32ull ? room : 32ull) * (uint32_t)sizeof(float4);
+    return w;
+}
+
+// INSTANCED (gsr_set_instances): the grid runs over DRAWN ids.  Instance k owns the drawn warps [warp0_k, warp0_k + ceil(count_k/32));
+// drawn warp warp0_k + j projects source splats first_k + 32 j + lane (lanes past count_k are dead) with the instance's V_k / cam_k and
+// writes record, key and value at its drawn id.  Everything after the projection -- scan, emit, sort, compositor -- is unchanged.
+// The default instantiation (INSTANCED = false) compiles to the same instruction stream as the kernel before instancing existed.
+template <bool INSTANCED = false>
+__global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
+                                                                                       const __grid_constant__ InstanceArgs ia = InstanceArgs()) {
 #ifndef GSR_CPU_EMU
     extern __shared__ __align__(128) unsigned char proj_smem[];
 #else
@@ -358,10 +396,22 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     const uint32_t id = id0 + lane;
 
     // ---- phase 1: TMA the warp's slices of planes 0..2 (planes are padded to a multiple of 256 splats) ----
+    // (instanced: every instance-only value lives inside `if constexpr` blocks -- even an unused declaration changes the default SASS)
+    if constexpr (INSTANCED) {
+        const InstanceWarp iw = instance_warp(a, ia, vwarp);
+        if (lane == 0) {   // a padding warp arrives with no bytes expected, so its wait completes at once
+            mbar_expect_tx(&s_bar[warp][0], 3u * iw.slice_bytes);
+            if (iw.slice_bytes) {
+#pragma unroll
+                for (int k = 0; k < 3; ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + iw.src0, iw.slice_bytes, &s_bar[warp][0]);
+            }
+        }
+    } else {
     if (lane == 0) {
         mbar_expect_tx(&s_bar[warp][0], 3u * 512u);
 #pragma unroll
         for (int k = 0; k < 3; ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + id0, 512u, &s_bar[warp][0]);
+    }
     }
 
     const uint32_t gx = (uint32_t)((a.u.dims[0] + TILE - 1) / TILE);
@@ -373,10 +423,22 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
 
     mbar_wait(&s_bar[warp][0], 0);
     bool colour_done = false;  // compaction path: records (incl. colour) are already written
-    if (!a.fast_reject) {
+    if constexpr (INSTANCED) {
+        const InstanceWarp iw = instance_warp(a, ia, vwarp);
+        if (lane < iw.live) {
+            // the instance's constants: V_k (16) | cam_k (3) | A_k | t_k (12), 128 B that every lane of the warp reads (L1 broadcasts)
+            const float *sk = ia.frame + (size_t)iw.k * INSTANCE_FRAME_FLOATS;
+            LaneOut o;
+            if (project_lane<false, true>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+                n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
+                r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
+            }
+            last_tile = o.last_tile;
+        }
+    } else if (!a.fast_reject) {
         if (id < a.num_splats) {
             LaneOut o;
-            if (project_lane<false>(a, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -390,7 +452,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         //      slot, so scan and emit below are unchanged and the emission order stays the splat-id order).
         bool live = false;
         LaneOut q;
-        if (id < a.num_splats) live = project_lane<true>(a, slab[lane], slab[32 + lane], slab[64 + lane], q);
+        if (id < a.num_splats) live = project_lane<true>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q);
         s_res[tid] = make_uint4(0u, 0u, 0u, 0xFFFFFFFFu);
         const uint32_t lmask = __ballot_sync(0xffffffffu, live);
         uint32_t wbase = 0;
@@ -405,7 +467,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
-            if (project_lane<false>(a, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
+            if (project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
                 float col[3];
                 sh_color<false>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
@@ -449,9 +511,16 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     //      CTA aggregates) while its SH bulk copies are in flight, so the other warps rarely find `s_ready` unset ----
     const bool bulk = !colour_done && nvis >= (uint32_t)a.sh_bulk_min;
     if (bulk && lane == 0) {
+        if constexpr (INSTANCED) {   // nvis > 0: a live warp, slice_bytes > 0
+            const InstanceWarp iw = instance_warp(a, ia, vwarp);
+            mbar_expect_tx(&s_bar[warp][1], 12u * iw.slice_bytes);
+#pragma unroll
+            for (int k = 3; k < NUM_PLANES; ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + iw.src0, iw.slice_bytes, &s_bar[warp][1]);
+        } else {
         mbar_expect_tx(&s_bar[warp][1], 12u * 512u);
 #pragma unroll
         for (int k = 3; k < NUM_PLANES; ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + id0, 512u, &s_bar[warp][1]);
+        }
     }
     if (closer) {
         const unsigned long long cta_base = lookback_exclusive(a.lookback, bid, (unsigned long long)cta_total, lane);
@@ -481,7 +550,8 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         }
     } else if (n && !colour_done) {
         float col[3];
-        sh_color<false>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
+        if constexpr (INSTANCED) sh_color<false>(a.soa + 3ull * a.plane_stride + instance_warp(a, ia, vwarp).src0 + lane, a.plane_stride, vx, vy, vz, col);
+        else sh_color<false>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
         float4 *rec = a.records + (uint64_t)id * 3u;
         rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
     }
@@ -591,7 +661,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 3) projection_sharded_kernel(con
         const uint32_t slot = g * PROJ_THREADS + tid;
         bool live = false;
         LaneOut q;
-        if (base_id + slot < a.num_splats) live = project_lane<true>(a, slab_at(slot, 0), slab_at(slot, 1), slab_at(slot, 2), q);
+        if (base_id + slot < a.num_splats) live = project_lane<true>(a, a.vp, a.u.camera_pos, nullptr, slab_at(slot, 0), slab_at(slot, 1), slab_at(slot, 2), q);
         const uint32_t lmask = __ballot_sync(0xffffffffu, live);
         uint32_t wbase = 0;
         if (lane == 0 && lmask) wbase = atomicAdd(&s_ncomp, (uint32_t)__popc(lmask));
@@ -606,7 +676,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 3) projection_sharded_kernel(con
         const uint32_t slot = s_list[it];
         const uint32_t gid = base_id + slot;
         LaneOut o;
-        const bool hit = project_lane<false>(a, slab_at(slot, 0), slab_at(slot, 1), slab_at(slot, 2), o);
+        const bool hit = project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, slab_at(slot, 0), slab_at(slot, 1), slab_at(slot, 2), o);
         if (hit && o.n) {
             float col[3];
             sh_color<false>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
@@ -801,7 +871,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         mbar_wait(&s_bar[warp][0], 0);
         if (li0 + lane < sp.count && id < a.num_splats) {
             LaneOut o;
-            if (project_lane<false>(a, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth; y1u = o.y0 + o.n / o.w;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -962,6 +1032,41 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     }
 }
 
+// ==============================================================================================================
+// Instances: the per-frame constants of every instance, composed from the frame's view matrix V and camera position c and the
+// instance's A|t and B|u = A^-1 | -A^-1 t (include/gsr.h gsr_set_instances; one rounding per operation, structurally zero terms skipped):
+//   V_k[4c+r] = (V[r] A[c][0] + V[4+r] A[c][1]) + V[8+r] A[c][2]          (c < 3)
+//   V_k[12+r] = ((V[r] t0 + V[4+r] t1) + V[8+r] t2) + V[12+r]
+//   cam_k[r]  = ((B[0][r] c0 + B[1][r] c1) + B[2][r] c2) + u[r]
+struct InstancePrepareArgs {
+    const float *xf;      // count x INSTANCE_XFORM_FLOATS
+    float v[16], cam[3];
+    uint32_t count;
+    float *out;           // count x INSTANCE_FRAME_FLOATS
+};
+
+__global__ void __launch_bounds__(256) instance_prepare_kernel(const __grid_constant__ InstancePrepareArgs p) {
+    for (uint32_t i = threadIdx.x; i < p.count; i += blockDim.x) {
+        const float *x = p.xf + (size_t)i * INSTANCE_XFORM_FLOATS;
+        float A[12], B[12];   // columns a0 a1 a2 t | b0 b1 b2 u
+#pragma unroll
+        for (int e = 0; e < 12; ++e) { A[e] = x[e]; B[e] = x[12 + e]; }
+        float *o = p.out + (size_t)i * INSTANCE_FRAME_FLOATS;
+        const float *V = p.v;
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) o[4 * c + r] = (V[r] * A[3 * c + 0] + V[4 + r] * A[3 * c + 1]) + V[8 + r] * A[3 * c + 2];
+#pragma unroll
+        for (int r = 0; r < 4; ++r) o[12 + r] = ((V[r] * A[9] + V[4 + r] * A[10]) + V[8 + r] * A[11]) + V[12 + r];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) o[16 + r] = ((B[r] * p.cam[0] + B[3 + r] * p.cam[1]) + B[6 + r] * p.cam[2]) + B[9 + r];
+#pragma unroll
+        for (int e = 0; e < 12; ++e) o[19 + e] = A[e];
+        o[31] = 0.0f;
+    }
+}
+
 }  // namespace
 
 uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_THREADS - 1) / PROJ_THREADS; }
@@ -972,12 +1077,15 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 int preload_projection_kernels() {
     cudaFuncAttributes fa;
     // dynamic shared memory opt-in is a per-device function attribute: set here, once per context creation, on the context's device
-    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROJ_SMEM_BYTES));
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROJ_SMEM_BYTES));
     GSR_CUDA_TRY(cudaFuncSetAttribute(projection_sharded_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SH_SLAB_BYTES));
     GSR_CUDA_TRY(cudaFuncSetAttribute(projection_scatter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROJ_SMEM_BYTES));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel));
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)PROJ_SMEM_BYTES));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<false>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_sharded_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_scatter_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, instance_prepare_kernel));
     return GSR_OK;
 }
 uint32_t projection_scatter_blocks(uint32_t count) { return count ? (count + PROJ_THREADS - 1) / PROJ_THREADS : 1u; }   // an empty slice still publishes its flags
@@ -1001,6 +1109,26 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream) {
         return GSR_OK;
     }
     projection_kernel<<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a);
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream) {
+    const uint32_t blocks = projection_num_blocks(a.num_splats);
+    if (blocks == 0) return GSR_OK;
+    projection_kernel<true><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia);
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream) {
+    if (count == 0) return GSR_OK;
+    InstancePrepareArgs p;
+    p.xf = xf;
+    memcpy(p.v, vp, sizeof p.v);
+    memcpy(p.cam, cam, sizeof p.cam);
+    p.count = count; p.out = out;
+    instance_prepare_kernel<<<1, 256, 0, stream>>>(p);
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }

@@ -159,6 +159,19 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_set_depth_compositing(self._ctx, C.c_void_p(scene_depth_ptr or None), C.c_void_p(depth_out_ptr or None)),
                    "gsr_set_depth_compositing")
 
+    def set_instances(self, instances) -> None:
+        """Draw placed, moving and repeated ranges of the splat buffer in one sorted frame (include/gsr.h gsr_set_instances).
+        instances: iterable of (first, count, transform), where transform is a Godot Transform3D in matrix form -- a (3, 4) array
+        [basis | origin] whose basis columns are the x, y, z axes (a (4, 4) matrix is accepted too) -- mapping the range's splats,
+        placed as the whole cloud is placed today, to their Godot world position.  An empty list switches instancing off.
+        Calling it every frame with the same (first, count) sequence only moves the instances (no host synchronisation)."""
+        items = list(instances)
+        arr = (_lib.GsrInstance * max(1, len(items)))()
+        for k, (first, count, transform) in enumerate(items):
+            arr[k].first, arr[k].count = int(first), int(count)
+            arr[k].to_frame[:] = [float(v) for v in godot_to_frame(transform, self.basis_override).T.reshape(12)]
+        _lib.check(_lib.lib().gsr_set_instances(self._ctx, arr, len(items)), "gsr_set_instances")
+
     def render_raw(self, vp32: np.ndarray, uniforms32: bytes, heatmap: float = 0.0, host_ptr: int | None = None,
                    asynchronous: bool = True, rgb_only: bool = False, out_format: int | None = None) -> None:
         """rasterize() with pre-packed push constants / uniform block (bench hot loop).  out_format: GSR_OUT_* of the host frame
@@ -332,6 +345,26 @@ class GaussianSplattingRasterizer:
 
     def keep_unsorted(self, enable: bool = True) -> None:
         _lib.check(_lib.lib().gsr_debug_keep_unsorted(self._ctx, int(enable)), "gsr_debug_keep_unsorted")
+
+
+def godot_to_frame(transform, basis_override) -> np.ndarray:
+    """A Godot Transform3D (matrix form, (3, 4) [basis | origin] or (4, 4)) -> the (3, 4) float32 [A | t] of gsr_instance.to_frame.
+
+    Frame space is where the uploaded splats, the view matrix and camera_pos live: a Godot world point p sits at F B p in frame
+    space, with F = diag(-1, -1, 1) and B = basis_override in matrix form (the convention of update_camera_matrices, uniforms_bytes
+    and get_splat_position).  An object placed by T therefore maps splat coordinates by M = F B T B^-1 F.  It is evaluated as
+    I + F B (T - I) B^-1 F in float64, so the identity maps to the identity exactly."""
+    T = np.asarray(transform, dtype=np.float64)
+    if T.shape == (4, 4):
+        T = T[:3]
+    assert T.shape == (3, 4), T.shape
+    D = np.eye(4)
+    D[:3] = T
+    D -= np.eye(4)
+    Fb = np.eye(4)
+    Fb[:3, :3] = np.diag([-1.0, -1.0, 1.0]) @ np.asarray(basis_override, dtype=np.float64).T
+    M = np.eye(4) + Fb @ D @ np.linalg.inv(Fb)
+    return M[:3].astype(np.float32)
 
 
 def sort_pairs(keys: np.ndarray, values: np.ndarray | None = None, device: int = 0):

@@ -65,7 +65,9 @@ enum {
     GSR_BUF_VALUES_UNSORTED = 5,
     GSR_BUF_FRAMEBUFFER = 6,  /* RGBA32F W*H (descriptors['render_texture']) */
     GSR_BUF_COMPOSITOR_TRACE = 7,       /* schedule trace of the last frame's compositor (gsr_debug_enable_trace) */
-    GSR_BUF_COMPOSITOR_TRACE_COUNT = 8  /* number of trace items written (uint32) */
+    GSR_BUF_COMPOSITOR_TRACE_COUNT = 8, /* number of trace items written (uint32) */
+    GSR_BUF_INSTANCES = 9               /* gsr_set_instances: 24 floats per instance, to_frame as given then the library's inverse
+                                           [A^-1 | -A^-1 t] rounded to float (both 3x4, column-major) */
 };
 
 typedef struct gsr_ctx gsr_ctx;       /* one rasterizer = one GaussianSplattingRasterizer instance */
@@ -255,6 +257,38 @@ GSR_API int gsr_set_framebuffer_external(gsr_ctx *ctx, void *device_ptr);
  *      or row_mod > 1, and those calls fail with GSR_ERR_STATE while the mode is on.  gsr_resize switches the mode off;
  *      gsr_pick keeps the default path (and leaves the depth-composited frame as it is).  GSR_ERR_STATE before gsr_resize. ---- */
 GSR_API int gsr_set_depth_compositing(gsr_ctx *ctx, const float *scene_depth_device, float *depth_out_device);
+
+/* ---- Splat instances (no reference counterpart: the reference draws one cloud at the origin).  An instance draws the source range
+ *      [first, first + count) of the uploaded splats with its own affine transform `to_frame` = [A | t] (3x4, column-major: columns
+ *      a0, a1, a2, t) from the range's splat coordinates (position * model_scale) into FRAME space, the space the uploaded splats, the
+ *      view matrix of view_proj and uniforms.camera_pos live in.  With n > 0 instances set, every later gsr_render* draws exactly the
+ *      instances' splats, all of them in ONE sorted frame, so overlapping clouds blend in the correct order:
+ *        - ranges may overlap and the same range may be drawn any number of times (one asset stored once, drawn many times);
+ *          splats outside every range are not drawn;
+ *        - instance k is projected with V_k = V * [A|t] in place of the view matrix and cam_k = A^-1 (camera_pos - t) in place of the
+ *          camera position: cull, EWA covariance, depth key and the SH view direction (evaluated in the object's own frame) follow
+ *          the default projection exactly; the records' position words hold the frame-space position A * sp + t, so gsr_pick returns
+ *          frame-space positions and depth compositing works unchanged.  For rigid and uniformly scaled transforms this is the
+ *          transformed cloud; with a non-uniform scale positions and covariances are still exact, but the SH colour is evaluated
+ *          in the object's frame (the coefficients are not rotated);
+ *        - drawn ids: instance k owns [32 w_k, 32 w_k + count_k), w_k = sum over j < k of ceil(count_j / 32); D = 32 * sum ceil(count/32).
+ *          Pairs of equal keys keep instance order, then source order.  GSR_BUF_RECORDS returns D records.
+ *      The array is copied; frames already enqueued keep the transforms they were enqueued with.  A call with the same (first, count)
+ *      sequence as the current instances only replaces the transforms: the per-frame path, it never synchronises the host (the
+ *      transforms reach the device through a mapped page-locked ring consumed by a kernel on the frame's stream; only a host more than
+ *      GSR_INSTANCE_RING frames ahead of the GPU waits for a slot).  Any other call re-lays out the drawn ids: it synchronises and may
+ *      reallocate (record tables for max(max_splats, D) ids; the sort capacity is raised to factor * D when D > max_splats).
+ *      n == 0 switches instancing off: the default frame.  GSR_ERR_INVALID, previous state kept: n > GSR_MAX_INSTANCES, a range beyond
+ *      max_splats, a non-finite entry, a singular A, D >= 2^32 - 256.  Single-context only: GSR_ERR_STATE with an attached group, peer
+ *      framebuffers, a partial band or row_mod > 1, and those calls fail with GSR_ERR_STATE while instances are set.  gsr_resize
+ *      keeps the instances. ---- */
+#define GSR_MAX_INSTANCES 4096
+#define GSR_INSTANCE_RING 8
+typedef struct gsr_instance {
+    uint64_t first, count;  /* source range of the uploaded splats */
+    float to_frame[12];     /* [A | t], column-major 3x4 */
+} gsr_instance;
+GSR_API int gsr_set_instances(gsr_ctx *ctx, const gsr_instance *instances, uint32_t n);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
