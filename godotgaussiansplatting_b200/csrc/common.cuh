@@ -12,6 +12,14 @@ constexpr int TILE = 16;            // rasterizer.gd:4 TILE_SIZE
 constexpr int NUM_PLANES = 15;      // 60-float Splat = 15 float4 planes in SoA
 constexpr int PROJ_THREADS = 256;   // gsplat_projection.glsl:31 local_size_x
 
+// SH storage by degree (gsr_config.sh_bands): B bands = degree + 1 hold K = B^2 coefficients per channel, stored coefficient-major RGB in
+// P = ceil(3K / 4) float4 planes after planes 0-2.  B = 1, 2, 3, 4 -> P = 1, 3, 7, 12 (64 / 96 / 160 / 240 B per splat).
+constexpr int SH_BANDS_MAX = 4;
+__host__ __device__ constexpr int sh_coeffs(int bands) { return bands * bands; }
+__host__ __device__ constexpr int sh_planes(int bands) { return (3 * bands * bands + 3) / 4; }
+__host__ __device__ constexpr int soa_planes(int bands) { return 3 + sh_planes(bands); }
+static_assert(soa_planes(SH_BANDS_MAX) == NUM_PLANES, "a degree-3 store is the 60-float Splat");
+
 // ---------------------------------------------------------------------------------------------
 // error plumbing
 // ---------------------------------------------------------------------------------------------
@@ -155,7 +163,8 @@ struct ProjectionArgs {
     unsigned long long *lookback;  // one word per projection CTA (256 splats)
     FrameState *frame;
 };
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream);
+// sh_bands: SH bands the frame evaluates (1..4, at most the store's); the kernel reads planes 0-2 and the first sh_planes(sh_bands) SH planes
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX);
 
 // ---------------------------------------------------------------------------------------------
 // splat instances (gsr_set_instances): ranges of the splat buffer drawn with their own affine transform into frame space
@@ -174,7 +183,7 @@ struct InstanceArgs {
     const uint32_t *warp_inst;              // instance of every drawn warp of the grid; 0xFFFFFFFF = padding warp
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream);
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX);
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
 // (mapped page-locked host memory on the frame path)
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream);
@@ -281,12 +290,15 @@ int composite_max_ctas_per_sm(int *out);
 int launch_tile_order(const uint2 *bounds, int32_t tile_begin, int32_t row_step, int32_t tiles_x, int32_t num_tiles, uint32_t *hint, uint32_t *order,
                       FrameState *frame, uint32_t sparse_tiles, uint32_t sparse_cta_limit, cudaStream_t stream);
 
-int launch_ply_to_soa(const float *ply, uint32_t nprops, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride, uint64_t first,
-                      cudaStream_t stream);
+// The standard 62-property layout of the original 3DGS trainer (x y z nx ny nz f_dc_0..2 f_rest_0..44 opacity scale_0..2 rot_0..3).
+constexpr gsr_ply_layout PLY_LAYOUT_3DGS = {62u, 3u, 0, 6, 9, 54, 55, 58};
+// PLY vertices of any layout -> the first `planes` (= soa_planes(store bands)) SoA planes
+int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
+                      uint64_t first, int planes, cudaStream_t stream);
 // present.cu: RGBA32F frame -> GSR_OUT_* (| GSR_OUT_SRGB_TO_LINEAR)
 int launch_present(const float4 *rgba, void *out, uint64_t pixels, int format, cudaStream_t stream);
 size_t present_bytes_per_pixel(int format);
-int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, cudaStream_t stream);
+int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, int planes, cudaStream_t stream);
 
 // cudaFuncGetAttributes on every kernel of a file: defeats lazy module loading before the first frame
 int preload_group_kernels();

@@ -38,7 +38,9 @@ struct gsr_ctx {
     uint64_t max_splats = 0, capacity = 0, plane_stride = 0, num_splats = 0;
     uint64_t cap_stride = 0;     // capacity rounded up to 1024 pairs: distance between the three pair buffers (keeps each 16-byte aligned)
     cudaStream_t stream = nullptr, own_stream = nullptr;
-    float4 *soa = nullptr;       // 15 planes x plane_stride
+    float4 *soa = nullptr;       // soa_planes(sh_bands) planes x plane_stride (15 for a degree-3 store)
+    int sh_bands = SH_BANDS_MAX; // SH bands the store keeps (gsr_config.sh_bands)
+    int sh_degree = -1;          // render degree (gsr_set_sh_degree); -1 = the stored degree
     float4 *records = nullptr;   // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -83,6 +85,7 @@ struct gsr_ctx {
     float4 *pick = nullptr;
     float4 *staging = nullptr;
     uint64_t staging_splats = 0;
+    uint64_t staging_bytes = 0;  // 16 B x stored planes x staging_splats (at least one 240-byte AoS struct)
     uint32_t *unsorted_keys = nullptr, *unsorted_vals = nullptr;
     bool keep_unsorted = false;
     int width = 0, height = 0, tiles_x = 0, tiles_y = 0, band_y0 = 0, band_y1 = 0;
@@ -183,6 +186,10 @@ void group_detach(gsr_ctx *c) {
 
 float4 *framebuffer(gsr_ctx *c) { return c->fb_ext ? c->fb_ext : (c->fb_last ? c->fb_last : c->fb); }
 
+// SH bands the next frame evaluates, and whether the context stores or renders fewer than 4 (single-context only, like depth compositing)
+int render_bands(const gsr_ctx *c) { return c->sh_degree < 0 ? c->sh_bands : c->sh_degree + 1; }
+bool reduced_sh(const gsr_ctx *c) { return c->sh_bands < SH_BANDS_MAX || render_bands(c) < SH_BANDS_MAX; }
+
 void free_ctx(gsr_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
@@ -247,12 +254,15 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     if (rc) return rc;
     if ((rc = use_device(cfg->device))) return rc;
     if (cfg->max_splats >= (1ull << 32) - 256ull) { set_last_error("max_splats must be < 2^32-256"); return GSR_ERR_INVALID; }
+    if (cfg->sh_bands > (uint32_t)SH_BANDS_MAX) { set_last_error("gsr_create: sh_bands %u > %d (degree 3)", cfg->sh_bands, SH_BANDS_MAX); return GSR_ERR_INVALID; }
     gsr_ctx *c = new (std::nothrow) gsr_ctx();
     if (!c) return GSR_ERR_OOM;
     c->device = cfg->device;
     c->flags = cfg->flags;
     if (!(c->flags & (GSR_FLAG_REFERENCE_QUIRKS | GSR_FLAG_FIXED_RANGES))) c->flags |= GSR_FLAG_REFERENCE_QUIRKS;
     c->max_splats = cfg->max_splats;
+    c->sh_bands = cfg->sh_bands ? (int)cfg->sh_bands : SH_BANDS_MAX;
+    const uint64_t planes = (uint64_t)soa_planes(c->sh_bands);
     const uint64_t factor = cfg->dup_capacity_factor ? cfg->dup_capacity_factor : 10;  // rasterizer.gd:79
     c->dup_factor = factor;
     c->capacity_max = (1ull << 30) - 1;  // look-back words carry 30-bit counts
@@ -291,7 +301,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
         if (se == cudaSuccess) se = cudaEventCreateWithFlags(&c->ev_copied[i], cudaEventDisableTiming);
     }
     if (se != cudaSuccess) { set_last_error("copy stream/events -> %s", cudaGetErrorString(se)); free_ctx(c); return GSR_ERR_CUDA; }
-    TRY_ALLOC(c->soa, sizeof(float4) * NUM_PLANES * c->plane_stride);
+    TRY_ALLOC(c->soa, sizeof(float4) * planes * c->plane_stride);
     TRY_ALLOC(c->records, sizeof(float4) * 3ull * c->max_splats);
     TRY_ALLOC(c->records2, sizeof(float4) * 3ull * c->max_splats);
     c->cap_stride = (c->capacity + 1023ull) & ~1023ull;
@@ -307,7 +317,9 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     TRY_ALLOC(c->pick, sizeof(float4));
     TRY_ALLOC(c->sync_word, sizeof(int32_t));
     c->staging_splats = c->max_splats < (1ull << 18) ? c->max_splats : (1ull << 18);
-    TRY_ALLOC(c->staging, sizeof(float4) * NUM_PLANES * c->staging_splats);
+    c->staging_bytes = sizeof(float4) * planes * c->staging_splats;
+    if (c->staging_bytes < 240ull) c->staging_bytes = 240ull;
+    TRY_ALLOC(c->staging, c->staging_bytes);
 #undef TRY_ALLOC
     rc = sort_workspace_create(c->sort, c->capacity, /*need_alt_buffers=*/false);
     if (rc) { free_ctx(c); return rc; }
@@ -325,7 +337,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
         set_last_error("cudaHostAlloc(frame mirror) failed"); c->host_ring = nullptr; free_ctx(c); return GSR_ERR_OOM;
     }
     memset(c->host_ring, 0, sizeof(FrameState) * GSR_HISTORY_FRAMES);
-    cudaMemsetAsync(c->soa, 0, sizeof(float4) * NUM_PLANES * c->plane_stride, c->stream);
+    cudaMemsetAsync(c->soa, 0, sizeof(float4) * planes * c->plane_stride, c->stream);
     cudaMemsetAsync(c->records, 0, sizeof(float4) * 3ull * c->max_splats, c->stream);
     cudaMemsetAsync(c->records2, 0, sizeof(float4) * 3ull * c->max_splats, c->stream);
     cudaMemsetAsync(c->pick, 0, sizeof(float4), c->stream);
@@ -363,11 +375,12 @@ GSR_API int gsr_upload_splats_aos(gsr_ctx *c, const float *splat60, uint64_t fir
     int rc = use_device(c->device);
     if (rc) return rc;
     GSR_CUDA_TRY(cudaStreamSynchronize(c->front_stream));   // a projection in flight reads the planes this call rewrites
+    const uint64_t per = c->staging_bytes / 240ull;           // 60-float structs per chunk (staging_splats for a degree-3 store)
     uint64_t done = 0;
     while (done < count) {
-        const uint64_t m = (count - done) < c->staging_splats ? (count - done) : c->staging_splats;
+        const uint64_t m = (count - done) < per ? (count - done) : per;
         GSR_CUDA_TRY(cudaMemcpyAsync(c->staging, splat60 + (done * 60ull), m * 240ull, cudaMemcpyHostToDevice, c->stream));
-        if ((rc = launch_aos_to_soa(c->staging, m, c->soa, c->plane_stride, first + done, c->stream))) return rc;
+        if ((rc = launch_aos_to_soa(c->staging, m, c->soa, c->plane_stride, first + done, soa_planes(c->sh_bands), c->stream))) return rc;
         done += m;
     }
     GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));  // the caller may free/reuse splat60 (buffer_update semantics)
@@ -375,26 +388,54 @@ GSR_API int gsr_upload_splats_aos(gsr_ctx *c, const float *splat60, uint64_t fir
     return GSR_OK;
 }
 
-GSR_API int gsr_upload_ply_raw(gsr_ctx *c, const float *ply, uint32_t nprops, uint64_t first, uint64_t count, float creation_time) {
-    if (!c || (!ply && count)) return GSR_ERR_INVALID;
-    if (nprops < 62 || nprops > 256) { set_last_error("gsr_upload_ply_raw: %u properties; need the 62 standard 3DGS floats (x..rot_3) first", nprops); return GSR_ERR_INVALID; }
+static int upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout &lay, uint64_t first, uint64_t count, float creation_time) {
     if (count > c->max_splats || first > c->max_splats - count) { set_last_error("upload range [%llu,%llu) exceeds max_splats %llu", (unsigned long long)first, (unsigned long long)(first + count), (unsigned long long)c->max_splats); return GSR_ERR_INVALID; }
     int rc = use_device(c->device);
     if (rc) return rc;
-    const uint64_t staging_floats = c->staging_splats * 60ull;  // the AoS staging buffer, reused for raw vertices
+    const uint32_t nprops = lay.nprops;
+    const uint64_t staging_floats = c->staging_bytes / sizeof(float);  // the AoS staging buffer, reused for raw vertices
     const uint64_t per = staging_floats / nprops;
-    if (per == 0) { set_last_error("gsr_upload_ply_raw: staging buffer too small"); return GSR_ERR_INVALID; }
+    if (per == 0) { set_last_error("gsr_upload_ply: staging buffer too small"); return GSR_ERR_INVALID; }
     GSR_CUDA_TRY(cudaStreamSynchronize(c->front_stream));   // a projection in flight reads the planes this call rewrites
     uint64_t done = 0;
     while (done < count) {
         const uint64_t m = (count - done) < per ? (count - done) : per;
         GSR_CUDA_TRY(cudaMemcpyAsync(c->staging, ply + done * nprops, m * nprops * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-        if ((rc = launch_ply_to_soa(reinterpret_cast<const float *>(c->staging), nprops, m, creation_time, c->soa, c->plane_stride, first + done, c->stream))) return rc;
+        if ((rc = launch_ply_to_soa(reinterpret_cast<const float *>(c->staging), lay, m, creation_time, c->soa, c->plane_stride, first + done,
+                                    soa_planes(c->sh_bands), c->stream))) return rc;
         done += m;
     }
     GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));
     if (first + count > c->num_splats) c->num_splats = first + count;
     return GSR_OK;
+}
+
+GSR_API int gsr_upload_ply_raw(gsr_ctx *c, const float *ply, uint32_t nprops, uint64_t first, uint64_t count, float creation_time) {
+    if (!c || (!ply && count)) return GSR_ERR_INVALID;
+    if (nprops < 62 || nprops > 256) { set_last_error("gsr_upload_ply_raw: %u properties; need the 62 standard 3DGS floats (x..rot_3) first", nprops); return GSR_ERR_INVALID; }
+    gsr_ply_layout lay = PLY_LAYOUT_3DGS;
+    lay.nprops = nprops;
+    return upload_ply(c, ply, lay, first, count, creation_time);
+}
+
+GSR_API int gsr_upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout *layout, uint64_t first, uint64_t count, float creation_time) {
+    if (!c || (!ply && count)) return GSR_ERR_INVALID;
+    if (!layout) { set_last_error("gsr_upload_ply: NULL layout"); return GSR_ERR_INVALID; }
+    const gsr_ply_layout &L = *layout;
+    if (L.nprops < 1 || L.nprops > 256) { set_last_error("gsr_upload_ply: nprops %u outside 1..256", L.nprops); return GSR_ERR_INVALID; }
+    if (L.sh_degree > 3) { set_last_error("gsr_upload_ply: sh_degree %u > 3", L.sh_degree); return GSR_ERR_INVALID; }
+    if ((L.sh_degree == 0) != (L.f_rest < 0)) { set_last_error("gsr_upload_ply: f_rest %d does not match sh_degree %u (-1 iff degree 0)", L.f_rest, L.sh_degree); return GSR_ERR_INVALID; }
+    const int64_t rest = 3ll * ((int64_t)(L.sh_degree + 1) * (L.sh_degree + 1) - 1);
+    const struct { const char *name; int32_t at; int64_t len; } groups[] = {
+        {"x", L.x, 3}, {"f_dc", L.f_dc, 3}, {"f_rest", L.f_rest, rest}, {"opacity", L.opacity, 1}, {"scale", L.scale, 3}, {"rot", L.rot, 4}};
+    for (const auto &g : groups) {
+        if (g.len == 0) continue;   // f_rest of a degree-0 file
+        if (g.at < 0 || (int64_t)g.at + g.len > (int64_t)L.nprops) {
+            set_last_error("gsr_upload_ply: %s at %d (+%lld floats) does not fit %u properties", g.name, g.at, (long long)g.len, L.nprops);
+            return GSR_ERR_INVALID;
+        }
+    }
+    return upload_ply(c, ply, L, first, count, creation_time);
 }
 
 GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
@@ -446,6 +487,7 @@ GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod)
     if (!c || row_mod < 1 || row_rem < 0 || row_rem >= row_mod) { set_last_error("gsr_set_row_interleave: need 0 <= rem < mod"); return GSR_ERR_INVALID; }
     if (c->depth_out && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && row_mod > 1) { set_last_error("gsr_set_row_interleave: instances are set (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -467,6 +509,7 @@ GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (row_begin < 0 || row_end > c->tiles_y || row_begin > row_end) { set_last_error("band [%d,%d) outside [0,%d]", row_begin, row_end, c->tiles_y); return GSR_ERR_INVALID; }
     if (c->depth_out && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: instances are set (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
     c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
     return GSR_OK;
@@ -687,10 +730,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         InstanceArgs ia;
         ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
         ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
-        if ((rc = launch_projection_instanced(pa, ia, fs))) return rc;
+        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c)))) return rc;
         launches += pa.num_splats ? 1 : 0;
     } else {
-        if ((rc = launch_projection(pa, fs))) return rc;
+        if ((rc = launch_projection(pa, fs, render_bands(c)))) return rc;
         launches += pa.num_splats ? 1 : 0;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[1], fs));  // end of the front part
@@ -973,6 +1016,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
     if (c->depth_out) { set_last_error("gsr_peer_export_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n) { set_last_error("gsr_peer_export_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -989,6 +1033,7 @@ GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
     if (c->depth_out) { set_last_error("gsr_peer_import_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n) { set_last_error("gsr_peer_import_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -1018,6 +1063,7 @@ constexpr uint32_t GROUP_MAGIC = 0x47535247u;  // "GRSG"
 GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
     if (!c || !blob) return GSR_ERR_INVALID;
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_group_export: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     if (!c->grp.arena) {
@@ -1048,6 +1094,7 @@ GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void
     if (!c->grp.arena || !c->fb) { set_last_error("gsr_group_attach before gsr_group_export"); return GSR_ERR_STATE; }
     if (c->depth_out && world > 1) { set_last_error("gsr_group_attach: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && world > 1) { set_last_error("gsr_group_attach: instances are set (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1310,6 +1357,21 @@ GSR_API int gsr_set_instances(gsr_ctx *c, const gsr_instance *instances, uint32_
     return GSR_OK;
 }
 
+GSR_API int gsr_set_sh_degree(gsr_ctx *c, int32_t degree) {
+    if (!c) return GSR_ERR_INVALID;
+    if (degree < -1 || degree > c->sh_bands - 1) {
+        set_last_error("gsr_set_sh_degree: degree %d outside -1..%d (the stored degree)", degree, c->sh_bands - 1);
+        return GSR_ERR_INVALID;
+    }
+    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
+    if (degree >= 0 && degree < SH_BANDS_MAX - 1 && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
+        set_last_error("gsr_set_sh_degree: single-context only below degree 3 (no group, peer framebuffers, partial band or row interleave)");
+        return GSR_ERR_STATE;
+    }
+    c->sh_degree = degree;   // read by the next render_enqueue: frames already enqueued keep their degree
+    return GSR_OK;
+}
+
 GSR_API int gsr_pick(gsr_ctx *c, uint32_t tile_id, float heatmap_factor, float out_xyzn[4]) {
     if (!c || !out_xyzn) return GSR_ERR_INVALID;
     if (c->width == 0) { set_last_error("gsr_pick before gsr_resize"); return GSR_ERR_STATE; }
@@ -1455,6 +1517,7 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
         case GSR_BUF_FRAMEBUFFER: src = framebuffer(c); avail = sizeof(float4) * (size_t)c->width * c->height; break;
         case GSR_BUF_COMPOSITOR_TRACE: src = c->trace; avail = c->trace ? sizeof(ulonglong4) * (size_t)c->trace_cap : 0; break;
         case GSR_BUF_COMPOSITOR_TRACE_COUNT: src = c->trace_count; avail = c->trace_count ? sizeof(uint32_t) : 0; break;
+        case GSR_BUF_SPLATS: src = c->soa; avail = sizeof(float4) * (size_t)soa_planes(c->sh_bands) * c->plane_stride; break;
         case GSR_BUF_INSTANCES: {   // host copy: no device involved
             avail = sizeof(float) * INSTANCE_XFORM_FLOATS * c->inst.n;
             if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }

@@ -2,7 +2,7 @@
 //
 // The reference keeps the 60-float std430 `Splat` struct in one AoS storage buffer
 // (gsplat_projection.glsl:33-40, written by util/ply_file.gd:71).  libgsr accepts exactly that struct at the
-// boundary (gsr_upload_splats_aos) and stores it as 15 float4 planes so that the projection kernel issues
+// boundary (gsr_upload_splats_aos) and stores it as 15 float4 planes (fewer for a store of a lower SH degree) so that the projection kernel issues
 // coalesced 128-bit loads and culled splats touch one plane only.
 #include "common.cuh"
 
@@ -12,17 +12,23 @@ namespace {
 
 constexpr int SPLATS_PER_BLOCK = 128;
 
+// `planes` = soa_planes(store bands): the SH planes past them are not stored, and the floats of the last stored SH plane past the store's
+// 3K coefficients are written as 0 (the AoS struct holds the next degree's coefficients there).
 __global__ void __launch_bounds__(256) aos_to_soa_kernel(const float4 *__restrict__ aos, uint64_t count, float4 *__restrict__ soa,
-                                                         uint64_t plane_stride, uint64_t first) {
+                                                         uint64_t plane_stride, uint64_t first, int planes = NUM_PLANES) {
     __shared__ float4 s[SPLATS_PER_BLOCK * NUM_PLANES];
     const uint64_t s0 = (uint64_t)blockIdx.x * SPLATS_PER_BLOCK;
     const uint32_t here = (uint32_t)((count - s0) < (uint64_t)SPLATS_PER_BLOCK ? (count - s0) : SPLATS_PER_BLOCK);
     const float4 *src = aos + s0 * NUM_PLANES;
     for (uint32_t i = threadIdx.x; i < here * NUM_PLANES; i += blockDim.x) s[i] = src[i];  // coalesced AoS read
     __syncthreads();
-    for (uint32_t i = threadIdx.x; i < here * NUM_PLANES; i += blockDim.x) {
+    // valid floats of the last stored plane: 3K - 4(P - 1) = 3, 4, 3, 4 for 1..4 bands
+    const uint32_t tail = (planes == soa_planes(1) || planes == soa_planes(3)) ? 3u : 4u;
+    for (uint32_t i = threadIdx.x; i < here * (uint32_t)planes; i += blockDim.x) {
         const uint32_t plane = i / here, k = i - plane * here;  // consecutive threads -> consecutive splats of one plane
-        soa[(uint64_t)plane * plane_stride + first + s0 + k] = s[k * NUM_PLANES + plane];
+        float4 v = s[k * NUM_PLANES + plane];
+        if (plane == (uint32_t)planes - 1u && tail == 3u) v.w = 0.0f;
+        soa[(uint64_t)plane * plane_stride + first + s0 + k] = v;
     }
 }
 
@@ -31,7 +37,7 @@ __global__ void __launch_bounds__(256) aos_to_soa_kernel(const float4 *__restric
 // shared memory so that the AoS read is coalesced, then every thread evaluates exp(scale) and the sigmoid in float64
 // (GDScript floats are doubles; the results are narrowed when they enter Vector3 / PackedFloat32Array), builds
 // Basis(Quaternion).transposed(), Sigma = (S R)^T (S R) with Godot's Basis*Basis operation order (including the
-// structurally-zero products, so signed zeros match), re-interleaves the SH coefficients and writes the 15 SoA planes.
+// structurally-zero products, so signed zeros match), re-interleaves the SH coefficients and writes the stored SoA planes (15 for a degree-3 store).
 constexpr int INGEST_SPLATS = 128;
 
 __device__ __forceinline__ void godot_basis_mul(const float a[3][3], const float b[3][3], float o[3][3]) {
@@ -41,11 +47,14 @@ __device__ __forceinline__ void godot_basis_mul(const float a[3][3], const float
         for (int j = 0; j < 3; ++j) o[i][j] = (b[0][j] * a[i][0] + b[1][j] * a[i][1]) + b[2][j] * a[i][2];
 }
 
+// `lay` names the property groups of a vertex (gsr_ply_layout; default: the standard 62-property layout) and `planes` = soa_planes(store
+// bands) the planes written.  SH coefficients above the file's degree are stored as 0, those above the store's degree are dropped.
 __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *__restrict__ ply, uint32_t nprops, uint64_t count, float creation_time,
-                                                                  float4 *__restrict__ soa, uint64_t plane_stride, uint64_t first) {
+                                                                  float4 *__restrict__ soa, uint64_t plane_stride, uint64_t first,
+                                                                  const gsr_ply_layout lay = PLY_LAYOUT_3DGS, int planes = NUM_PLANES) {
 #ifndef GSR_CPU_EMU
     extern __shared__ float s_v[];  // [INGEST_SPLATS][nprops]
-#else  // tests/kernel_emu (CPU logic pre-flight): nprops <= 256 (gsr_upload_ply_raw rejects more)
+#else  // tests/kernel_emu (CPU logic pre-flight): nprops <= 256 (gsr_upload_ply rejects more)
     __shared__ float s_v[INGEST_SPLATS * 256];
 #endif
     const uint64_t s0 = (uint64_t)blockIdx.x * INGEST_SPLATS;
@@ -57,8 +66,9 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
     const float *p = s_v + (size_t)threadIdx.x * nprops;
     const uint64_t id = first + s0 + threadIdx.x;
 
-    const float sc0 = (float)exp((double)p[55]), sc1 = (float)exp((double)p[56]), sc2 = (float)exp((double)p[57]);
-    const float qx = p[59], qy = p[60], qz = p[61], qw = p[58];  // Quaternion(rot_1, rot_2, rot_3, rot_0)
+    const float *ps = p + lay.scale, *pr = p + lay.rot, *px = p + lay.x, *pd = p + lay.f_dc;
+    const float sc0 = (float)exp((double)ps[0]), sc1 = (float)exp((double)ps[1]), sc2 = (float)exp((double)ps[2]);
+    const float qx = pr[1], qy = pr[2], qz = pr[3], qw = pr[0];  // Quaternion(rot_1, rot_2, rot_3, rot_0)
     const float d = ((qx * qx + qy * qy) + qz * qz) + qw * qw;
     const float s = 2.0f / d;
     const float xs = qx * s, ys = qy * s, zs = qz * s;
@@ -78,17 +88,29 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
 #pragma unroll
         for (int c = 0; c < 3; ++c) Mt[r][c] = M[c][r];
     godot_basis_mul(Mt, M, Cv);
-    const float opacity = (float)(1.0 / (1.0 + exp(-(double)p[54])));
+    const float opacity = (float)(1.0 / (1.0 + exp(-(double)p[lay.opacity])));
 
-    soa[0 * plane_stride + id] = make_float4(p[0], p[1], p[2], creation_time);
+    soa[0 * plane_stride + id] = make_float4(px[0], px[1], px[2], creation_time);
     soa[1 * plane_stride + id] = make_float4(Cv[0][0], Cv[0][1], Cv[0][2], Cv[1][1]);
     soa[2 * plane_stride + id] = make_float4(Cv[1][2], Cv[2][2], opacity, 0.0f);
-    float sh[48];  // coefficient-major RGB: DC, then f_rest R 0..14 | G 15..29 | B 30..44 re-interleaved (:65-69)
-    sh[0] = p[6]; sh[1] = p[7]; sh[2] = p[8];
+    // coefficient-major RGB: DC, then f_rest R | G | B (rest = K_file - 1 floats per channel) re-interleaved (:65-69)
+    const uint32_t rest = (lay.sh_degree + 1u) * (lay.sh_degree + 1u) - 1u;
+    const uint32_t kept = (uint32_t)(planes - 3) == (uint32_t)sh_planes(4) ? 16u : (uint32_t)(planes - 3) == (uint32_t)sh_planes(3) ? 9u
+                        : (uint32_t)(planes - 3) == (uint32_t)sh_planes(2) ? 4u : 1u;   // K of the store
+    const float *pf = p + (lay.f_rest < 0 ? 0 : lay.f_rest);   // every index below stays inside the vertex, also for a coefficient not read
+    float sh[48];
+    sh[0] = pd[0]; sh[1] = pd[1]; sh[2] = pd[2];
 #pragma unroll
-    for (int k = 0; k < 15; ++k) { sh[3 + 3 * k + 0] = p[9 + k]; sh[3 + 3 * k + 1] = p[9 + 15 + k]; sh[3 + 3 * k + 2] = p[9 + 30 + k]; }
+    for (uint32_t k = 0; k < 15; ++k) {
+        const bool in = k < rest && k + 1u < kept;
+        const uint32_t kr = in ? k : 0u;
+        sh[3 + 3 * k + 0] = in ? pf[kr] : 0.0f;
+        sh[3 + 3 * k + 1] = in ? pf[rest + kr] : 0.0f;
+        sh[3 + 3 * k + 2] = in ? pf[2 * rest + kr] : 0.0f;
+    }
 #pragma unroll
-    for (int k = 0; k < 12; ++k) soa[(uint64_t)(3 + k) * plane_stride + id] = make_float4(sh[4 * k], sh[4 * k + 1], sh[4 * k + 2], sh[4 * k + 3]);
+    for (int k = 0; k < 12; ++k)
+        if (k < planes - 3) soa[(uint64_t)(3 + k) * plane_stride + id] = make_float4(sh[4 * k], sh[4 * k + 1], sh[4 * k + 2], sh[4 * k + 3]);
 }
 
 }  // namespace
@@ -102,21 +124,21 @@ int preload_ingest_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, aos_to_soa_kernel));
     return GSR_OK;
 }
-int launch_ply_to_soa(const float *ply, uint32_t nprops, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride, uint64_t first,
-                      cudaStream_t stream) {
+int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
+                      uint64_t first, int planes, cudaStream_t stream) {
     if (count == 0) return GSR_OK;
-    const size_t smem = sizeof(float) * (size_t)INGEST_SPLATS * nprops;
+    const size_t smem = sizeof(float) * (size_t)INGEST_SPLATS * layout.nprops;
     if (smem > 48 * 1024) GSR_CUDA_TRY(cudaFuncSetAttribute(ply_to_soa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const uint32_t blocks = (uint32_t)((count + INGEST_SPLATS - 1) / INGEST_SPLATS);
-    ply_to_soa_kernel<<<blocks, INGEST_SPLATS, smem, stream>>>(ply, nprops, count, creation_time, soa, plane_stride, first);
+    ply_to_soa_kernel<<<blocks, INGEST_SPLATS, smem, stream>>>(ply, layout.nprops, count, creation_time, soa, plane_stride, first, layout, planes);
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }
 
-int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, cudaStream_t stream) {
+int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, int planes, cudaStream_t stream) {
     if (count == 0) return GSR_OK;
     const uint32_t blocks = (uint32_t)((count + SPLATS_PER_BLOCK - 1) / SPLATS_PER_BLOCK);
-    aos_to_soa_kernel<<<blocks, 256, 0, stream>>>(aos, count, soa, plane_stride, first);
+    aos_to_soa_kernel<<<blocks, 256, 0, stream>>>(aos, count, soa, plane_stride, first, planes);
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }

@@ -116,13 +116,19 @@ inline void mbar_wait(uint64_t *, uint32_t) {}
 
 // SH colour (gsplat_projection.glsl:94-121), streamed six planes (= 8 coefficients x RGB) at a time so that at
 // most 24 coefficient registers are live.  `src[k * stride]` is SH plane k of this splat (shared slab or global).
-template <bool FROM_SMEM>
+// SH_BANDS < 4 (gsr_set_sh_degree, reduced stores): only the first sh_planes(SH_BANDS) planes are read and only the coefficients
+// < K = SH_BANDS^2 are evaluated, in the same order with the same operations.  The degree-3 evaluation of the same splat with the
+// coefficients >= K set to zero adds +-0 to r for a finite view direction, and NaN (so colour 0 after the final max) for a non-finite
+// one (a splat at the camera position); `skip` = 0 * ((x + y) + z) is exactly that sum, so the frame stays bit for bit the zero-padded
+// cloud's (DESIGN.md section 5.9).
+template <bool FROM_SMEM, int SH_BANDS = SH_BANDS_MAX>
 __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, float x, float y, float z, float col[3]) {
+    constexpr int K = sh_coeffs(SH_BANDS), P = sh_planes(SH_BANDS), P0 = P < 6 ? P : 6;
     const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
     {
         float sh[24];
 #pragma unroll
-        for (int k = 0; k < 6; ++k) {
+        for (int k = 0; k < P0; ++k) {
             const float4 v = FROM_SMEM ? src[(uint64_t)k * stride] : __ldg(src + (uint64_t)k * stride);
             sh[4 * k + 0] = v.x; sh[4 * k + 1] = v.y; sh[4 * k + 2] = v.z; sh[4 * k + 3] = v.w;
         }
@@ -130,21 +136,25 @@ __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, flo
         for (int ch = 0; ch < 3; ++ch) {
 #define SHC(k) (sh[3 * (k) + ch])
             float r = 0.5f + SHC(0) * SH_C0;
+            if constexpr (K > 1) {
             r = r - SHC(1) * SH_C1 * y;
             r = r + SHC(2) * SH_C1 * z;
             r = r - SHC(3) * SH_C1 * x;
+            }
+            if constexpr (K > 4) {
             r = r + SHC(4) * SH_C2_0 * xy;
             r = r - SHC(5) * SH_C2_1 * yz;
             r = r + SHC(6) * SH_C2_2 * (2.0f * zz - xx - yy);
             r = r - SHC(7) * SH_C2_3 * xz;
+            }
 #undef SHC
             col[ch] = r;
         }
     }
-    {
+    if constexpr (K > 8) {
         float sh[24];
 #pragma unroll
-        for (int k = 0; k < 6; ++k) {
+        for (int k = 0; k < P - 6; ++k) {
             const float4 v = FROM_SMEM ? src[(uint64_t)(6 + k) * stride] : __ldg(src + (uint64_t)(6 + k) * stride);
             sh[4 * k + 0] = v.x; sh[4 * k + 1] = v.y; sh[4 * k + 2] = v.z; sh[4 * k + 3] = v.w;
         }
@@ -153,6 +163,7 @@ __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, flo
 #define SHC(k) (sh[3 * ((k) - 8) + ch])
             float r = col[ch];
             r = r + SHC(8) * SH_C2_4 * (xx - yy);
+            if constexpr (K > 9) {
             r = r - SHC(9) * SH_C3_0 * y * (3.0f * xx - yy);
             r = r + SHC(10) * SH_C3_1 * x * yz;
             r = r - SHC(11) * SH_C3_2 * y * (4.0f * zz - xx - yy);
@@ -160,9 +171,16 @@ __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, flo
             r = r - SHC(13) * SH_C3_4 * x * (4.0f * zz - xx - yy);
             r = r + SHC(14) * SH_C3_5 * z * (xx - yy);
             r = r - SHC(15) * SH_C3_6 * x * (xx - 3.0f * yy);
+            }
 #undef SHC
-            col[ch] = g_max(0.0f, r);
+            if constexpr (K == sh_coeffs(SH_BANDS_MAX)) col[ch] = g_max(0.0f, r);
+            else col[ch] = r;
         }
+    }
+    if constexpr (K < sh_coeffs(SH_BANDS_MAX)) {
+        const float skip = 0.0f * ((x + y) + z);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) col[ch] = g_max(0.0f, col[ch] + skip);
     }
 }
 
@@ -328,7 +346,7 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
 //            warp's 32 splats) into the warp's shared slab and everybody waits on the warp's mbarrier;
 //            cull + EWA + rect => duplicate count; the last warp of the CTA to get here publishes the CTA
 //            aggregate, before phase 2, so that successor CTAs never wait on this CTA's colour work;
-//   phase 2: if at least `sh_bulk_min` lanes emit keys, twelve more 512-byte bulk copies bring the SH planes
+//   phase 2: if at least `sh_bulk_min` lanes emit keys, twelve more 512-byte bulk copies (P = sh_planes(SH_BANDS)) bring the SH planes
 //            (6 KB in flight per warp at zero register cost); otherwise the few live lanes gather their
 //            192 bytes with plain 128-bit loads (sparse view / out-of-band warps of a multi-GPU shard);
 //   then records are written, the closer's look-back resolves the CTA's base offset, and every warp emits its keys.
@@ -338,6 +356,11 @@ constexpr int PROJ_WARPS = PROJ_THREADS / 32;
 #endif
 constexpr size_t PROJ_SLAB_BYTES = sizeof(float4) * NUM_PLANES * 32;             // 7680 B per warp
 constexpr size_t PROJ_SMEM_BYTES = PROJ_SLAB_BYTES * PROJ_WARPS;                // 61440 B per CTA
+
+// the per-warp slab of a kernel that keeps planes 0-2 and `sh_bands` bands of SH planes (PROJ_SLAB_BYTES at 4 bands).  Used in place, never
+// as a local constant: even an unused local declaration changes the default kernel's SASS.
+__host__ __device__ constexpr size_t proj_slab_bytes(int sh_bands) { return sizeof(float4) * (size_t)soa_planes(sh_bands) * 32u; }
+static_assert(proj_slab_bytes(SH_BANDS_MAX) == PROJ_SLAB_BYTES, "the degree-3 slab");
 
 // Instanced warp: its instance k, first source splat, live lanes and the bytes of one plane slice (0 for a padding warp of the last CTA).
 struct InstanceWarp { uint32_t k; uint64_t src0; uint32_t live, slice_bytes; };
@@ -360,7 +383,9 @@ __device__ __forceinline__ InstanceWarp instance_warp(const ProjectionArgs &a, c
 // drawn warp warp0_k + j projects source splats first_k + 32 j + lane (lanes past count_k are dead) with the instance's V_k / cam_k and
 // writes record, key and value at its drawn id.  Everything after the projection -- scan, emit, sort, compositor -- is unchanged.
 // The default instantiation (INSTANCED = false) compiles to the same instruction stream as the kernel before instancing existed.
-template <bool INSTANCED = false>
+// SH_BANDS (gsr_set_sh_degree, reduced stores): phase 2 brings only the first sh_planes(SH_BANDS) SH planes, and the warp's slab holds
+// soa_planes(SH_BANDS) planes.  Every degree-only difference is a constant or an `if constexpr`: SH_BANDS = 4 is the degree-3 kernel.
+template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX>
 __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
                                                                                        const __grid_constant__ InstanceArgs ia = InstanceArgs()) {
 #ifndef GSR_CPU_EMU
@@ -379,7 +404,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     __shared__ uint32_t s_ncomp;
 
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    float4 *slab = reinterpret_cast<float4 *>(proj_smem + (size_t)warp * PROJ_SLAB_BYTES);  // [15][32]
+    float4 *slab = reinterpret_cast<float4 *>(proj_smem + (size_t)warp * proj_slab_bytes(SH_BANDS));  // [SOA_PLANES][32]
     if (lane == 0) {
         mbar_init(&s_bar[warp][0], 1);
         mbar_init(&s_bar[warp][1], 1);
@@ -463,13 +488,13 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         const uint32_t nsurv = s_ncomp;
         if (tid < nsurv) {
             const uint32_t li = s_list[tid];
-            const float4 *sl = reinterpret_cast<const float4 *>(proj_smem + (size_t)(li >> 5) * PROJ_SLAB_BYTES);
+            const float4 *sl = reinterpret_cast<const float4 *>(proj_smem + (size_t)(li >> 5) * proj_slab_bytes(SH_BANDS));
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
             if (project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
                 float col[3];
-                sh_color<false>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
+                sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
                 rec[0] = o.r0; rec[1] = o.r1; rec[2] = make_float4(col[0], col[1], col[2], o.opacity);
                 s_res[li] = make_uint4(o.n, o.x0 | (o.y0 << 16), o.w | (o.depth << 16), (uint32_t)o.last_tile);
@@ -513,13 +538,13 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     if (bulk && lane == 0) {
         if constexpr (INSTANCED) {   // nvis > 0: a live warp, slice_bytes > 0
             const InstanceWarp iw = instance_warp(a, ia, vwarp);
-            mbar_expect_tx(&s_bar[warp][1], 12u * iw.slice_bytes);
+            mbar_expect_tx(&s_bar[warp][1], (uint32_t)sh_planes(SH_BANDS) * iw.slice_bytes);
 #pragma unroll
-            for (int k = 3; k < NUM_PLANES; ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + iw.src0, iw.slice_bytes, &s_bar[warp][1]);
+            for (int k = 3; k < soa_planes(SH_BANDS); ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + iw.src0, iw.slice_bytes, &s_bar[warp][1]);
         } else {
-        mbar_expect_tx(&s_bar[warp][1], 12u * 512u);
+        mbar_expect_tx(&s_bar[warp][1], (uint32_t)sh_planes(SH_BANDS) * 512u);
 #pragma unroll
-        for (int k = 3; k < NUM_PLANES; ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + id0, 512u, &s_bar[warp][1]);
+        for (int k = 3; k < soa_planes(SH_BANDS); ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + id0, 512u, &s_bar[warp][1]);
         }
     }
     if (closer) {
@@ -544,14 +569,14 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         mbar_wait(&s_bar[warp][1], 0);
         if (n) {
             float col[3];
-            sh_color<true>(slab + 3 * 32 + lane, 32, vx, vy, vz, col);
+            sh_color<true, SH_BANDS>(slab + 3 * 32 + lane, 32, vx, vy, vz, col);
             float4 *rec = a.records + (uint64_t)id * 3u;
             rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
         }
     } else if (n && !colour_done) {
         float col[3];
-        if constexpr (INSTANCED) sh_color<false>(a.soa + 3ull * a.plane_stride + instance_warp(a, ia, vwarp).src0 + lane, a.plane_stride, vx, vy, vz, col);
-        else sh_color<false>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
+        if constexpr (INSTANCED) sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + instance_warp(a, ia, vwarp).src0 + lane, a.plane_stride, vx, vy, vz, col);
+        else sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
         float4 *rec = a.records + (uint64_t)id * 3u;
         rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
     }
@@ -1074,6 +1099,18 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 #ifndef GSR_CPU_EMU  // host side: CUDA only
 // Force-load this file's kernels (CUDA loads modules lazily; a first launch that has to load code while another context's
 // kernel spins on a flag this launch would satisfy can stall the host: see gsr_group_attach).
+// dynamic shared memory of projection_kernel<*, B>: the slabs of its eight warps
+constexpr size_t projection_smem_bytes(int sh_bands) { return proj_slab_bytes(sh_bands) * PROJ_WARPS; }
+static_assert(projection_smem_bytes(SH_BANDS_MAX) == PROJ_SMEM_BYTES, "the degree-3 slab");
+
+template <bool INSTANCED, int B>
+int preload_projection_variant() {
+    cudaFuncAttributes fa;
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)projection_smem_bytes(B)));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B>));
+    return GSR_OK;
+}
+
 int preload_projection_kernels() {
     cudaFuncAttributes fa;
     // dynamic shared memory opt-in is a per-device function attribute: set here, once per context creation, on the context's device
@@ -1086,6 +1123,11 @@ int preload_projection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_scatter_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, instance_prepare_kernel));
+    // the lower-degree variants (gsr_set_sh_degree, reduced stores): a frame may switch to one at any time
+    int rc;
+    if ((rc = preload_projection_variant<false, 1>()) || (rc = preload_projection_variant<false, 2>()) || (rc = preload_projection_variant<false, 3>()) ||
+        (rc = preload_projection_variant<true, 1>()) || (rc = preload_projection_variant<true, 2>()) || (rc = preload_projection_variant<true, 3>()))
+        return rc;
     return GSR_OK;
 }
 uint32_t projection_scatter_blocks(uint32_t count) { return count ? (count + PROJ_THREADS - 1) / PROJ_THREADS : 1u; }   // an empty slice still publishes its flags
@@ -1099,7 +1141,7 @@ int launch_projection_scatter(const ProjectionArgs &frame_args, const ScatterPee
     return GSR_OK;
 }
 
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream) {
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
     if (a.fast_reject) {  // sharded variant: 1024 splats per CTA
@@ -1108,15 +1150,25 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream) {
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }
-    projection_kernel<<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a);
+    switch (sh_bands) {   // (the sharded variant above reads a degree-3 store: reduced degrees are single-context only)
+        case 1: projection_kernel<false, 1><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a); break;
+        case 2: projection_kernel<false, 2><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a); break;
+        case 3: projection_kernel<false, 3><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a); break;
+        default: projection_kernel<<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a); break;
+    }
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }
 
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream) {
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    projection_kernel<true><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia);
+    switch (sh_bands) {
+        case 1: projection_kernel<true, 1><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia); break;
+        case 2: projection_kernel<true, 2><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia); break;
+        case 3: projection_kernel<true, 3><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia); break;
+        default: projection_kernel<true><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia); break;
+    }
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }

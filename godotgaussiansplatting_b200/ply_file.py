@@ -12,6 +12,8 @@ code evaluates them, so the result is bit-identical to the C oracle's restatemen
 """
 from __future__ import annotations
 
+from dataclasses import dataclass
+
 import numpy as np
 
 STRUCT_SIZE = 60  # floats (util/ply_file.gd:29)
@@ -68,6 +70,66 @@ class PlyFile:
     def table(self) -> np.ndarray:
         return self.vertices.reshape(self.size, len(self.properties))
 
+    def layout(self) -> "PlyLayout":
+        """Where each property group sits in a vertex, and the file's SH degree, from the property names (include/gsr.h
+        gsr_ply_layout).  Normals and extra properties are allowed anywhere; every group must be contiguous and in order."""
+        names = list(self.properties)
+        pos = {n: i for i, n in enumerate(names)}
+
+        def group(first_names):
+            missing = [n for n in first_names if n not in pos]
+            if missing:
+                raise ValueError(f"PLY has no {', '.join(missing)} property")
+            at = pos[first_names[0]]
+            if [pos[n] for n in first_names] != list(range(at, at + len(first_names))):
+                raise ValueError(f"PLY properties {first_names[0]}..{first_names[-1]} are not contiguous")
+            return at
+
+        n_rest = sum(1 for n in names if n.startswith("f_rest_"))
+        if n_rest not in SH_REST_FLOATS:
+            raise ValueError(f"PLY has {n_rest} f_rest properties; an SH degree 0..3 file has 0, 9, 24 or 45")
+        degree = SH_REST_FLOATS.index(n_rest)
+        return PlyLayout(nprops=len(names), sh_degree=degree, x=group(["x", "y", "z"]), f_dc=group([f"f_dc_{i}" for i in range(3)]),
+                         f_rest=group([f"f_rest_{i}" for i in range(n_rest)]) if n_rest else -1, opacity=group(["opacity"]),
+                         scale=group([f"scale_{i}" for i in range(3)]), rot=group([f"rot_{i}" for i in range(4)]))
+
+
+SH_REST_FLOATS = (0, 9, 24, 45)   # f_rest floats of an SH degree 0..3 file: 3 * ((degree + 1)^2 - 1)
+
+
+@dataclass(frozen=True)
+class PlyLayout:
+    """include/gsr.h gsr_ply_layout: index of x (y, z follow), f_dc_0, f_rest_0 (-1 iff degree 0), opacity, scale_0, rot_0."""
+    nprops: int
+    sh_degree: int
+    x: int
+    f_dc: int
+    f_rest: int
+    opacity: int
+    scale: int
+    rot: int
+
+
+PLY_LAYOUT_3DGS = PlyLayout(nprops=62, sh_degree=3, x=0, f_dc=6, f_rest=9, opacity=54, scale=55, rot=58)   # the original 3DGS trainer's
+
+
+def degree_properties(sh_degree: int, normals: bool = True, extra: tuple = ()) -> list[str]:
+    """Property names of a 3DGS PLY of SH degree `sh_degree` (the trainer's order), optionally without nx ny nz, plus `extra` names."""
+    names = ["x", "y", "z"] + (["nx", "ny", "nz"] if normals else []) + ["f_dc_0", "f_dc_1", "f_dc_2"]
+    names += [f"f_rest_{i}" for i in range(SH_REST_FLOATS[sh_degree])]
+    names += ["opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"]
+    return names + list(extra)
+
+
+def narrow_table(table62: np.ndarray, sh_degree: int, normals: bool = True) -> np.ndarray:
+    """The vertex table of degree `sh_degree` (degree_properties order) that holds the coefficients of a standard 62-property table up to
+    that degree: the table a lower-degree PLY of the same splats holds.  Its coefficients above the degree are dropped."""
+    t = np.asarray(table62, dtype=np.float32)
+    k = SH_REST_FLOATS[sh_degree] // 3
+    rest = t[:, 9:54].reshape(-1, 3, 15)[:, :, :k].reshape(t.shape[0], 3 * k)
+    cols = [t[:, 0:3]] + ([t[:, 3:6]] if normals else []) + [t[:, 6:9], rest, t[:, 54:62]]
+    return np.ascontiguousarray(np.concatenate(cols, axis=1), dtype=np.float32)
+
 
 def default_properties(nprops: int = 62) -> list[str]:
     names = ["x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2"] + [f"f_rest_{i}" for i in range(45)]
@@ -84,16 +146,18 @@ def _basis_mul(a, b):
     return o
 
 
-def swizzle_splats(p: np.ndarray, creation_time: float) -> np.ndarray:
-    """util/ply_file.gd:41-69 for a block of vertices. p: (m, nprops>=62) float32 -> (m, 60) float32."""
+def swizzle_splats(p: np.ndarray, creation_time: float, layout: PlyLayout | None = None) -> np.ndarray:
+    """util/ply_file.gd:41-69 for a block of vertices. p: (m, nprops) float32 -> (m, 60) float32.  layout: PlyFile.layout() of the
+    table (default: the standard 62-property layout); SH coefficients above the file's degree are zero."""
     p = np.asarray(p, dtype=np.float32)
+    L = layout or PLY_LAYOUT_3DGS
     m = p.shape[0]
     out = np.zeros((m, STRUCT_SIZE), dtype=np.float32)
-    out[:, 0:3] = p[:, 0:3]
+    out[:, 0:3] = p[:, L.x:L.x + 3]
     out[:, 3] = F(creation_time)
     # exp() is a GDScript float (float64); narrowed when stored in Vector3 (real_t = float32)
-    sc = [np.exp(p[:, 55 + k].astype(np.float64)).astype(np.float32) for k in range(3)]
-    qx, qy, qz, qw = p[:, 59], p[:, 60], p[:, 61], p[:, 58]  # Quaternion(rot_1, rot_2, rot_3, rot_0)
+    sc = [np.exp(p[:, L.scale + k].astype(np.float64)).astype(np.float32) for k in range(3)]
+    qx, qy, qz, qw = p[:, L.rot + 1], p[:, L.rot + 2], p[:, L.rot + 3], p[:, L.rot]  # Quaternion(rot_1, rot_2, rot_3, rot_0)
     d = ((qx * qx + qy * qy) + qz * qz) + qw * qw
     s = F(2.0) / d
     xs, ys, zs = qx * s, qy * s, qz * s
@@ -111,15 +175,17 @@ def swizzle_splats(p: np.ndarray, creation_time: float) -> np.ndarray:
     out[:, 4], out[:, 5], out[:, 6] = Cv[0][0], Cv[0][1], Cv[0][2]
     out[:, 7], out[:, 8], out[:, 9] = Cv[1][1], Cv[1][2], Cv[2][2]
     with np.errstate(over="ignore"):
-        out[:, 10] = (1.0 / (1.0 + np.exp(-p[:, 54].astype(np.float64)))).astype(np.float32)
-    out[:, 12:15] = p[:, 6:9]
-    rest = p[:, 9:54].reshape(m, 3, 15)  # channel-major in the file
-    out[:, 15:60] = rest.transpose(0, 2, 1).reshape(m, 45)  # coefficient-major RGB
+        out[:, 10] = (1.0 / (1.0 + np.exp(-p[:, L.opacity].astype(np.float64)))).astype(np.float32)
+    out[:, 12:15] = p[:, L.f_dc:L.f_dc + 3]
+    k = SH_REST_FLOATS[L.sh_degree] // 3
+    if k:
+        rest = p[:, L.f_rest:L.f_rest + 3 * k].reshape(m, 3, k)  # channel-major in the file
+        out[:, 15:15 + 3 * k] = rest.transpose(0, 2, 1).reshape(m, 3 * k)  # coefficient-major RGB
     return out
 
 
 def load_gaussian_splats(point_cloud: PlyFile, stride: int, upload, should_terminate=None, num_points_loaded=None,
-                         callback=None, clock=None) -> None:
+                         callback=None, clock=None, layout: PlyLayout | None = None) -> None:
     """util/ply_file.gd:28-77.  `upload(first_splat, block60)` plays the role of device.buffer_update
     (:71); `clock()` returns seconds (Time.get_ticks_msec()*1e-3, :40) and stamps each chunk."""
     assert stride >= 1, "stride must be >= 1 (the reference requires size >= 1000)"
@@ -130,7 +196,7 @@ def load_gaussian_splats(point_cloud: PlyFile, stride: int, upload, should_termi
         if should_terminate is not None and should_terminate[0]:
             return
         lo, hi = i * stride, min(n, (i + 1) * stride)
-        block = swizzle_splats(table[lo:hi], clock() if clock else 0.0)
+        block = swizzle_splats(table[lo:hi], clock() if clock else 0.0, layout)
         if should_terminate is not None and should_terminate[0]:
             return
         upload(lo, block)

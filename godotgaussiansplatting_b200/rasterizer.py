@@ -19,7 +19,7 @@ import numpy as np
 
 from . import _lib
 from .camera import Camera3D, pack_camera_push_constants, transform_to_projection
-from .ply_file import PlyFile, load_gaussian_splats
+from .ply_file import PlyFile, PlyLayout, load_gaussian_splats
 
 TILE_SIZE = 16            # rasterizer.gd:4
 WORKGROUP_SIZE = 512      # rasterizer.gd:5
@@ -46,7 +46,9 @@ class RenderTexture:
 
 class GaussianSplattingRasterizer:
     def __init__(self, point_cloud: PlyFile, output_texture_size, render_texture: RenderTexture | None, camera: Camera3D,
-                 device: int = 0, flags: int = 0, dup_capacity_factor: int = 10, clock=None):
+                 device: int = 0, flags: int = 0, dup_capacity_factor: int = 10, clock=None, sh_bands: int | None = None):
+        """sh_bands: SH bands the context stores (gsr_config.sh_bands, 1..4 = degree + 1); None = the file's degree + 1, or 4 when its
+        properties do not name a 3DGS layout."""
         self.should_enable_heatmap = [False]
         self.render_scale = [1.0]
         self.model_scale = [1.0]
@@ -57,6 +59,11 @@ class GaussianSplattingRasterizer:
         self.loaded_callbacks = []  # signal `loaded`
         self._ctx = C.c_void_p(None)
         self._device, self._flags, self._factor = device, flags, dup_capacity_factor
+        try:
+            self._layout = point_cloud.layout()
+        except ValueError:
+            self._layout = None   # not a named 3DGS layout: the standard 62-property order, as the reference reads it
+        self._sh_bands = int(sh_bands) if sh_bands is not None else (self._layout.sh_degree + 1 if self._layout else 0)
         self._clock = clock or (lambda: _time.monotonic())
         self._t0 = self._clock()
         self.tile_dims = (0, 0)
@@ -100,7 +107,7 @@ class GaussianSplattingRasterizer:
         device_ingest=True runs the per-splat preprocessing of ply_file.gd:44-69 on the GPU instead of in numpy."""
         assert self.render_texture is not None, "An output Texture2DRD must be set!"
         L = _lib.lib()
-        cfg = _lib.GsrConfig(self._device, self._flags, max(1, self.point_cloud.size), self._factor, 0)
+        cfg = _lib.GsrConfig(self._device, self._flags, max(1, self.point_cloud.size), self._factor, self._sh_bands)
         _lib.check(L.gsr_create(C.byref(cfg), C.byref(self._ctx)), "gsr_create")
         w, h = self._texture_size
         _lib.check(L.gsr_resize(self._ctx, w, h), "gsr_resize")
@@ -115,12 +122,15 @@ class GaussianSplattingRasterizer:
             table, n, i = self.point_cloud.table, self.point_cloud.size, 0
             while i * stride < n and not self.should_terminate_thread[0]:
                 lo, hi = i * stride, min(n, (i + 1) * stride)
-                self.upload_ply_raw(table[lo:hi], lo, self.ticks())
+                if self._layout is None:
+                    self.upload_ply_raw(table[lo:hi], lo, self.ticks())
+                else:
+                    self.upload_ply(table[lo:hi], self._layout, lo, self.ticks())
                 i += 1
             self._emit_loaded()
             return
         load_gaussian_splats(self.point_cloud, stride, self._upload, self.should_terminate_thread, self.num_splats_loaded,
-                             self._emit_loaded, clock=self.ticks)
+                             self._emit_loaded, clock=self.ticks, layout=self._layout)
 
     def _upload(self, first: int, block60: np.ndarray) -> None:
         block60 = np.ascontiguousarray(block60, dtype=np.float32)
@@ -142,6 +152,22 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_upload_ply_raw(self._ctx, t.ctypes.data_as(C.POINTER(C.c_float)), t.shape[1], first, t.shape[0],
                                                  float(creation_time)), "gsr_upload_ply_raw")
         self.num_splats_loaded[0] = max(self.num_splats_loaded[0], first + t.shape[0])
+
+    def upload_ply(self, table: np.ndarray, layout: PlyLayout, first: int = 0, creation_time: float = 0.0) -> None:
+        """Device-side ingest of PLY vertices of any SH degree and property order (include/gsr.h gsr_upload_ply); layout: PlyFile.layout()."""
+        if not self._ctx:
+            raise RuntimeError("init_gpu() first")
+        t = np.ascontiguousarray(table, dtype=np.float32)
+        lay = _lib.GsrPlyLayout(layout.nprops, layout.sh_degree, layout.x, layout.f_dc, layout.f_rest, layout.opacity, layout.scale, layout.rot)
+        assert t.ndim == 2 and t.shape[1] == layout.nprops, (t.shape, layout.nprops)
+        _lib.check(_lib.lib().gsr_upload_ply(self._ctx, t.ctypes.data_as(C.POINTER(C.c_float)), C.byref(lay), first, t.shape[0],
+                                             float(creation_time)), "gsr_upload_ply")
+        self.num_splats_loaded[0] = max(self.num_splats_loaded[0], first + t.shape[0])
+
+    def set_sh_degree(self, degree: int) -> None:
+        """SH degree of the colour of the frames rendered from now on (include/gsr.h gsr_set_sh_degree): 0 .. the stored degree, -1 = the
+        stored degree (the default).  A lower degree trades view-dependent colour for projection bytes."""
+        _lib.check(_lib.lib().gsr_set_sh_degree(self._ctx, int(degree)), "gsr_set_sh_degree")
 
     def _emit_loaded(self):
         self.is_loaded = True

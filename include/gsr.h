@@ -66,8 +66,10 @@ enum {
     GSR_BUF_FRAMEBUFFER = 6,  /* RGBA32F W*H (descriptors['render_texture']) */
     GSR_BUF_COMPOSITOR_TRACE = 7,       /* schedule trace of the last frame's compositor (gsr_debug_enable_trace) */
     GSR_BUF_COMPOSITOR_TRACE_COUNT = 8, /* number of trace items written (uint32) */
-    GSR_BUF_INSTANCES = 9               /* gsr_set_instances: 24 floats per instance, to_frame as given then the library's inverse
+    GSR_BUF_INSTANCES = 9,              /* gsr_set_instances: 24 floats per instance, to_frame as given then the library's inverse
                                            [A^-1 | -A^-1 t] rounded to float (both 3x4, column-major) */
+    GSR_BUF_SPLATS = 10                 /* the stored splat planes, plane-major: (3 + P) x plane_stride float4, plane_stride = max_splats
+                                           rounded up to 256 (gsr_config.sh_bands) */
 };
 
 typedef struct gsr_ctx gsr_ctx;       /* one rasterizer = one GaussianSplattingRasterizer instance */
@@ -78,7 +80,10 @@ typedef struct gsr_config {
     uint32_t flags;               /* GSR_FLAG_*; 0 = GSR_FLAG_REFERENCE_QUIRKS */
     uint64_t max_splats;          /* point_cloud.size (rasterizer.gd:79,83) */
     uint32_t dup_capacity_factor; /* initial sort capacity = factor * max_splats; 0 -> 10 (rasterizer.gd:79); grows on demand */
-    uint32_t reserved;
+    uint32_t sh_bands;            /* SH bands the context stores = SH degree + 1: 1 (DC only) .. 4 (degree 3); 0 -> 4.  The splat buffer holds
+                                     3 + P float4 planes per splat, P = ceil(3 B^2 / 4) = 1, 3, 7, 12: 64 / 96 / 160 / 240 bytes.  Uploads drop
+                                     the coefficients the store does not keep.  > 4: GSR_ERR_INVALID.  A store of fewer than 4 bands is
+                                     single-context only (see gsr_set_sh_degree). */
 } gsr_config;
 
 typedef struct gsr_stats {
@@ -129,6 +134,20 @@ GSR_API int gsr_upload_splats_aos(gsr_ctx *ctx, const float *splat60, uint64_t f
  * PlyFile.load_gaussian_splats (util/ply_file.gd:44-69: exp(scale), quaternion -> R, Sigma = R S^2 R^T, sigmoid(opacity),
  * SH re-interleave) runs on the device and writes the SoA planes directly; `creation_time` stamps the chunk (:40,47). */
 GSR_API int gsr_upload_ply_raw(gsr_ctx *ctx, const float *ply, uint32_t nprops, uint64_t first, uint64_t count, float creation_time);
+
+/* Same, for PLY vertices of any SH degree and property order (DC-only exports, degree-1 and degree-2 trainings, files without the
+ * nx ny nz normals, extra properties): `layout` names where each group sits in a vertex of `nprops` floats.  f_rest holds
+ * 3 * ((sh_degree + 1)^2 - 1) floats, channel-major (R.., G.., B..) as the 3DGS trainer writes them.  Coefficients above the file's
+ * degree are stored as zero, those above the store's (gsr_config.sh_bands) are dropped.  The preprocessing is that of
+ * gsr_upload_ply_raw, which is this call with the standard layout {62, 3, 0, 6, 9, 54, 55, 58}.  GSR_ERR_INVALID: a NULL layout,
+ * nprops outside 1..256, sh_degree > 3, a group that does not fit inside nprops, f_rest >= 0 with sh_degree 0 or < 0 with
+ * sh_degree > 0, or an upload range beyond max_splats. */
+typedef struct gsr_ply_layout {
+    uint32_t nprops;     /* floats per vertex, 1..256 */
+    uint32_t sh_degree;  /* of the file, 0..3 */
+    int32_t x, f_dc, f_rest, opacity, scale, rot;  /* index of x (y, z follow), f_dc_0, f_rest_0 (-1 iff degree 0), opacity, scale_0, rot_0 */
+} gsr_ply_layout;
+GSR_API int gsr_upload_ply(gsr_ctx *ctx, const float *ply, const gsr_ply_layout *layout, uint64_t first, uint64_t count, float creation_time);
 
 /* ---- texture_size setter (rasterizer.gd:26-48): reallocates tile_bounds + render_texture ---- */
 GSR_API int gsr_resize(gsr_ctx *ctx, int32_t width, int32_t height);
@@ -289,6 +308,16 @@ typedef struct gsr_instance {
     float to_frame[12];     /* [A | t], column-major 3x4 */
 } gsr_instance;
 GSR_API int gsr_set_instances(gsr_ctx *ctx, const gsr_instance *instances, uint32_t n);
+
+/* ---- SH degree of the rendered colour (no reference counterpart: the reference always evaluates degree 3).  Frames enqueued after
+ *      the call evaluate the view-dependent colour up to `degree` (0 = the DC colour only) from the first P = ceil(3 (degree+1)^2 / 4)
+ *      SH planes, so a lower degree also reads fewer bytes.  -1 = the stored degree (gsr_config.sh_bands - 1), the default.  The degree
+ *      is read when a frame is enqueued: frames already enqueued keep theirs, and the call never synchronises.  A frame drawn at
+ *      degree d is bit for bit the frame of the same cloud with every coefficient above degree d set to zero (DESIGN.md section 5.9).
+ *      GSR_ERR_INVALID: a degree below -1 or above the stored one.  A degree below 3, like a store of fewer than 4 bands, is
+ *      single-context only: GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those calls
+ *      (and gsr_group_export) fail with GSR_ERR_STATE on such a store or while a degree below 3 is set. ---- */
+GSR_API int gsr_set_sh_degree(gsr_ctx *ctx, int32_t degree);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
