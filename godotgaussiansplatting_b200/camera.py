@@ -3,9 +3,12 @@
 * `perspective` restates Godot 4.3 `Projection::set_perspective` (engine source not vendored in the
   reference; stated from knowledge of Godot 4.x) -- what `Camera3D.get_camera_projection()` returns
   for the defaults fov 75, near 0.05, far 4000, keep_aspect = KEEP_HEIGHT (main.tscn:36-38).
-* `pack_camera_push_constants` follows util/gaussian_splatting_rasterizer.gd:175-195 literally.
+* `orthogonal` restates Godot 4 `Projection::set_orthogonal(size, aspect, near, far, flip_fov)` the same way (not executed in
+  Godot here; libgsr accepts any matrix, so parity does not depend on matching the engine's last bit).
+* `pack_camera_push_constants` follows util/gaussian_splatting_rasterizer.gd:175-195 literally; with keep_w_row=True it packs the
+  projection's w row as given (what a GSR_FLAG_ORTHOGRAPHIC context needs to see an orthographic camera).
 * `Camera3D` mirrors the handful of members the rasterizer touches (global_position,
-  get_camera_transform, get_camera_projection); `reset()` follows util/camera.gd:151-153.
+  get_camera_transform, get_camera_projection, projection / size / keep_aspect); `reset()` follows util/camera.gd:151-153.
 * `orbit_camera` generates the 1-degree-per-frame orbit of BASELINE.json config c3 (SURVEY 8d).
 """
 from __future__ import annotations
@@ -33,6 +36,27 @@ def perspective(fovy_degrees: float, aspect: float, z_near: float, z_far: float)
     return m.reshape(16)
 
 
+def orthogonal(size: float, aspect: float, z_near: float, z_far: float, flip_fov: bool = False) -> np.ndarray:
+    """Godot Projection columns x,y,z,w flattened (16 float32, column-major) of Projection::set_orthogonal(size, aspect, near, far,
+    flip_fov): `size` is the view's height (flip_fov False, KEEP_HEIGHT) or width (flip_fov True, KEEP_WIDTH) in world units.
+    real_t is float; the engine's double literals (2.0) make those quotients double, rounded to float when stored."""
+    size, aspect = F(size), F(aspect)
+    if not flip_fov:
+        size = size * aspect
+    left, right = -size / F(2), size / F(2)
+    bottom, top = -size / aspect / F(2), size / aspect / F(2)
+    z_near, z_far = F(z_near), F(z_far)
+    m = np.zeros((4, 4), dtype=np.float32)  # m[c][r]; set_identity first
+    m[0][0] = F(2.0 / float(right - left))
+    m[3][0] = -((right + left) / (right - left))
+    m[1][1] = F(2.0 / float(top - bottom))
+    m[3][1] = -((top + bottom) / (top - bottom))
+    m[2][2] = F(-2.0 / float(z_far - z_near))
+    m[3][2] = -((z_far + z_near) / (z_far - z_near))
+    m[3][3] = F(1.0)
+    return m.reshape(16)
+
+
 def transform_to_projection(basis_cols: np.ndarray, origin: np.ndarray) -> np.ndarray:
     """Godot Projection(Transform3D): columns (x,0),(y,0),(z,0),(origin,1)."""
     m = np.zeros((4, 4), dtype=np.float32)
@@ -42,8 +66,10 @@ def transform_to_projection(basis_cols: np.ndarray, origin: np.ndarray) -> np.nd
     return m.reshape(16)
 
 
-def pack_camera_push_constants(view16: np.ndarray, proj16: np.ndarray) -> np.ndarray:
-    """util/gaussian_splatting_rasterizer.gd:181-193 -> 32 float32 (view_matrix, projection_matrix)."""
+def pack_camera_push_constants(view16: np.ndarray, proj16: np.ndarray, keep_w_row: bool = False) -> np.ndarray:
+    """util/gaussian_splatting_rasterizer.gd:181-193 -> 32 float32 (view_matrix, projection_matrix).  The reference overwrites the
+    projection's w row with (0, 0, -1, 0); keep_w_row=True packs it as given.  Perspective and frustum matrices have that w row, so
+    both give the same bytes for them; an orthographic matrix keeps its (0, 0, 0, 1) (include/gsr.h GSR_FLAG_ORTHOGRAPHIC)."""
     v = np.asarray(view16, dtype=np.float32).reshape(4, 4)
     p = np.asarray(proj16, dtype=np.float32).reshape(4, 4)
     x, y, z, w = v[0], v[1], v[2], v[3]
@@ -60,6 +86,8 @@ def pack_camera_push_constants(view16: np.ndarray, proj16: np.ndarray) -> np.nda
         p[1][0], p[1][1], p[1][2], 0.0,
         p[2][0], p[2][1], p[2][2], -1.0,
         p[3][0], p[3][1], p[3][2], 0.0], dtype=np.float32)
+    if keep_w_row:
+        out[[19, 23, 27, 31]] = p[:, 3]
     return out
 
 
@@ -68,11 +96,18 @@ def _normalize(v):
     return v / np.linalg.norm(v)
 
 
-class Camera3D:
-    """Minimal stand-in for Godot's Camera3D as used by the rasterizer (fov/near/far defaults of the engine)."""
+PROJECTION_PERSPECTIVE, PROJECTION_ORTHOGONAL = 0, 1   # Camera3D.ProjectionType (PROJECTION_FRUSTUM = 2 is not mirrored)
+KEEP_WIDTH, KEEP_HEIGHT = 0, 1                          # Camera3D.KeepAspect
 
-    def __init__(self, fov: float = 75.0, near: float = 0.05, far: float = 4000.0):
+
+class Camera3D:
+    """Minimal stand-in for Godot's Camera3D as used by the rasterizer (fov/near/far/size defaults of the engine).  keep_aspect applies to
+    the orthographic projection; the perspective one is the KEEP_HEIGHT matrix of the reference's scene."""
+
+    def __init__(self, fov: float = 75.0, near: float = 0.05, far: float = 4000.0, projection: int = PROJECTION_PERSPECTIVE,
+                 size: float = 1.0, keep_aspect: int = KEEP_HEIGHT):
         self.fov, self.near, self.far = float(fov), float(near), float(far)
+        self.projection, self.size, self.keep_aspect = int(projection), float(size), int(keep_aspect)
         self.basis = np.eye(3, dtype=np.float32)  # rows of this array are the basis COLUMNS x, y, z
         self.global_position = np.zeros(3, dtype=np.float32)
         self.aspect = 16.0 / 9.0
@@ -99,6 +134,8 @@ class Camera3D:
         return transform_to_projection(self.basis, self.global_position)
 
     def get_camera_projection(self) -> np.ndarray:
+        if self.projection == PROJECTION_ORTHOGONAL:
+            return orthogonal(self.size, self.aspect, self.near, self.far, flip_fov=self.keep_aspect == KEEP_WIDTH)
         return perspective(self.fov, self.aspect, self.near, self.far)
 
 

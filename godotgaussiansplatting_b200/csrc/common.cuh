@@ -163,8 +163,9 @@ struct ProjectionArgs {
     unsigned long long *lookback;  // one word per projection CTA (256 splats)
     FrameState *frame;
 };
-// sh_bands: SH bands the frame evaluates (1..4, at most the store's); the kernel reads planes 0-2 and the first sh_planes(sh_bands) SH planes
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX);
+// sh_bands: SH bands the frame evaluates (1..4, at most the store's); the kernel reads planes 0-2 and the first sh_planes(sh_bands) SH planes.
+// ortho: the frame's projection is orthographic (GSR_FLAG_ORTHOGRAPHIC; decided on the host at enqueue time, single-context only)
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false);
 
 // ---------------------------------------------------------------------------------------------
 // splat instances (gsr_set_instances): ranges of the splat buffer drawn with their own affine transform into frame space
@@ -183,7 +184,7 @@ struct InstanceArgs {
     const uint32_t *warp_inst;              // instance of every drawn warp of the grid; 0xFFFFFFFF = padding warp
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX);
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false);
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
 // (mapped page-locked host memory on the frame path)
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream);

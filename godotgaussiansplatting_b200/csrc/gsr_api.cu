@@ -617,18 +617,32 @@ static GroupPeers group_peers(const gsr_ctx *c, int parity) {
     return p;
 }
 
+// GSR_FLAG_ORTHOGRAPHIC: whether the frame takes the orthographic projection path (its projection's w row is exactly (0, 0, 0, 1)), and
+// GSR_ERR_STATE when it does on a context that is not single-context (checked before anything of the frame is enqueued).
+static int frame_is_orthographic(const gsr_ctx *c, const float *view_proj, bool *ortho) {
+    *ortho = (c->flags & GSR_FLAG_ORTHOGRAPHIC) && view_proj[19] == 0.0f && view_proj[23] == 0.0f && view_proj[27] == 0.0f && view_proj[31] == 1.0f;
+    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
+    if (*ortho && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
+        set_last_error("orthographic frame: single-context only (no group, peer framebuffers, partial band or row interleave)");
+        return GSR_ERR_STATE;
+    }
+    return GSR_OK;
+}
+
 static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *uniforms32, float heatmap_factor, float4 *target = nullptr,
                           const GroupFrame *gf = nullptr) {
     if (!c || !view_proj || !uniforms32) return GSR_ERR_INVALID;
     if (c->width == 0) { set_last_error("gsr_render before gsr_resize"); return GSR_ERR_STATE; }
+    bool ortho = false;
+    int rc = frame_is_orthographic(c, view_proj, &ortho);
+    if (rc) return rc;
     Uniforms u;
     memcpy(&u, uniforms32, sizeof u);
     if (u.dims[0] != c->width || u.dims[1] != c->height) {
         set_last_error("uniform dims %dx%d differ from gsr_resize %dx%d", u.dims[0], u.dims[1], c->width, c->height);
         return GSR_ERR_INVALID;
     }
-    int rc = use_device(c->device);
-    if (rc) return rc;
+    if ((rc = use_device(c->device))) return rc;
     if ((rc = track_capacity(c))) return rc;
     cudaStream_t s = c->stream;
     // Front / back overlap.  The front part of a frame (clear + projection: HBM-bound) needs nothing from the frame before it, the back
@@ -730,10 +744,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         InstanceArgs ia;
         ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
         ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
-        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c)))) return rc;
+        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho))) return rc;
         launches += pa.num_splats ? 1 : 0;
     } else {
-        if ((rc = launch_projection(pa, fs, render_bands(c)))) return rc;
+        if ((rc = launch_projection(pa, fs, render_bands(c), ortho))) return rc;
         launches += pa.num_splats ? 1 : 0;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[1], fs));  // end of the front part
@@ -880,6 +894,11 @@ static int readback_enqueue(gsr_ctx *c, float4 *frame, int slot, void *pinned_ho
 
 static int render_async_impl(gsr_ctx *c, const float *view_proj, const void *uniforms32, float heatmap_factor, void *pinned_host, int format) {
     if (!c) return GSR_ERR_INVALID;
+    if (view_proj) {   // an orthographic frame on a sharded context enqueues nothing (the group and peer paths below enqueue waits before the frame)
+        bool ortho = false;
+        const int rc = frame_is_orthographic(c, view_proj, &ortho);
+        if (rc) return rc;
+    }
     if (c->grp.world > 1) {   // shard group: every rank enqueues the same frame; rows land in the presenting rank's frames
         if (pinned_host) { set_last_error("group mode: render with a NULL host pointer on every rank, then gsr_readback_async on rank 0"); return GSR_ERR_STATE; }
         int rc = use_device(c->device);

@@ -196,7 +196,11 @@ struct LaneOut {  // what one splat contributes (valid when n > 0)
 // V (16 floats) and cam (3) stand for the view matrix and uniforms.camera_pos: the frame's own (a.vp, a.u.camera_pos), or an
 // instance's V_k = V * M_k and cam_k = M_k^-1 * camera_pos (instance_prepare_kernel).  INST: `At` is the instance's A|t (12 floats,
 // column-major) and the record's position words hold the FRAME-space position A * sp + t instead of sp.
-template <bool QUICK, bool INST = false>
+// ORTHO (GSR_FLAG_ORTHOGRAPHIC, a projection whose w row is (0, 0, 0, 1)): the cull keeps the whole [near, far] slab (clip.z in
+// [-w, w]), the EWA Jacobian is the constant diag(focal_base) (no depth divide, no mean clamp, no z terms in b), every splat is seen
+// along the camera's forward axis (-V[2], -V[6], -V[10]) and the depth key is linear in view depth (DESIGN.md section 5.10).  Every
+// orthographic difference is an `if constexpr` or a constant condition: ORTHO = false is the perspective lane as it always was.
+template <bool QUICK, bool INST = false, bool ORTHO = false>
 __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const float *V, const float *cam, const float *At, const float4 pt,
                                              const float4 ca, const float4 cb, LaneOut &o) {
     const float *P = a.vp + 16;  // X[c][r] = X[4*c + r]
@@ -212,7 +216,11 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
 #pragma unroll
             for (int r = 0; r < 4; ++r) clip[r] = ((P[0 + r] * view[0] + P[4 + r] * view[1]) + P[8 + r] * view[2]) + P[12 + r] * view[3];
             const float vb = clip[3] * 1.2f;
+            if constexpr (ORTHO) {   // the full [near, far] slab: clip.z in [-w, w]
+                if (clip[0] < -vb || clip[1] < -vb || clip[2] < -clip[3] || clip[0] > vb || clip[1] > vb || clip[2] > clip[3]) return false;
+            } else {
             if (clip[0] < -vb || clip[1] < -vb || clip[2] < 0.0f || clip[0] > vb || clip[1] > vb || clip[2] > clip[3]) return false;
+            }
 
 
             // :169-174 load-in animation
@@ -224,7 +232,8 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
 
             // per-frame constants (focal = dims*0.5*tan_fov_inv, +-tan_fov*1.3) are evaluated once on the host with
             // the same IEEE operations (ProjectionArgs::focal_base, lim_lo, lim_hi)
-            const float z_inv = 1.0f / view[2];
+            // (orthographic: focal = focal_base exactly -- x * 1.0f is x -- and mx, my are unused)
+            const float z_inv = ORTHO ? 1.0f : 1.0f / view[2];
             const float focal0 = a.focal_base[0] * z_inv, focal1 = a.focal_base[1] * z_inv;
             const float mx = g_clamp(view[0] * z_inv, a.lim_lo[0], a.lim_hi[0]);
             const float my = g_clamp(view[1] * z_inv, a.lim_lo[1], a.lim_hi[1]);
@@ -232,7 +241,7 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             const float ipx = ((ndc0 + 1.0f) * 0.5f - 1.0f * (1.0f - tf)) * (float)(W - 1);
             const float ipy = ((ndc1 + 1.0f) * 0.5f - 0.75f * (1.0f - tf)) * (float)(H - 1);
 
-            if (a.fast_reject) {
+            if (!ORTHO && a.fast_reject) {   // (orthographic frames are single-context only: never sharded)
                 // Sharded fast mode: a CONSERVATIVE radius decides whether the splat can touch a tile row this context
                 // owns; if not, the exact math below would end in "nt == 0" anyway.  With e1 <= trace(cov_2d) + 0.32,
                 // trace(J W S' W^T J^T) <= lambda_max(S') |J|_F^2 |W|_2^2 <= |S'|_F |J|_F^2 |W|_2^2 and pow(op, 0.2) <= max(1, op):
@@ -267,8 +276,13 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             float B0[3], B1[3];
 #pragma unroll
             for (int r = 0; r < 3; ++r) {
+                if constexpr (ORTHO) {   // the Jacobian's z column is structurally zero too
+                    B0[r] = V[4 * r + 0] * focal0;
+                    B1[r] = V[4 * r + 1] * focal1;
+                } else {
                 B0[r] = V[4 * r + 0] * focal0 + V[4 * r + 2] * j02;
                 B1[r] = V[4 * r + 1] * focal1 + V[4 * r + 2] * j12;
+                }
             }
             // t1 = transpose(b) * cov_3d: T0[c] = t1[c][0] = sum_k b[0][k]*cov3[c][k], T1[c] = t1[c][1]
             float T0[3], T1[3];
@@ -333,8 +347,16 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             o.r0.x = ipx; o.r0.y = ipy; o.r0.z = sp0; o.r0.w = sp1;                        // image_pos, pos_xy
             o.r1.x = cz / det; o.r1.y = -cy / det; o.r1.z = cx / det; o.r1.w = sp2;        // conic, pos_z
             }
+            if constexpr (ORTHO) {   // the view direction is the camera's forward axis in the splat's frame (the one above is dead code here)
+                const float f0 = -V[2], f1 = -V[6], f2 = -V[10];
+                const float inv_len = 1.0f / sqrtf((f0 * f0 + f1 * f1) + f2 * f2);
+                o.vx = f0 * inv_len; o.vy = f1 * inv_len; o.vz = f2 * inv_len;
+                // linear in view depth across [near, far]: the cubic key of :218 would crowd the near half into a few bins
+                o.depth = ((uint32_t)(g_clamp(ndc2 * 0.5f + 0.5f, 0.0f, 1.0f) * 65535.0f)) & 0xFFFFu;
+            } else {
             // :218
             o.depth = ((uint32_t)(ndc2 * ndc2 * ndc2 * 65535.0f)) & 0xFFFFu;
+            }
             o.n = nt; o.x0 = (uint32_t)x0; o.y0 = (uint32_t)y0; o.w = (uint32_t)(x1 - x0);
 
     return true;
@@ -385,7 +407,8 @@ __device__ __forceinline__ InstanceWarp instance_warp(const ProjectionArgs &a, c
 // The default instantiation (INSTANCED = false) compiles to the same instruction stream as the kernel before instancing existed.
 // SH_BANDS (gsr_set_sh_degree, reduced stores): phase 2 brings only the first sh_planes(SH_BANDS) SH planes, and the warp's slab holds
 // soa_planes(SH_BANDS) planes.  Every degree-only difference is a constant or an `if constexpr`: SH_BANDS = 4 is the degree-3 kernel.
-template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX>
+// ORTHO (GSR_FLAG_ORTHOGRAPHIC): every lane runs project_lane<.., ORTHO>; nothing else of the kernel changes.
+template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false>
 __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
                                                                                        const __grid_constant__ InstanceArgs ia = InstanceArgs()) {
 #ifndef GSR_CPU_EMU
@@ -454,7 +477,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             // the instance's constants: V_k (16) | cam_k (3) | A_k | t_k (12), 128 B that every lane of the warp reads (L1 broadcasts)
             const float *sk = ia.frame + (size_t)iw.k * INSTANCE_FRAME_FLOATS;
             LaneOut o;
-            if (project_lane<false, true>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false, true, ORTHO>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -463,7 +486,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     } else if (!a.fast_reject) {
         if (id < a.num_splats) {
             LaneOut o;
-            if (project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false, false, ORTHO>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -477,7 +500,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         //      slot, so scan and emit below are unchanged and the emission order stays the splat-id order).
         bool live = false;
         LaneOut q;
-        if (id < a.num_splats) live = project_lane<true>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q);
+        if (id < a.num_splats) live = project_lane<true, false, ORTHO>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q);
         s_res[tid] = make_uint4(0u, 0u, 0u, 0xFFFFFFFFu);
         const uint32_t lmask = __ballot_sync(0xffffffffu, live);
         uint32_t wbase = 0;
@@ -492,7 +515,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
-            if (project_lane<false>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
+            if (project_lane<false, false, ORTHO>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
                 float col[3];
                 sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
@@ -1103,11 +1126,19 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 constexpr size_t projection_smem_bytes(int sh_bands) { return proj_slab_bytes(sh_bands) * PROJ_WARPS; }
 static_assert(projection_smem_bytes(SH_BANDS_MAX) == PROJ_SMEM_BYTES, "the degree-3 slab");
 
-template <bool INSTANCED, int B>
+template <bool INSTANCED, int B, bool ORTHO = false>
 int preload_projection_variant() {
     cudaFuncAttributes fa;
-    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)projection_smem_bytes(B)));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B>));
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)projection_smem_bytes(B)));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO>));
+    return GSR_OK;
+}
+template <bool INSTANCED>
+int preload_projection_ortho() {
+    int rc;
+    if ((rc = preload_projection_variant<INSTANCED, 1, true>()) || (rc = preload_projection_variant<INSTANCED, 2, true>()) ||
+        (rc = preload_projection_variant<INSTANCED, 3, true>()) || (rc = preload_projection_variant<INSTANCED, 4, true>()))
+        return rc;
     return GSR_OK;
 }
 
@@ -1128,6 +1159,8 @@ int preload_projection_kernels() {
     if ((rc = preload_projection_variant<false, 1>()) || (rc = preload_projection_variant<false, 2>()) || (rc = preload_projection_variant<false, 3>()) ||
         (rc = preload_projection_variant<true, 1>()) || (rc = preload_projection_variant<true, 2>()) || (rc = preload_projection_variant<true, 3>()))
         return rc;
+    // the orthographic variants (GSR_FLAG_ORTHOGRAPHIC): any frame may be orthographic
+    if ((rc = preload_projection_ortho<false>()) || (rc = preload_projection_ortho<true>())) return rc;
     return GSR_OK;
 }
 uint32_t projection_scatter_blocks(uint32_t count) { return count ? (count + PROJ_THREADS - 1) / PROJ_THREADS : 1u; }   // an empty slice still publishes its flags
@@ -1141,9 +1174,25 @@ int launch_projection_scatter(const ProjectionArgs &frame_args, const ScatterPee
     return GSR_OK;
 }
 
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands) {
+// projection_kernel<INSTANCED, B, true> for B = sh_bands (the orthographic frames: single-context only, never sharded)
+template <bool INSTANCED>
+void launch_projection_ortho(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t blocks, cudaStream_t stream, int sh_bands) {
+    switch (sh_bands) {
+        case 1: projection_kernel<INSTANCED, 1, true><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia); break;
+        case 2: projection_kernel<INSTANCED, 2, true><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia); break;
+        case 3: projection_kernel<INSTANCED, 3, true><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia); break;
+        default: projection_kernel<INSTANCED, SH_BANDS_MAX, true><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia); break;
+    }
+}
+
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
+    if (ortho) {
+        launch_projection_ortho<false>(a, InstanceArgs(), blocks, stream, sh_bands);
+        GSR_CUDA_TRY(cudaGetLastError());
+        return GSR_OK;
+    }
     if (a.fast_reject) {  // sharded variant: 1024 splats per CTA
         const uint32_t sblocks = (a.num_splats + SH_SPLATS - 1) / SH_SPLATS;
         projection_sharded_kernel<<<sblocks, PROJ_THREADS, SH_SLAB_BYTES, stream>>>(a);
@@ -1160,9 +1209,14 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
     return GSR_OK;
 }
 
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands) {
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
+    if (ortho) {
+        launch_projection_ortho<true>(a, ia, blocks, stream, sh_bands);
+        GSR_CUDA_TRY(cudaGetLastError());
+        return GSR_OK;
+    }
     switch (sh_bands) {
         case 1: projection_kernel<true, 1><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia); break;
         case 2: projection_kernel<true, 2><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia); break;

@@ -339,7 +339,9 @@ class GaussianSplattingRasterizer:
         if (self.camera_transform is None or not np.array_equal(view, self.camera_transform)
                 or not np.array_equal(proj, self.camera_projection)):
             self.camera_transform, self.camera_projection = view, proj
-            self.camera_push_constants = pack_camera_push_constants(view, proj)
+            # a GSR_FLAG_ORTHOGRAPHIC context sees the projection's own w row (the reference packing forces the perspective one);
+            # for perspective and frustum matrices both give the same bytes
+            self.camera_push_constants = pack_camera_push_constants(view, proj, keep_w_row=bool(self._flags & _lib.GSR_FLAG_ORTHOGRAPHIC))
             return True
         return False
 

@@ -55,6 +55,18 @@ enum {
                                             contraction the frame is bit-identical to the reference's own shader text executed on the CPU
                                             (oracle/_ref; oracle.set_blend_contraction(False)). */
 
+#define GSR_FLAG_ORTHOGRAPHIC 0x20u /* render orthographic cameras (Godot Camera3D.PROJECTION_ORTHOGONAL).  On a context created with this
+                                      flag, a frame whose projection's w row is exactly (0, 0, 0, 1) -- view_proj[19] == 0, [23] == 0,
+                                      [27] == 0, [31] == 1, what Godot's Projection::set_orthogonal gives -- takes the orthographic
+                                      projection path: the cull keeps the whole [near, far] slab, the EWA Jacobian has no depth divide,
+                                      the SH view direction is the camera's forward axis, and the 16-bit depth key is linear in view
+                                      depth, t = clamp(ndc.z * 0.5 + 0.5, 0, 1), key = uint(t * 65535).  It resolves depth to
+                                      (far - near) / 65536: set near / far around the content.  Every other frame (perspective and
+                                      frustum matrices, anything the reference's packing produces: it writes (0, 0, -1, 0)) takes the
+                                      perspective path unchanged.  The choice is made per frame when it is enqueued, without a sync.
+                                      Single-context only: an orthographic frame on a context with a shard group, peer framebuffers, a
+                                      partial band or row interleave returns GSR_ERR_STATE and enqueues nothing. */
+
 /* ---- gsr_debug_copy selectors (parity taps; not on the frame path) ---- */
 enum {
     GSR_BUF_RECORDS = 0, /* 48 B RasterizeData per splat id (gsplat_projection.glsl:42-48), max_splats entries */
