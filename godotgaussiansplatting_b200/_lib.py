@@ -23,7 +23,7 @@ EXPORTS = [
     "gsr_create", "gsr_destroy", "gsr_set_stream", "gsr_upload_splats_aos", "gsr_upload_ply_raw", "gsr_upload_ply", "gsr_resize", "gsr_set_band", "gsr_set_row_interleave", "gsr_band_sync_word", "gsr_band_fixup", "gsr_render",
     "gsr_render_async", "gsr_render_async_rgb", "gsr_render_async_fmt", "gsr_output_bytes", "gsr_present_device", "gsr_readback_async", "gsr_peer_export_framebuffers", "gsr_peer_import_framebuffers",
     "gsr_stream_join", "gsr_group_export", "gsr_group_attach", "gsr_group_detach", "gsr_group_set_present", "gsr_readback_rows_async", "gsr_sync", "gsr_framebuffer_device_ptr", "gsr_set_framebuffer_external",
-    "gsr_set_depth_compositing", "gsr_set_instances", "gsr_set_sh_degree", "gsr_pick",
+    "gsr_set_depth_compositing", "gsr_set_instances", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_upload_ply_filtered", "gsr_pick",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -86,6 +86,7 @@ def lib():
         L.gsr_upload_splats_aos.argtypes = [vp, fp, C.c_uint64, C.c_uint64]
         L.gsr_upload_ply_raw.argtypes = [vp, fp, u32, C.c_uint64, C.c_uint64, C.c_float]
         L.gsr_upload_ply.argtypes = [vp, fp, C.POINTER(GsrPlyLayout), C.c_uint64, C.c_uint64, C.c_float]
+        L.gsr_upload_ply_filtered.argtypes = [vp, fp, C.POINTER(GsrPlyLayout), C.c_int32, C.c_uint64, C.c_uint64, C.c_float]
         L.gsr_resize.argtypes = [vp, C.c_int32, C.c_int32]
         L.gsr_set_band.argtypes = [vp, C.c_int32, C.c_int32]
         L.gsr_set_row_interleave.argtypes = [vp, C.c_int32, C.c_int32]
@@ -115,6 +116,7 @@ def lib():
         L.gsr_set_depth_compositing.argtypes = [vp, vp, vp]
         L.gsr_set_instances.argtypes = [vp, C.POINTER(GsrInstance), u32]
         L.gsr_set_sh_degree.argtypes = [vp, C.c_int32]
+        L.gsr_set_antialiasing.argtypes = [vp, C.c_float]
         L.gsr_pick.argtypes = [vp, u32, C.c_float, fp]
         L.gsr_get_stats.argtypes = [vp, C.POINTER(GsrStats)]
         L.gsr_get_frame_history.argtypes = [vp, u32, C.POINTER(GsrFrameRecord), C.POINTER(u32)]

@@ -1,6 +1,7 @@
 // common.cuh -- shared declarations of libgsr (sm_90a).  Product code: never includes anything from oracle/.
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 #include <stdio.h>
 
@@ -160,12 +161,16 @@ struct ProjectionArgs {
     float4 *records;         // 3 float4 per splat id (RasterizeData layout)
     uint32_t *keys, *values;
     uint32_t capacity;
+    float aa_variance;         // gsr_set_antialiasing: the 2D filter's variance (px^2); read only by the anti-aliased kernels.  It fills the
+                               // padding after `capacity`: the struct's size, and so the offset of the kernels' second parameter, is unchanged
     unsigned long long *lookback;  // one word per projection CTA (256 splats)
     FrameState *frame;
 };
+static_assert(sizeof(ProjectionArgs) == 288 && offsetof(ProjectionArgs, lookback) == 272, "ProjectionArgs keeps its layout");
 // sh_bands: SH bands the frame evaluates (1..4, at most the store's); the kernel reads planes 0-2 and the first sh_planes(sh_bands) SH planes.
 // ortho: the frame's projection is orthographic (GSR_FLAG_ORTHOGRAPHIC; decided on the host at enqueue time, single-context only)
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false);
+// aa: the frame is anti-aliased with a.aa_variance > 0 (gsr_set_antialiasing; read at enqueue time, single-context only)
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false, bool aa = false);
 
 // ---------------------------------------------------------------------------------------------
 // splat instances (gsr_set_instances): ranges of the splat buffer drawn with their own affine transform into frame space
@@ -184,7 +189,8 @@ struct InstanceArgs {
     const uint32_t *warp_inst;              // instance of every drawn warp of the grid; 0xFFFFFFFF = padding warp
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false);
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false,
+                                bool aa = false);
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
 // (mapped page-locked host memory on the frame path)
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream);
@@ -294,8 +300,9 @@ int launch_tile_order(const uint2 *bounds, int32_t tile_begin, int32_t row_step,
 // The standard 62-property layout of the original 3DGS trainer (x y z nx ny nz f_dc_0..2 f_rest_0..44 opacity scale_0..2 rot_0..3).
 constexpr gsr_ply_layout PLY_LAYOUT_3DGS = {62u, 3u, 0, 6, 9, 54, 55, 58};
 // PLY vertices of any layout -> the first `planes` (= soa_planes(store bands)) SoA planes
+// filter_3d: index of Mip-Splatting's per-splat `filter_3D` property in a vertex (gsr_upload_ply_filtered), -1 = none
 int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
-                      uint64_t first, int planes, cudaStream_t stream);
+                      uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d = -1);
 // present.cu: RGBA32F frame -> GSR_OUT_* (| GSR_OUT_SRGB_TO_LINEAR)
 int launch_present(const float4 *rgba, void *out, uint64_t pixels, int format, cudaStream_t stream);
 size_t present_bytes_per_pixel(int format);

@@ -41,6 +41,7 @@ struct gsr_ctx {
     float4 *soa = nullptr;       // soa_planes(sh_bands) planes x plane_stride (15 for a degree-3 store)
     int sh_bands = SH_BANDS_MAX; // SH bands the store keeps (gsr_config.sh_bands)
     int sh_degree = -1;          // render degree (gsr_set_sh_degree); -1 = the stored degree
+    float aa_variance = 0.0f;    // anti-aliasing filter of the next frames (gsr_set_antialiasing); 0 = off
     float4 *records = nullptr;   // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -388,7 +389,8 @@ GSR_API int gsr_upload_splats_aos(gsr_ctx *c, const float *splat60, uint64_t fir
     return GSR_OK;
 }
 
-static int upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout &lay, uint64_t first, uint64_t count, float creation_time) {
+static int upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout &lay, uint64_t first, uint64_t count, float creation_time,
+                      int32_t filter_3d = -1) {
     if (count > c->max_splats || first > c->max_splats - count) { set_last_error("upload range [%llu,%llu) exceeds max_splats %llu", (unsigned long long)first, (unsigned long long)(first + count), (unsigned long long)c->max_splats); return GSR_ERR_INVALID; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -402,7 +404,7 @@ static int upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout &lay, u
         const uint64_t m = (count - done) < per ? (count - done) : per;
         GSR_CUDA_TRY(cudaMemcpyAsync(c->staging, ply + done * nprops, m * nprops * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         if ((rc = launch_ply_to_soa(reinterpret_cast<const float *>(c->staging), lay, m, creation_time, c->soa, c->plane_stride, first + done,
-                                    soa_planes(c->sh_bands), c->stream))) return rc;
+                                    soa_planes(c->sh_bands), c->stream, filter_3d))) return rc;
         done += m;
     }
     GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -418,8 +420,7 @@ GSR_API int gsr_upload_ply_raw(gsr_ctx *c, const float *ply, uint32_t nprops, ui
     return upload_ply(c, ply, lay, first, count, creation_time);
 }
 
-GSR_API int gsr_upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout *layout, uint64_t first, uint64_t count, float creation_time) {
-    if (!c || (!ply && count)) return GSR_ERR_INVALID;
+static int check_ply_layout(const gsr_ply_layout *layout) {
     if (!layout) { set_last_error("gsr_upload_ply: NULL layout"); return GSR_ERR_INVALID; }
     const gsr_ply_layout &L = *layout;
     if (L.nprops < 1 || L.nprops > 256) { set_last_error("gsr_upload_ply: nprops %u outside 1..256", L.nprops); return GSR_ERR_INVALID; }
@@ -435,7 +436,26 @@ GSR_API int gsr_upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout *l
             return GSR_ERR_INVALID;
         }
     }
-    return upload_ply(c, ply, L, first, count, creation_time);
+    return GSR_OK;
+}
+
+GSR_API int gsr_upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout *layout, uint64_t first, uint64_t count, float creation_time) {
+    if (!c || (!ply && count)) return GSR_ERR_INVALID;
+    const int rc = check_ply_layout(layout);
+    if (rc) return rc;
+    return upload_ply(c, ply, *layout, first, count, creation_time);
+}
+
+GSR_API int gsr_upload_ply_filtered(gsr_ctx *c, const float *ply, const gsr_ply_layout *layout, int32_t filter_3d, uint64_t first, uint64_t count,
+                                    float creation_time) {
+    if (!c || (!ply && count)) return GSR_ERR_INVALID;
+    const int rc = check_ply_layout(layout);
+    if (rc) return rc;
+    if (filter_3d < -1 || filter_3d >= (int32_t)layout->nprops) {
+        set_last_error("gsr_upload_ply_filtered: filter_3d %d outside -1..%u", filter_3d, layout->nprops - 1);
+        return GSR_ERR_INVALID;
+    }
+    return upload_ply(c, ply, *layout, first, count, creation_time, filter_3d);
 }
 
 GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
@@ -488,6 +508,7 @@ GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod)
     if (c->depth_out && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && row_mod > 1) { set_last_error("gsr_set_row_interleave: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (c->aa_variance > 0.0f && row_mod > 1) { set_last_error("gsr_set_row_interleave: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -510,6 +531,7 @@ GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (c->depth_out && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (c->aa_variance > 0.0f && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
     c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
     return GSR_OK;
@@ -718,6 +740,8 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     pa.sh_bulk_min = (fast || c->row_mod > 1) ? 1 : 12;
     pa.records = records; pa.keys = keys_in; pa.values = vals_in; pa.capacity = (uint32_t)c->capacity;
     pa.lookback = c->lookback; pa.frame = c->frame;
+    pa.aa_variance = c->aa_variance;   // read here: frames already enqueued keep their filter
+    const bool aa = c->aa_variance > 0.0f;
     if (gf) {
         // group mode: the projection is sharded by SPLATS.  This rank projects its slice and stores every pair and record into the
         // memory of the rank that owns it (peer stores over NVLink); the back part then waits for the other sources' flags and packs
@@ -744,10 +768,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         InstanceArgs ia;
         ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
         ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
-        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho))) return rc;
+        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa))) return rc;
         launches += pa.num_splats ? 1 : 0;
     } else {
-        if ((rc = launch_projection(pa, fs, render_bands(c), ortho))) return rc;
+        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa))) return rc;
         launches += pa.num_splats ? 1 : 0;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[1], fs));  // end of the front part
@@ -1036,6 +1060,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (c->depth_out) { set_last_error("gsr_peer_export_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n) { set_last_error("gsr_peer_export_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_export_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -1053,6 +1078,7 @@ GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (c->depth_out) { set_last_error("gsr_peer_import_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n) { set_last_error("gsr_peer_import_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_import_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -1083,6 +1109,7 @@ GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
     if (!c || !blob) return GSR_ERR_INVALID;
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_group_export: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (c->aa_variance > 0.0f) { set_last_error("gsr_group_export: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     if (!c->grp.arena) {
@@ -1114,6 +1141,7 @@ GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void
     if (c->depth_out && world > 1) { set_last_error("gsr_group_attach: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && world > 1) { set_last_error("gsr_group_attach: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (c->aa_variance > 0.0f && world > 1) { set_last_error("gsr_group_attach: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1388,6 +1416,21 @@ GSR_API int gsr_set_sh_degree(gsr_ctx *c, int32_t degree) {
         return GSR_ERR_STATE;
     }
     c->sh_degree = degree;   // read by the next render_enqueue: frames already enqueued keep their degree
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_antialiasing(gsr_ctx *c, float filter_variance) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!(filter_variance >= 0.0f && filter_variance <= 64.0f)) {   // NaN fails both
+        set_last_error("gsr_set_antialiasing: filter variance %g outside 0..64 px^2", (double)filter_variance);
+        return GSR_ERR_INVALID;
+    }
+    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
+    if (filter_variance > 0.0f && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
+        set_last_error("gsr_set_antialiasing: single-context only (no group, peer framebuffers, partial band or row interleave)");
+        return GSR_ERR_STATE;
+    }
+    c->aa_variance = filter_variance;   // read by the next render_enqueue: frames already enqueued keep their filter
     return GSR_OK;
 }
 

@@ -49,9 +49,14 @@ __device__ __forceinline__ void godot_basis_mul(const float a[3][3], const float
 
 // `lay` names the property groups of a vertex (gsr_ply_layout; default: the standard 62-property layout) and `planes` = soa_planes(store
 // bands) the planes written.  SH coefficients above the file's degree are stored as 0, those above the store's degree are dropped.
+// FILTER3D (gsr_upload_ply_filtered): property `filter_3d` is Mip-Splatting's per-splat 3D filter f.  With f > 0 the splat is stored
+// with the filter folded in, in float64 and narrowed once: q_i = exp(scale_i)^2, q'_i = q_i + f*f, scale_i = sqrt(q'_i) and opacity =
+// sigmoid * sqrt((q_0 q_1 q_2) / (q'_0 q'_1 q'_2)).  f <= 0 or NaN: stored exactly as without the filter.
+template <bool FILTER3D = false>
 __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *__restrict__ ply, uint32_t nprops, uint64_t count, float creation_time,
                                                                   float4 *__restrict__ soa, uint64_t plane_stride, uint64_t first,
-                                                                  const gsr_ply_layout lay = PLY_LAYOUT_3DGS, int planes = NUM_PLANES) {
+                                                                  const gsr_ply_layout lay = PLY_LAYOUT_3DGS, int planes = NUM_PLANES,
+                                                                  int32_t filter_3d = -1) {
 #ifndef GSR_CPU_EMU
     extern __shared__ float s_v[];  // [INGEST_SPLATS][nprops]
 #else  // tests/kernel_emu (CPU logic pre-flight): nprops <= 256 (gsr_upload_ply rejects more)
@@ -67,7 +72,18 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
     const uint64_t id = first + s0 + threadIdx.x;
 
     const float *ps = p + lay.scale, *pr = p + lay.rot, *px = p + lay.x, *pd = p + lay.f_dc;
-    const float sc0 = (float)exp((double)ps[0]), sc1 = (float)exp((double)ps[1]), sc2 = (float)exp((double)ps[2]);
+    const double e0 = exp((double)ps[0]), e1 = exp((double)ps[1]), e2 = exp((double)ps[2]);
+    const double sigmoid = 1.0 / (1.0 + exp(-(double)p[lay.opacity]));
+    float sc0 = (float)e0, sc1 = (float)e1, sc2 = (float)e2, opacity = (float)sigmoid;
+    if constexpr (FILTER3D) {
+        const double f = (double)p[filter_3d];
+        if (f > 0.0) {
+            const double q0 = e0 * e0, q1 = e1 * e1, q2 = e2 * e2, ff = f * f;
+            const double g0 = q0 + ff, g1 = q1 + ff, g2 = q2 + ff;
+            sc0 = (float)sqrt(g0); sc1 = (float)sqrt(g1); sc2 = (float)sqrt(g2);
+            opacity = (float)(sigmoid * sqrt(((q0 * q1) * q2) / ((g0 * g1) * g2)));
+        }
+    }
     const float qx = pr[1], qy = pr[2], qz = pr[3], qw = pr[0];  // Quaternion(rot_1, rot_2, rot_3, rot_0)
     const float d = ((qx * qx + qy * qy) + qz * qz) + qw * qw;
     const float s = 2.0f / d;
@@ -88,7 +104,6 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
 #pragma unroll
         for (int c = 0; c < 3; ++c) Mt[r][c] = M[c][r];
     godot_basis_mul(Mt, M, Cv);
-    const float opacity = (float)(1.0 / (1.0 + exp(-(double)p[lay.opacity])));
 
     soa[0 * plane_stride + id] = make_float4(px[0], px[1], px[2], creation_time);
     soa[1 * plane_stride + id] = make_float4(Cv[0][0], Cv[0][1], Cv[0][2], Cv[1][1]);
@@ -120,17 +135,24 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
 // kernel spins on a flag this launch would satisfy can stall the host: see gsr_group_attach).
 int preload_ingest_kernels() {
     cudaFuncAttributes fa;
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel<false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel<true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, aos_to_soa_kernel));
     return GSR_OK;
 }
 int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
-                      uint64_t first, int planes, cudaStream_t stream) {
+                      uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d) {
     if (count == 0) return GSR_OK;
     const size_t smem = sizeof(float) * (size_t)INGEST_SPLATS * layout.nprops;
-    if (smem > 48 * 1024) GSR_CUDA_TRY(cudaFuncSetAttribute(ply_to_soa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const uint32_t blocks = (uint32_t)((count + INGEST_SPLATS - 1) / INGEST_SPLATS);
-    ply_to_soa_kernel<<<blocks, INGEST_SPLATS, smem, stream>>>(ply, layout.nprops, count, creation_time, soa, plane_stride, first, layout, planes);
+    if (filter_3d >= 0) {
+        if (smem > 48 * 1024) GSR_CUDA_TRY(cudaFuncSetAttribute(ply_to_soa_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ply_to_soa_kernel<true><<<blocks, INGEST_SPLATS, smem, stream>>>(ply, layout.nprops, count, creation_time, soa, plane_stride, first, layout, planes,
+                                                                         filter_3d);
+    } else {
+        if (smem > 48 * 1024) GSR_CUDA_TRY(cudaFuncSetAttribute(ply_to_soa_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ply_to_soa_kernel<false><<<blocks, INGEST_SPLATS, smem, stream>>>(ply, layout.nprops, count, creation_time, soa, plane_stride, first, layout, planes);
+    }
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }

@@ -200,7 +200,10 @@ struct LaneOut {  // what one splat contributes (valid when n > 0)
 // [-w, w]), the EWA Jacobian is the constant diag(focal_base) (no depth divide, no mean clamp, no z terms in b), every splat is seen
 // along the camera's forward axis (-V[2], -V[6], -V[10]) and the depth key is linear in view depth (DESIGN.md section 5.10).  Every
 // orthographic difference is an `if constexpr` or a constant condition: ORTHO = false is the perspective lane as it always was.
-template <bool QUICK, bool INST = false, bool ORTHO = false>
+// AA (gsr_set_antialiasing, v = a.aa_variance > 0): the 2D covariance is dilated by v instead of 0.3, and the splat's opacity is
+// multiplied by coef = sqrt(max(0.000025, det(cov_2d) / det(cov_2d + v I))) -- the compensated filter of anti-aliased trainings.  That
+// opacity drives both the radius and the record (DESIGN.md section 5.11).  AA = false is the lane as it always was.
+template <bool QUICK, bool INST = false, bool ORTHO = false, bool AA = false>
 __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const float *V, const float *cam, const float *At, const float4 pt,
                                              const float4 ca, const float4 cb, LaneOut &o) {
     const float *P = a.vp + 16;  // X[c][r] = X[4*c + r]
@@ -295,7 +298,8 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             const float c2_00 = (T0[0] * B0[0] + T0[1] * B0[1]) + T0[2] * B0[2];
             const float c2_01 = (T1[0] * B0[0] + T1[1] * B0[1]) + T1[2] * B0[2];
             const float c2_11 = (T1[0] * B1[0] + T1[1] * B1[1]) + T1[2] * B1[2];
-            const float cx = c2_00 + 0.3f, cy = c2_01, cz = c2_11 + 0.3f;
+            const float dil = AA ? a.aa_variance : 0.3f;   // (anti-aliased: the filter's variance)
+            const float cx = c2_00 + dil, cy = c2_01, cz = c2_11 + dil;
 
             // :177-182
             const float det = cx * cz - cy * cy;
@@ -304,11 +308,13 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             const float sq = sqrtf(g_max(0.1f, mid * mid - det));
             const float e1 = mid + 1.0f * sq, e2 = mid + -1.0f * sq;
             if (e1 < 0.0f || e2 < 0.0f) return false;
+            // anti-aliased: the opacity compensated for the filter's dilation, the splat's opacity from here on (g_max: NaN gives the floor)
+            const float opacity = AA ? splat_opacity * sqrtf(g_max(0.000025f, (c2_00 * c2_11 - c2_01 * c2_01) / det)) : splat_opacity;
 
             // :184-185 ndc / image_pos: computed above (same operations), before the early reject
 
             // :190-194
-            const float radius = det_pow(splat_opacity, 0.2f) * 2.5f * sqrtf(g_max(e1, e2));
+            const float radius = det_pow(opacity, 0.2f) * 2.5f * sqrtf(g_max(e1, e2));
             if (!(fabsf(ipx) <= 3.0e38f) || !(fabsf(ipy) <= 3.0e38f) || !(radius <= 3.0e38f)) return false;  // gsr spec: non-finite => culled
             const float fgx = (float)gx, fgy = (float)gy;
             int32_t x0 = (int32_t)g_clamp((ipx - radius) / 16.0f, 0.0f, fgx);
@@ -334,7 +340,7 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             if constexpr (INST) {   // frame-space position w = A * sp + t (what gsr_pick and depth compositing read)
                 const float d0 = sp0 - cam[0], d1 = sp1 - cam[1], d2 = sp2 - cam[2];
                 const float inv_len = 1.0f / sqrtf((d0 * d0 + d1 * d1) + d2 * d2);
-                o.vx = d0 * inv_len; o.vy = d1 * inv_len; o.vz = d2 * inv_len; o.opacity = splat_opacity;
+                o.vx = d0 * inv_len; o.vy = d1 * inv_len; o.vz = d2 * inv_len; o.opacity = opacity;
                 const float w0 = ((At[0] * sp0 + At[3] * sp1) + At[6] * sp2) + At[9];
                 const float w1 = ((At[1] * sp0 + At[4] * sp1) + At[7] * sp2) + At[10];
                 const float w2 = ((At[2] * sp0 + At[5] * sp1) + At[8] * sp2) + At[11];
@@ -343,7 +349,7 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             } else {   // (the frame's camera_pos is read from the grid constants as written here: the default SASS stays as it was)
             const float d0 = sp0 - a.u.camera_pos[0], d1 = sp1 - a.u.camera_pos[1], d2 = sp2 - a.u.camera_pos[2];
             const float inv_len = 1.0f / sqrtf((d0 * d0 + d1 * d1) + d2 * d2);
-            o.vx = d0 * inv_len; o.vy = d1 * inv_len; o.vz = d2 * inv_len; o.opacity = splat_opacity;
+            o.vx = d0 * inv_len; o.vy = d1 * inv_len; o.vz = d2 * inv_len; o.opacity = opacity;
             o.r0.x = ipx; o.r0.y = ipy; o.r0.z = sp0; o.r0.w = sp1;                        // image_pos, pos_xy
             o.r1.x = cz / det; o.r1.y = -cy / det; o.r1.z = cx / det; o.r1.w = sp2;        // conic, pos_z
             }
@@ -407,8 +413,9 @@ __device__ __forceinline__ InstanceWarp instance_warp(const ProjectionArgs &a, c
 // The default instantiation (INSTANCED = false) compiles to the same instruction stream as the kernel before instancing existed.
 // SH_BANDS (gsr_set_sh_degree, reduced stores): phase 2 brings only the first sh_planes(SH_BANDS) SH planes, and the warp's slab holds
 // soa_planes(SH_BANDS) planes.  Every degree-only difference is a constant or an `if constexpr`: SH_BANDS = 4 is the degree-3 kernel.
-// ORTHO (GSR_FLAG_ORTHOGRAPHIC): every lane runs project_lane<.., ORTHO>; nothing else of the kernel changes.
-template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false>
+// ORTHO (GSR_FLAG_ORTHOGRAPHIC) and AA (gsr_set_antialiasing): every lane runs project_lane<.., ORTHO, AA>; nothing else of the kernel
+// changes.
+template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false>
 __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
                                                                                        const __grid_constant__ InstanceArgs ia = InstanceArgs()) {
 #ifndef GSR_CPU_EMU
@@ -477,7 +484,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             // the instance's constants: V_k (16) | cam_k (3) | A_k | t_k (12), 128 B that every lane of the warp reads (L1 broadcasts)
             const float *sk = ia.frame + (size_t)iw.k * INSTANCE_FRAME_FLOATS;
             LaneOut o;
-            if (project_lane<false, true, ORTHO>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false, true, ORTHO, AA>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -486,7 +493,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     } else if (!a.fast_reject) {
         if (id < a.num_splats) {
             LaneOut o;
-            if (project_lane<false, false, ORTHO>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false, false, ORTHO, AA>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -500,7 +507,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         //      slot, so scan and emit below are unchanged and the emission order stays the splat-id order).
         bool live = false;
         LaneOut q;
-        if (id < a.num_splats) live = project_lane<true, false, ORTHO>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q);
+        if (id < a.num_splats) live = project_lane<true, false, ORTHO, AA>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q);
         s_res[tid] = make_uint4(0u, 0u, 0u, 0xFFFFFFFFu);
         const uint32_t lmask = __ballot_sync(0xffffffffu, live);
         uint32_t wbase = 0;
@@ -515,7 +522,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
-            if (project_lane<false, false, ORTHO>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
+            if (project_lane<false, false, ORTHO, AA>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
                 float col[3];
                 sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
@@ -1126,18 +1133,19 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 constexpr size_t projection_smem_bytes(int sh_bands) { return proj_slab_bytes(sh_bands) * PROJ_WARPS; }
 static_assert(projection_smem_bytes(SH_BANDS_MAX) == PROJ_SMEM_BYTES, "the degree-3 slab");
 
-template <bool INSTANCED, int B, bool ORTHO = false>
+template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false>
 int preload_projection_variant() {
     cudaFuncAttributes fa;
-    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)projection_smem_bytes(B)));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO>));
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)projection_smem_bytes(B)));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA>));
     return GSR_OK;
 }
-template <bool INSTANCED>
-int preload_projection_ortho() {
+// projection_kernel<INSTANCED, 1..4, ORTHO, AA>
+template <bool INSTANCED, bool ORTHO, bool AA = false>
+int preload_projection_bands() {
     int rc;
-    if ((rc = preload_projection_variant<INSTANCED, 1, true>()) || (rc = preload_projection_variant<INSTANCED, 2, true>()) ||
-        (rc = preload_projection_variant<INSTANCED, 3, true>()) || (rc = preload_projection_variant<INSTANCED, 4, true>()))
+    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA>()) ||
+        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA>()))
         return rc;
     return GSR_OK;
 }
@@ -1160,7 +1168,11 @@ int preload_projection_kernels() {
         (rc = preload_projection_variant<true, 1>()) || (rc = preload_projection_variant<true, 2>()) || (rc = preload_projection_variant<true, 3>()))
         return rc;
     // the orthographic variants (GSR_FLAG_ORTHOGRAPHIC): any frame may be orthographic
-    if ((rc = preload_projection_ortho<false>()) || (rc = preload_projection_ortho<true>())) return rc;
+    if ((rc = preload_projection_bands<false, true>()) || (rc = preload_projection_bands<true, true>())) return rc;
+    // the anti-aliased variants (gsr_set_antialiasing), perspective and orthographic: the next frame may switch to one at any time
+    if ((rc = preload_projection_bands<false, false, true>()) || (rc = preload_projection_bands<true, false, true>()) ||
+        (rc = preload_projection_bands<false, true, true>()) || (rc = preload_projection_bands<true, true, true>()))
+        return rc;
     return GSR_OK;
 }
 uint32_t projection_scatter_blocks(uint32_t count) { return count ? (count + PROJ_THREADS - 1) / PROJ_THREADS : 1u; }   // an empty slice still publishes its flags
@@ -1174,22 +1186,29 @@ int launch_projection_scatter(const ProjectionArgs &frame_args, const ScatterPee
     return GSR_OK;
 }
 
-// projection_kernel<INSTANCED, B, true> for B = sh_bands (the orthographic frames: single-context only, never sharded)
-template <bool INSTANCED>
-void launch_projection_ortho(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t blocks, cudaStream_t stream, int sh_bands) {
+// projection_kernel<INSTANCED, B, ORTHO, AA> for B = sh_bands (the orthographic and the anti-aliased frames: single-context only, never sharded)
+template <bool INSTANCED, bool ORTHO, bool AA>
+void launch_projection_bands(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t blocks, cudaStream_t stream, int sh_bands) {
     switch (sh_bands) {
-        case 1: projection_kernel<INSTANCED, 1, true><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia); break;
-        case 2: projection_kernel<INSTANCED, 2, true><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia); break;
-        case 3: projection_kernel<INSTANCED, 3, true><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia); break;
-        default: projection_kernel<INSTANCED, SH_BANDS_MAX, true><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia); break;
+        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia); break;
+        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia); break;
+        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia); break;
+        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia); break;
     }
 }
+template <bool INSTANCED>
+void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t blocks, cudaStream_t stream, int sh_bands, bool ortho,
+                               bool aa) {
+    if (!aa) launch_projection_bands<INSTANCED, true, false>(a, ia, blocks, stream, sh_bands);
+    else if (ortho) launch_projection_bands<INSTANCED, true, true>(a, ia, blocks, stream, sh_bands);
+    else launch_projection_bands<INSTANCED, false, true>(a, ia, blocks, stream, sh_bands);
+}
 
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho) {
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho) {
-        launch_projection_ortho<false>(a, InstanceArgs(), blocks, stream, sh_bands);
+    if (ortho || aa) {
+        launch_projection_special<false>(a, InstanceArgs(), blocks, stream, sh_bands, ortho, aa);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }
@@ -1209,11 +1228,11 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
     return GSR_OK;
 }
 
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho) {
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho) {
-        launch_projection_ortho<true>(a, ia, blocks, stream, sh_bands);
+    if (ortho || aa) {
+        launch_projection_special<true>(a, ia, blocks, stream, sh_bands, ortho, aa);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }

@@ -91,7 +91,8 @@ class PlyFile:
         degree = SH_REST_FLOATS.index(n_rest)
         return PlyLayout(nprops=len(names), sh_degree=degree, x=group(["x", "y", "z"]), f_dc=group([f"f_dc_{i}" for i in range(3)]),
                          f_rest=group([f"f_rest_{i}" for i in range(n_rest)]) if n_rest else -1, opacity=group(["opacity"]),
-                         scale=group([f"scale_{i}" for i in range(3)]), rot=group([f"rot_{i}" for i in range(4)]))
+                         scale=group([f"scale_{i}" for i in range(3)]), rot=group([f"rot_{i}" for i in range(4)]),
+                         filter_3d=pos.get("filter_3D", -1))
 
 
 SH_REST_FLOATS = (0, 9, 24, 45)   # f_rest floats of an SH degree 0..3 file: 3 * ((degree + 1)^2 - 1)
@@ -99,7 +100,8 @@ SH_REST_FLOATS = (0, 9, 24, 45)   # f_rest floats of an SH degree 0..3 file: 3 *
 
 @dataclass(frozen=True)
 class PlyLayout:
-    """include/gsr.h gsr_ply_layout: index of x (y, z follow), f_dc_0, f_rest_0 (-1 iff degree 0), opacity, scale_0, rot_0."""
+    """include/gsr.h gsr_ply_layout: index of x (y, z follow), f_dc_0, f_rest_0 (-1 iff degree 0), opacity, scale_0, rot_0; and
+    filter_3d, the index of Mip-Splatting's `filter_3D` property or -1 (the filter_3d argument of gsr_upload_ply_filtered)."""
     nprops: int
     sh_degree: int
     x: int
@@ -108,6 +110,7 @@ class PlyLayout:
     opacity: int
     scale: int
     rot: int
+    filter_3d: int = -1
 
 
 PLY_LAYOUT_3DGS = PlyLayout(nprops=62, sh_degree=3, x=0, f_dc=6, f_rest=9, opacity=54, scale=55, rot=58)   # the original 3DGS trainer's
@@ -148,7 +151,8 @@ def _basis_mul(a, b):
 
 def swizzle_splats(p: np.ndarray, creation_time: float, layout: PlyLayout | None = None) -> np.ndarray:
     """util/ply_file.gd:41-69 for a block of vertices. p: (m, nprops) float32 -> (m, 60) float32.  layout: PlyFile.layout() of the
-    table (default: the standard 62-property layout); SH coefficients above the file's degree are zero."""
+    table (default: the standard 62-property layout); SH coefficients above the file's degree are zero.  A layout with filter_3d >= 0
+    folds Mip-Splatting's 3D filter into scale and opacity with the float64 operations of gsr_upload_ply_filtered."""
     p = np.asarray(p, dtype=np.float32)
     L = layout or PLY_LAYOUT_3DGS
     m = p.shape[0]
@@ -156,7 +160,20 @@ def swizzle_splats(p: np.ndarray, creation_time: float, layout: PlyLayout | None
     out[:, 0:3] = p[:, L.x:L.x + 3]
     out[:, 3] = F(creation_time)
     # exp() is a GDScript float (float64); narrowed when stored in Vector3 (real_t = float32)
-    sc = [np.exp(p[:, L.scale + k].astype(np.float64)).astype(np.float32) for k in range(3)]
+    with np.errstate(over="ignore"):
+        e = [np.exp(p[:, L.scale + k].astype(np.float64)) for k in range(3)]
+        sigmoid = 1.0 / (1.0 + np.exp(-p[:, L.opacity].astype(np.float64)))
+    opacity = sigmoid.astype(np.float32)
+    if L.filter_3d >= 0:   # Mip-Splatting: q'_i = exp(scale_i)^2 + f^2 for the splats with f > 0
+        f = p[:, L.filter_3d].astype(np.float64)
+        on = f > 0.0
+        with np.errstate(over="ignore", under="ignore", invalid="ignore"):
+            q = [ek * ek for ek in e]
+            g = [qk + f * f for qk in q]
+            coef = np.sqrt(((q[0] * q[1]) * q[2]) / ((g[0] * g[1]) * g[2]))
+            e = [np.where(on, np.sqrt(gk), ek) for gk, ek in zip(g, e)]
+            opacity = np.where(on, sigmoid * coef, sigmoid).astype(np.float32)
+    sc = [ek.astype(np.float32) for ek in e]
     qx, qy, qz, qw = p[:, L.rot + 1], p[:, L.rot + 2], p[:, L.rot + 3], p[:, L.rot]  # Quaternion(rot_1, rot_2, rot_3, rot_0)
     d = ((qx * qx + qy * qy) + qz * qz) + qw * qw
     s = F(2.0) / d
@@ -174,8 +191,7 @@ def swizzle_splats(p: np.ndarray, creation_time: float, layout: PlyLayout | None
     Cv = _basis_mul(Mt, M)
     out[:, 4], out[:, 5], out[:, 6] = Cv[0][0], Cv[0][1], Cv[0][2]
     out[:, 7], out[:, 8], out[:, 9] = Cv[1][1], Cv[1][2], Cv[2][2]
-    with np.errstate(over="ignore"):
-        out[:, 10] = (1.0 / (1.0 + np.exp(-p[:, L.opacity].astype(np.float64)))).astype(np.float32)
+    out[:, 10] = opacity
     out[:, 12:15] = p[:, L.f_dc:L.f_dc + 3]
     k = SH_REST_FLOATS[L.sh_degree] // 3
     if k:

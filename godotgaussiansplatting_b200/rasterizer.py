@@ -46,9 +46,13 @@ class RenderTexture:
 
 class GaussianSplattingRasterizer:
     def __init__(self, point_cloud: PlyFile, output_texture_size, render_texture: RenderTexture | None, camera: Camera3D,
-                 device: int = 0, flags: int = 0, dup_capacity_factor: int = 10, clock=None, sh_bands: int | None = None):
+                 device: int = 0, flags: int = 0, dup_capacity_factor: int = 10, clock=None, sh_bands: int | None = None,
+                 antialiasing: float | None = None):
         """sh_bands: SH bands the context stores (gsr_config.sh_bands, 1..4 = degree + 1); None = the file's degree + 1, or 4 when its
-        properties do not name a 3DGS layout."""
+        properties do not name a 3DGS layout.
+        antialiasing: the 2D filter variance of anti-aliased trainings (include/gsr.h gsr_set_antialiasing; 0 = off); None = 0.1, the
+        Mip-Splatting filter, when the file carries `filter_3D`, else off.  A file with `filter_3D` is loaded with its 3D filter folded
+        into scale and opacity (gsr_upload_ply_filtered) whatever this value is."""
         self.should_enable_heatmap = [False]
         self.render_scale = [1.0]
         self.model_scale = [1.0]
@@ -64,6 +68,8 @@ class GaussianSplattingRasterizer:
         except ValueError:
             self._layout = None   # not a named 3DGS layout: the standard 62-property order, as the reference reads it
         self._sh_bands = int(sh_bands) if sh_bands is not None else (self._layout.sh_degree + 1 if self._layout else 0)
+        has_filter_3d = self._layout is not None and self._layout.filter_3d >= 0
+        self._antialiasing = float(antialiasing) if antialiasing is not None else (0.1 if has_filter_3d else 0.0)
         self._clock = clock or (lambda: _time.monotonic())
         self._t0 = self._clock()
         self.tile_dims = (0, 0)
@@ -112,6 +118,8 @@ class GaussianSplattingRasterizer:
         w, h = self._texture_size
         _lib.check(L.gsr_resize(self._ctx, w, h), "gsr_resize")
         self._bind_texture()
+        if self._antialiasing:
+            self.set_antialiasing(self._antialiasing)
         self.should_terminate_thread[0] = False
         self.num_splats_loaded[0] = 0
         if not load:
@@ -154,20 +162,33 @@ class GaussianSplattingRasterizer:
         self.num_splats_loaded[0] = max(self.num_splats_loaded[0], first + t.shape[0])
 
     def upload_ply(self, table: np.ndarray, layout: PlyLayout, first: int = 0, creation_time: float = 0.0) -> None:
-        """Device-side ingest of PLY vertices of any SH degree and property order (include/gsr.h gsr_upload_ply); layout: PlyFile.layout()."""
+        """Device-side ingest of PLY vertices of any SH degree and property order (include/gsr.h gsr_upload_ply); layout: PlyFile.layout().
+        A layout with a `filter_3D` property goes through gsr_upload_ply_filtered (Mip-Splatting's 3D filter)."""
         if not self._ctx:
             raise RuntimeError("init_gpu() first")
         t = np.ascontiguousarray(table, dtype=np.float32)
         lay = _lib.GsrPlyLayout(layout.nprops, layout.sh_degree, layout.x, layout.f_dc, layout.f_rest, layout.opacity, layout.scale, layout.rot)
         assert t.ndim == 2 and t.shape[1] == layout.nprops, (t.shape, layout.nprops)
-        _lib.check(_lib.lib().gsr_upload_ply(self._ctx, t.ctypes.data_as(C.POINTER(C.c_float)), C.byref(lay), first, t.shape[0],
-                                             float(creation_time)), "gsr_upload_ply")
+        ptr = t.ctypes.data_as(C.POINTER(C.c_float))
+        if layout.filter_3d >= 0:
+            _lib.check(_lib.lib().gsr_upload_ply_filtered(self._ctx, ptr, C.byref(lay), layout.filter_3d, first, t.shape[0], float(creation_time)),
+                       "gsr_upload_ply_filtered")
+        else:
+            _lib.check(_lib.lib().gsr_upload_ply(self._ctx, ptr, C.byref(lay), first, t.shape[0], float(creation_time)), "gsr_upload_ply")
         self.num_splats_loaded[0] = max(self.num_splats_loaded[0], first + t.shape[0])
 
     def set_sh_degree(self, degree: int) -> None:
         """SH degree of the colour of the frames rendered from now on (include/gsr.h gsr_set_sh_degree): 0 .. the stored degree, -1 = the
         stored degree (the default).  A lower degree trades view-dependent colour for projection bytes."""
         _lib.check(_lib.lib().gsr_set_sh_degree(self._ctx, int(degree)), "gsr_set_sh_degree")
+
+    def set_antialiasing(self, filter_variance: float) -> None:
+        """The 2D filter of anti-aliased trainings for the frames rendered from now on (include/gsr.h gsr_set_antialiasing): 0 = off
+        (the reference's +0.3 dilation), 0.3 = 3DGS --antialiasing / gsplat "antialiased", 0.1 = Mip-Splatting."""
+        v = float(filter_variance)
+        if self._ctx:
+            _lib.check(_lib.lib().gsr_set_antialiasing(self._ctx, v), "gsr_set_antialiasing")
+        self._antialiasing = v
 
     def _emit_loaded(self):
         self.is_loaded = True

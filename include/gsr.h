@@ -161,6 +161,16 @@ typedef struct gsr_ply_layout {
 } gsr_ply_layout;
 GSR_API int gsr_upload_ply(gsr_ctx *ctx, const float *ply, const gsr_ply_layout *layout, uint64_t first, uint64_t count, float creation_time);
 
+/* gsr_upload_ply, plus the per-splat 3D filter of Mip-Splatting: filter_3d = index of the `filter_3D` property, -1 = none
+ * (then exactly gsr_upload_ply).  Mip-Splatting's trainer writes filter_3D to point_cloud.ply and its renderer folds it into scale and
+ * opacity; gsr_upload_ply ignores the property, so such a cloud renders too thin.  Here, for a splat with f = filter_3D > 0, in float64
+ * and narrowed to float once: q_i = exp(scale_i)^2, q'_i = q_i + f*f, the covariance is built from the scales sqrt(q'_i) and the opacity
+ * is sigmoid(opacity) * sqrt((q_0 q_1 q_2) / (q'_0 q'_1 q'_2)).  A splat with f <= 0 or NaN is stored exactly as gsr_upload_ply stores
+ * it.  Load-time data preparation: any context may use it.  GSR_ERR_INVALID: what gsr_upload_ply rejects, or filter_3d outside
+ * -1..nprops-1.  Such clouds are trained with the 2D filter of gsr_set_antialiasing at 0.1. */
+GSR_API int gsr_upload_ply_filtered(gsr_ctx *ctx, const float *ply, const gsr_ply_layout *layout, int32_t filter_3d,
+                                    uint64_t first, uint64_t count, float creation_time);
+
 /* ---- texture_size setter (rasterizer.gd:26-48): reallocates tile_bounds + render_texture ---- */
 GSR_API int gsr_resize(gsr_ctx *ctx, int32_t width, int32_t height);
 
@@ -330,6 +340,21 @@ GSR_API int gsr_set_instances(gsr_ctx *ctx, const gsr_instance *instances, uint3
  *      single-context only: GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those calls
  *      (and gsr_group_export) fail with GSR_ERR_STATE on such a store or while a degree below 3 is set. ---- */
 GSR_API int gsr_set_sh_degree(gsr_ctx *ctx, int32_t degree);
+
+/* ---- Anti-aliased trainings (no reference counterpart: the reference dilates the 2D covariance by a fixed 0.3 px^2 and keeps the
+ *      opacity as stored).  The original 3DGS trainer with --antialiasing, gsplat / nerfstudio with rasterize_mode="antialiased" and
+ *      Mip-Splatting dilate by a variance v and also scale the opacity by sqrt(det(cov_2d) / det(cov_2d + v I)); their opacities are
+ *      trained for that factor, so drawn the reference's way every sub-pixel splat is too opaque, more so as the camera zooms out.
+ *      filter_variance: 0 = off (the reference: +0.3 dilation, opacity as stored; the default).
+ *      > 0: frames enqueued afterwards dilate the 2D covariance by filter_variance (px^2) and multiply the opacity by the
+ *      compensation factor coef = sqrt(max(0.000025, det(cov_2d) / det(cov_2d + v I))) (GLSL max: NaN gives the floor); that
+ *      opacity also sets the splat's radius.  0.3 = 3DGS --antialiasing / gsplat "antialiased"; 0.1 = Mip-Splatting's 2D filter.
+ *      The value is read when a frame is enqueued: frames already enqueued keep theirs, and the call never synchronises.  Back at 0
+ *      the frame is bit for bit that of a context that never used the filter.  gsr_resize keeps the setting.  GSR_ERR_INVALID,
+ *      previous state kept: a negative, NaN or infinite variance, or one above 64.  Single-context only: turning the filter on returns
+ *      GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those calls (and gsr_group_export)
+ *      fail with GSR_ERR_STATE while it is on. ---- */
+GSR_API int gsr_set_antialiasing(gsr_ctx *ctx, float filter_variance);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
