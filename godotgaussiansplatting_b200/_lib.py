@@ -15,7 +15,8 @@ GSR_OK, GSR_ERR_INVALID, GSR_ERR_CUDA, GSR_ERR_OOM, GSR_ERR_STATE, GSR_ERR_OVERF
 GSR_FLAG_REFERENCE_QUIRKS, GSR_FLAG_FIXED_RANGES, GSR_FLAG_FAST_REJECT, GSR_FLAG_STATIC_CAPACITY, GSR_FLAG_UNCONTRACTED_BLEND = 0x1, 0x2, 0x4, 0x8, 0x10
 GSR_FLAG_ORTHOGRAPHIC = 0x20
 (GSR_BUF_RECORDS, GSR_BUF_KEYS, GSR_BUF_VALUES, GSR_BUF_BOUNDS, GSR_BUF_KEYS_UNSORTED, GSR_BUF_VALUES_UNSORTED,
- GSR_BUF_FRAMEBUFFER, GSR_BUF_COMPOSITOR_TRACE, GSR_BUF_COMPOSITOR_TRACE_COUNT, GSR_BUF_INSTANCES, GSR_BUF_SPLATS) = range(11)
+ GSR_BUF_FRAMEBUFFER, GSR_BUF_COMPOSITOR_TRACE, GSR_BUF_COMPOSITOR_TRACE_COUNT, GSR_BUF_INSTANCES, GSR_BUF_SPLATS, GSR_BUF_DEPTH_WORDS_UNSORTED) = range(12)
+GSR_DEPTH_ORDER_KEY16, GSR_DEPTH_ORDER_VIEW_DEPTH = 0, 1
 GSR_MAX_INSTANCES, GSR_INSTANCE_RING = 4096, 8
 
 # every symbol include/gsr.h declares (tests/test_abi.py checks the header against this list and the .so)
@@ -23,7 +24,7 @@ EXPORTS = [
     "gsr_create", "gsr_destroy", "gsr_set_stream", "gsr_upload_splats_aos", "gsr_upload_ply_raw", "gsr_upload_ply", "gsr_resize", "gsr_set_band", "gsr_set_row_interleave", "gsr_band_sync_word", "gsr_band_fixup", "gsr_render",
     "gsr_render_async", "gsr_render_async_rgb", "gsr_render_async_fmt", "gsr_output_bytes", "gsr_present_device", "gsr_readback_async", "gsr_peer_export_framebuffers", "gsr_peer_import_framebuffers",
     "gsr_stream_join", "gsr_group_export", "gsr_group_attach", "gsr_group_detach", "gsr_group_set_present", "gsr_readback_rows_async", "gsr_sync", "gsr_framebuffer_device_ptr", "gsr_set_framebuffer_external",
-    "gsr_set_depth_compositing", "gsr_set_instances", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_upload_ply_filtered", "gsr_pick",
+    "gsr_set_depth_compositing", "gsr_set_instances", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_upload_ply_filtered", "gsr_pick",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -117,6 +118,7 @@ def lib():
         L.gsr_set_instances.argtypes = [vp, C.POINTER(GsrInstance), u32]
         L.gsr_set_sh_degree.argtypes = [vp, C.c_int32]
         L.gsr_set_antialiasing.argtypes = [vp, C.c_float]
+        L.gsr_set_depth_order.argtypes = [vp, C.c_int32]
         L.gsr_pick.argtypes = [vp, u32, C.c_float, fp]
         L.gsr_get_stats.argtypes = [vp, C.POINTER(GsrStats)]
         L.gsr_get_frame_history.argtypes = [vp, u32, C.POINTER(GsrFrameRecord), C.POINTER(u32)]

@@ -129,6 +129,11 @@ struct SortWorkspace {
     uint64_t max_n = 0;
     uint32_t max_tiles = 0;
     int grid_hist = 0, grid_sweep_pairs = 0, grid_sweep_keys = 0;
+    // depth-order sort (gsr_set_depth_order; sort_workspace_enable_depth): [6][256] histograms + [6] tickets, [6][depth_max_tiles][256]
+    // look-back words (depth_max_tiles counts the wide passes' tiles, the smaller ones)
+    uint32_t *depth_hist = nullptr, *depth_status = nullptr;
+    uint32_t depth_max_tiles = 0;
+    int grid_sweep_wide = 0;
     size_t bytes() const;
 };
 int sort_workspace_create(SortWorkspace &ws, uint64_t max_n, bool need_alt_buffers);
@@ -138,6 +143,12 @@ void sort_workspace_destroy(SortWorkspace &ws);
 // keys/vals.  vals/alt_vals may be null (keys only).  *launches += kernels launched.
 int sort_pairs_device(SortWorkspace &ws, uint32_t *keys, uint32_t *vals, const uint32_t *n_ptr, uint32_t *alt_keys,
                       uint32_t *alt_vals, cudaStream_t stream, int *launches);
+// The depth-order sort's workspace (allocated once; GSR_ERR_OOM leaves ws as it was).
+int sort_workspace_enable_depth(SortWorkspace &ws);
+// Sorts n pairs stably by (key >> 16, depth word): the frame's (tile, ord(view depth)) order.  6 passes ping-pong between keys / vals /
+// depth and the alt buffers; the result is back in keys / vals (depth is scratch: it ends sorted by the word alone).  *launches += 7.
+int sort_pairs_depth_device(SortWorkspace &ws, uint32_t *keys, uint32_t *vals, uint32_t *depth, const uint32_t *n_ptr, uint32_t *alt_keys,
+                            uint32_t *alt_vals, uint32_t *alt_depth, cudaStream_t stream, int *launches);
 uint32_t sort_tile_keys();
 
 // ---------------------------------------------------------------------------------------------
@@ -170,7 +181,14 @@ static_assert(sizeof(ProjectionArgs) == 288 && offsetof(ProjectionArgs, lookback
 // sh_bands: SH bands the frame evaluates (1..4, at most the store's); the kernel reads planes 0-2 and the first sh_planes(sh_bands) SH planes.
 // ortho: the frame's projection is orthographic (GSR_FLAG_ORTHOGRAPHIC; decided on the host at enqueue time, single-context only)
 // aa: the frame is anti-aliased with a.aa_variance > 0 (gsr_set_antialiasing; read at enqueue time, single-context only)
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false, bool aa = false);
+// depth_words: non-null = the frame is sorted by view depth (gsr_set_depth_order; single-context only): the projection also stores
+// depth_words[g] = depth_order_word(d) beside keys[g] / values[g], d the pair's splat's view depth
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false, bool aa = false,
+                      uint32_t *depth_words = nullptr);
+
+// gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
+// bit set).  Every finite value orders as its float does, -0 just before +0.
+__host__ __device__ __forceinline__ uint32_t depth_order_word(uint32_t bits) { return bits ^ ((bits >> 31) ? 0xFFFFFFFFu : 0x80000000u); }
 
 // ---------------------------------------------------------------------------------------------
 // splat instances (gsr_set_instances): ranges of the splat buffer drawn with their own affine transform into frame space
@@ -190,7 +208,7 @@ struct InstanceArgs {
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false,
-                                bool aa = false);
+                                bool aa = false, uint32_t *depth_words = nullptr);
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
 // (mapped page-locked host memory on the frame path)
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream);

@@ -42,10 +42,12 @@ struct gsr_ctx {
     int sh_bands = SH_BANDS_MAX; // SH bands the store keeps (gsr_config.sh_bands)
     int sh_degree = -1;          // render degree (gsr_set_sh_degree); -1 = the stored degree
     float aa_variance = 0.0f;    // anti-aliasing filter of the next frames (gsr_set_antialiasing); 0 = off
+    int32_t depth_order = GSR_DEPTH_ORDER_KEY16;   // sort order of the next frames (gsr_set_depth_order)
     float4 *records = nullptr;   // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
     uint32_t *vals = nullptr;    // 3 * capacity
+    uint32_t *depth_words = nullptr;   // 3 * capacity like keys, allocated by the first switch to GSR_DEPTH_ORDER_VIEW_DEPTH
     uint32_t *keys_cur = nullptr, *vals_cur = nullptr;   // sorted pairs of the most recent frame
     float4 *records_cur = nullptr;                       // record table the most recent frame composited from
     // front / back overlap: the projection of frame f+1 (front: HBM-bound) runs on its own stream beside the compositor of frame f
@@ -88,6 +90,7 @@ struct gsr_ctx {
     uint64_t staging_splats = 0;
     uint64_t staging_bytes = 0;  // 16 B x stored planes x staging_splats (at least one 240-byte AoS struct)
     uint32_t *unsorted_keys = nullptr, *unsorted_vals = nullptr;
+    uint32_t *unsorted_depth = nullptr;   // GSR_BUF_DEPTH_WORDS_UNSORTED: with keep_unsorted once depth_words exist
     bool keep_unsorted = false;
     int width = 0, height = 0, tiles_x = 0, tiles_y = 0, band_y0 = 0, band_y1 = 0;
     bool band_set = false;
@@ -190,6 +193,21 @@ float4 *framebuffer(gsr_ctx *c) { return c->fb_ext ? c->fb_ext : (c->fb_last ? c
 // SH bands the next frame evaluates, and whether the context stores or renders fewer than 4 (single-context only, like depth compositing)
 int render_bands(const gsr_ctx *c) { return c->sh_degree < 0 ? c->sh_bands : c->sh_degree + 1; }
 bool reduced_sh(const gsr_ctx *c) { return c->sh_bands < SH_BANDS_MAX || render_bands(c) < SH_BANDS_MAX; }
+bool view_depth_order(const gsr_ctx *c) { return c->depth_order == GSR_DEPTH_ORDER_VIEW_DEPTH; }
+
+// The depth-order buffers at the current capacity: the depth words (3 * cap_stride), GSR_BUF_DEPTH_WORDS_UNSORTED while unsorted pairs
+// are kept, and the sorter's depth-order workspace.  On failure nothing is left half allocated.
+int alloc_depth_order(gsr_ctx *c) {
+    if (!c->depth_words) {
+        uint32_t *dw = nullptr;
+        GSR_CUDA_TRY(cudaMalloc((void **)&dw, sizeof(uint32_t) * 3ull * c->cap_stride));
+        int rc = sort_workspace_enable_depth(c->sort);
+        if (rc) { cudaFree(dw); return rc; }
+        c->depth_words = dw;
+    }
+    if (c->unsorted_keys && !c->unsorted_depth) GSR_CUDA_TRY(cudaMalloc((void **)&c->unsorted_depth, sizeof(uint32_t) * c->capacity));
+    return GSR_OK;
+}
 
 void free_ctx(gsr_ctx *c) {
     if (!c) return;
@@ -208,6 +226,7 @@ void free_ctx(gsr_ctx *c) {
     for (int i = 0; i < c->grp.n_opened; ++i) cudaIpcCloseMemHandle(c->grp.opened[i]);
     cudaFree(c->grp.arena);
     cudaFree(c->unsorted_keys); cudaFree(c->unsorted_vals); cudaFree(c->trace); cudaFree(c->trace_count);
+    cudaFree(c->depth_words); cudaFree(c->unsorted_depth);
     cudaFree(c->inst.desc); cudaFree(c->inst.warps); cudaFree(c->inst.frame);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
     for (int i = 0; i < GSR_INSTANCE_RING; ++i) if (c->inst.ev[i]) cudaEventDestroy(c->inst.ev[i]);
@@ -509,6 +528,7 @@ GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod)
     if (c->inst.n && row_mod > 1) { set_last_error("gsr_set_row_interleave: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && row_mod > 1) { set_last_error("gsr_set_row_interleave: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (view_depth_order(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -532,6 +552,7 @@ GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (c->inst.n && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (view_depth_order(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
     c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
     return GSR_OK;
@@ -587,7 +608,11 @@ static int grow_capacity(gsr_ctx *c, uint64_t want) {
         GSR_CUDA_TRY(cudaMalloc((void **)&c->unsorted_keys, sizeof(uint32_t) * c->capacity));
         GSR_CUDA_TRY(cudaMalloc((void **)&c->unsorted_vals, sizeof(uint32_t) * c->capacity));
     }
-    return sort_workspace_create(c->sort, c->capacity, /*need_alt_buffers=*/false);
+    int rc = sort_workspace_create(c->sort, c->capacity, /*need_alt_buffers=*/false);
+    if (rc || !c->depth_words) return rc;
+    // the depth-order buffers grow with the pairs once they exist
+    cudaFree(c->depth_words); cudaFree(c->unsorted_depth); c->depth_words = c->unsorted_depth = nullptr;
+    return alloc_depth_order(c);
 }
 
 // Examine the mirrors of the frames that have completed since the last call (no host sync: event queries) and grow the
@@ -742,6 +767,13 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     pa.lookback = c->lookback; pa.frame = c->frame;
     pa.aa_variance = c->aa_variance;   // read here: frames already enqueued keep their filter
     const bool aa = c->aa_variance > 0.0f;
+    // gsr_set_depth_order, read here like the filter: the projection stores every pair's depth word beside its key, and the sort orders
+    // the pairs by (tile, depth word) instead of by the key (a group frame cannot occur: the mode refuses groups)
+    uint32_t *depth_in = nullptr, *depth_alt = nullptr;
+    if (view_depth_order(c) && !gf) {
+        depth_in = c->depth_words + (size_t)half * c->cap_stride;
+        depth_alt = c->depth_words + 2ull * c->cap_stride;
+    }
     if (gf) {
         // group mode: the projection is sharded by SPLATS.  This rank projects its slice and stores every pair and record into the
         // memory of the rank that owns it (peer stores over NVLink); the back part then waits for the other sources' flags and packs
@@ -768,10 +800,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         InstanceArgs ia;
         ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
         ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
-        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa))) return rc;
+        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa, depth_in))) return rc;
         launches += pa.num_splats ? 1 : 0;
     } else {
-        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa))) return rc;
+        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa, depth_in))) return rc;
         launches += pa.num_splats ? 1 : 0;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[1], fs));  // end of the front part
@@ -800,9 +832,14 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     if (c->keep_unsorted) {
         GSR_CUDA_TRY(cudaMemcpyAsync(c->unsorted_keys, keys_in, sizeof(uint32_t) * c->capacity, cudaMemcpyDeviceToDevice, s));
         GSR_CUDA_TRY(cudaMemcpyAsync(c->unsorted_vals, vals_in, sizeof(uint32_t) * c->capacity, cudaMemcpyDeviceToDevice, s));
+        if (depth_in) GSR_CUDA_TRY(cudaMemcpyAsync(c->unsorted_depth, depth_in, sizeof(uint32_t) * c->capacity, cudaMemcpyDeviceToDevice, s));
     }
     const uint32_t *m_ptr = reinterpret_cast<const uint32_t *>(reinterpret_cast<const char *>(c->frame) + offsetof(FrameState, dup_sorted));
-    if ((rc = sort_pairs_device(c->sort, keys_in, vals_in, m_ptr, keys_alt, vals_alt, s, &launches))) return rc;
+    if (depth_in) {
+        if ((rc = sort_pairs_depth_device(c->sort, keys_in, vals_in, depth_in, m_ptr, keys_alt, vals_alt, depth_alt, s, &launches))) return rc;
+    } else {
+        if ((rc = sort_pairs_device(c->sort, keys_in, vals_in, m_ptr, keys_alt, vals_alt, s, &launches))) return rc;
+    }
     GSR_CUDA_TRY(cudaEventRecord(ev[4], s));  // 'Sort'
 
     const int sharded = fast ? 2 : ((!(c->band_y0 == 0 && c->band_y1 == c->tiles_y) || c->row_mod > 1) ? 1 : 0);
@@ -1061,6 +1098,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (c->inst.n) { set_last_error("gsr_peer_export_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_export_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (view_depth_order(c)) { set_last_error("gsr_peer_export_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -1079,6 +1117,7 @@ GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (c->inst.n) { set_last_error("gsr_peer_import_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_import_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (view_depth_order(c)) { set_last_error("gsr_peer_import_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -1110,6 +1149,7 @@ GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_group_export: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_group_export: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (view_depth_order(c)) { set_last_error("gsr_group_export: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     if (!c->grp.arena) {
@@ -1142,6 +1182,7 @@ GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void
     if (c->inst.n && world > 1) { set_last_error("gsr_group_attach: instances are set (single-context only)"); return GSR_ERR_STATE; }
     if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && world > 1) { set_last_error("gsr_group_attach: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
+    if (view_depth_order(c) && world > 1) { set_last_error("gsr_group_attach: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1434,6 +1475,26 @@ GSR_API int gsr_set_antialiasing(gsr_ctx *c, float filter_variance) {
     return GSR_OK;
 }
 
+GSR_API int gsr_set_depth_order(gsr_ctx *c, int32_t mode) {
+    if (!c) return GSR_ERR_INVALID;
+    if (mode != GSR_DEPTH_ORDER_KEY16 && mode != GSR_DEPTH_ORDER_VIEW_DEPTH) {
+        set_last_error("gsr_set_depth_order: mode %d is neither GSR_DEPTH_ORDER_KEY16 nor GSR_DEPTH_ORDER_VIEW_DEPTH", mode);
+        return GSR_ERR_INVALID;
+    }
+    if (mode == GSR_DEPTH_ORDER_VIEW_DEPTH) {
+        const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
+        if (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1) {
+            set_last_error("gsr_set_depth_order: single-context only (no group, peer framebuffers, partial band or row interleave)");
+            return GSR_ERR_STATE;
+        }
+        int rc = use_device(c->device);
+        if (rc) return rc;
+        if ((rc = alloc_depth_order(c))) return rc;   // the first switch only (cudaMalloc may synchronise)
+    }
+    c->depth_order = mode;   // read by the next render_enqueue: frames already enqueued keep their order
+    return GSR_OK;
+}
+
 GSR_API int gsr_pick(gsr_ctx *c, uint32_t tile_id, float heatmap_factor, float out_xyzn[4]) {
     if (!c || !out_xyzn) return GSR_ERR_INVALID;
     if (c->width == 0) { set_last_error("gsr_pick before gsr_resize"); return GSR_ERR_STATE; }
@@ -1527,6 +1588,7 @@ GSR_API int gsr_debug_keep_unsorted(gsr_ctx *c, int enable) {
         GSR_CUDA_TRY(cudaMalloc((void **)&c->unsorted_keys, sizeof(uint32_t) * c->capacity));
         GSR_CUDA_TRY(cudaMalloc((void **)&c->unsorted_vals, sizeof(uint32_t) * c->capacity));
     }
+    if (enable && c->depth_words && !c->unsorted_depth) GSR_CUDA_TRY(cudaMalloc((void **)&c->unsorted_depth, sizeof(uint32_t) * c->capacity));
     c->keep_unsorted = enable != 0;
     return GSR_OK;
 }
@@ -1576,6 +1638,7 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
         case GSR_BUF_BOUNDS: src = c->bounds; avail = sizeof(uint2) * (size_t)c->tiles_x * c->tiles_y; break;
         case GSR_BUF_KEYS_UNSORTED: src = c->unsorted_keys; avail = c->unsorted_keys ? sizeof(uint32_t) * c->capacity : 0; break;
         case GSR_BUF_VALUES_UNSORTED: src = c->unsorted_vals; avail = c->unsorted_vals ? sizeof(uint32_t) * c->capacity : 0; break;
+        case GSR_BUF_DEPTH_WORDS_UNSORTED: src = c->unsorted_depth; avail = c->unsorted_depth ? sizeof(uint32_t) * c->capacity : 0; break;
         case GSR_BUF_FRAMEBUFFER: src = framebuffer(c); avail = sizeof(float4) * (size_t)c->width * c->height; break;
         case GSR_BUF_COMPOSITOR_TRACE: src = c->trace; avail = c->trace ? sizeof(ulonglong4) * (size_t)c->trace_cap : 0; break;
         case GSR_BUF_COMPOSITOR_TRACE_COUNT: src = c->trace_count; avail = c->trace_count ? sizeof(uint32_t) : 0; break;

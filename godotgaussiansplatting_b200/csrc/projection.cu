@@ -415,9 +415,15 @@ __device__ __forceinline__ InstanceWarp instance_warp(const ProjectionArgs &a, c
 // soa_planes(SH_BANDS) planes.  Every degree-only difference is a constant or an `if constexpr`: SH_BANDS = 4 is the degree-3 kernel.
 // ORTHO (GSR_FLAG_ORTHOGRAPHIC) and AA (gsr_set_antialiasing): every lane runs project_lane<.., ORTHO, AA>; nothing else of the kernel
 // changes.
-template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false>
+// DEPTH (gsr_set_depth_order): every pair also gets depth_words[g] = depth_order_word(d), d = -(((V2 x + V6 y) + V10 z) + V14) of the
+// record's (frame-space) position with the frame's view matrix -- the depth compositing's d, and -view[2] of project_lane without
+// instances.  The pointer travels in a third parameter, so the first two keep their offsets (a plain pointer parameter, unlike a
+// __grid_constant__ struct, changes the register allocation of the other instantiations).  Never with the compaction path (sharded only).
+struct DepthArgs { uint32_t *words = nullptr; };
+template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false, bool DEPTH = false>
 __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
-                                                                                       const __grid_constant__ InstanceArgs ia = InstanceArgs()) {
+                                                                                       const __grid_constant__ InstanceArgs ia = InstanceArgs(),
+                                                                                       const __grid_constant__ DepthArgs da = DepthArgs()) {
 #ifndef GSR_CPU_EMU
     extern __shared__ __align__(128) unsigned char proj_smem[];
 #else
@@ -626,6 +632,10 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     //      step, which keeps one huge splat from serialising a lane for hundreds of iterations. ----
     constexpr uint32_t EMIT_SMALL = 4;
     const uint32_t my_off = incl - n;
+    uint32_t dword = 0u;
+    if constexpr (DEPTH) {
+        if (n) dword = depth_order_word(__float_as_uint(-(((a.vp[2] * r0.z + a.vp[6] * r0.w) + a.vp[10] * r1.w) + a.vp[14] * 1.0f)));
+    }
     if (n != 0u && n <= EMIT_SMALL) {
         uint32_t x = x0u, y = y0u;
         const uint32_t x1 = x0u + wu;
@@ -636,6 +646,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
                 if (g < (unsigned long long)a.capacity) {
                     a.keys[g] = ((y * gx + x) << 16) | depth;
                     a.values[g] = id;
+                    if constexpr (DEPTH) da.words[g] = dword;
                 }
                 if (++x == x1) { x = x0u; y += (uint32_t)a.row_mod; }
             }
@@ -648,12 +659,15 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         const uint32_t sn = __shfl_sync(0xffffffffu, n, src), soff = __shfl_sync(0xffffffffu, my_off, src);
         const uint32_t sx0 = __shfl_sync(0xffffffffu, x0u, src), sy0 = __shfl_sync(0xffffffffu, y0u, src);
         const uint32_t sw = __shfl_sync(0xffffffffu, wu, src), sdepth = __shfl_sync(0xffffffffu, depth, src);
+        uint32_t sdword = 0u;
+        if constexpr (DEPTH) sdword = __shfl_sync(0xffffffffu, dword, src);
         for (uint32_t j = lane; j < sn; j += 32u) {
             const uint32_t ry = j / sw, rx = j - ry * sw;
             const unsigned long long g = base + soff + j;
             if (g < (unsigned long long)a.capacity) {
                 a.keys[g] = (((sy0 + ry * (uint32_t)a.row_mod) * gx + sx0 + rx) << 16) | sdepth;
                 a.values[g] = id0 + (uint32_t)src;
+                if constexpr (DEPTH) da.words[g] = sdword;
             }
         }
     }
@@ -1133,19 +1147,20 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 constexpr size_t projection_smem_bytes(int sh_bands) { return proj_slab_bytes(sh_bands) * PROJ_WARPS; }
 static_assert(projection_smem_bytes(SH_BANDS_MAX) == PROJ_SMEM_BYTES, "the degree-3 slab");
 
-template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false>
+template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false, bool DEPTH = false>
 int preload_projection_variant() {
     cudaFuncAttributes fa;
-    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)projection_smem_bytes(B)));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA>));
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)projection_smem_bytes(B)));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH>));
     return GSR_OK;
 }
-// projection_kernel<INSTANCED, 1..4, ORTHO, AA>
-template <bool INSTANCED, bool ORTHO, bool AA = false>
+// projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH>
+template <bool INSTANCED, bool ORTHO, bool AA = false, bool DEPTH = false>
 int preload_projection_bands() {
     int rc;
-    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA>()) ||
-        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA>()))
+    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA, DEPTH>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA, DEPTH>()) ||
+        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA, DEPTH>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA, DEPTH>()))
         return rc;
     return GSR_OK;
 }
@@ -1173,6 +1188,12 @@ int preload_projection_kernels() {
     if ((rc = preload_projection_bands<false, false, true>()) || (rc = preload_projection_bands<true, false, true>()) ||
         (rc = preload_projection_bands<false, true, true>()) || (rc = preload_projection_bands<true, true, true>()))
         return rc;
+    // the depth-order variants (gsr_set_depth_order) of all of the above
+    if ((rc = preload_projection_bands<false, false, false, true>()) || (rc = preload_projection_bands<true, false, false, true>()) ||
+        (rc = preload_projection_bands<false, true, false, true>()) || (rc = preload_projection_bands<true, true, false, true>()) ||
+        (rc = preload_projection_bands<false, false, true, true>()) || (rc = preload_projection_bands<true, false, true, true>()) ||
+        (rc = preload_projection_bands<false, true, true, true>()) || (rc = preload_projection_bands<true, true, true, true>()))
+        return rc;
     return GSR_OK;
 }
 uint32_t projection_scatter_blocks(uint32_t count) { return count ? (count + PROJ_THREADS - 1) / PROJ_THREADS : 1u; }   // an empty slice still publishes its flags
@@ -1186,29 +1207,40 @@ int launch_projection_scatter(const ProjectionArgs &frame_args, const ScatterPee
     return GSR_OK;
 }
 
-// projection_kernel<INSTANCED, B, ORTHO, AA> for B = sh_bands (the orthographic and the anti-aliased frames: single-context only, never sharded)
-template <bool INSTANCED, bool ORTHO, bool AA>
-void launch_projection_bands(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t blocks, cudaStream_t stream, int sh_bands) {
+// projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH> for B = sh_bands (the orthographic, anti-aliased and depth-order frames: single-context
+// only, never sharded)
+template <bool INSTANCED, bool ORTHO, bool AA, bool DEPTH>
+void launch_projection_bands(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, uint32_t blocks, cudaStream_t stream, int sh_bands) {
     switch (sh_bands) {
-        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia); break;
-        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia); break;
-        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia); break;
-        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia); break;
+        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia, DepthArgs{dw}); break;
+        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia, DepthArgs{dw}); break;
+        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia, DepthArgs{dw}); break;
+        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia, DepthArgs{dw}); break;
+    }
+}
+template <bool INSTANCED, bool DEPTH>
+void launch_projection_modes(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, uint32_t blocks, cudaStream_t stream, int sh_bands,
+                             bool ortho, bool aa) {
+    if (ortho) {
+        if (aa) launch_projection_bands<INSTANCED, true, true, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
+        else launch_projection_bands<INSTANCED, true, false, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
+    } else {
+        if (aa) launch_projection_bands<INSTANCED, false, true, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
+        else launch_projection_bands<INSTANCED, false, false, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
     }
 }
 template <bool INSTANCED>
-void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t blocks, cudaStream_t stream, int sh_bands, bool ortho,
-                               bool aa) {
-    if (!aa) launch_projection_bands<INSTANCED, true, false>(a, ia, blocks, stream, sh_bands);
-    else if (ortho) launch_projection_bands<INSTANCED, true, true>(a, ia, blocks, stream, sh_bands);
-    else launch_projection_bands<INSTANCED, false, true>(a, ia, blocks, stream, sh_bands);
+void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, uint32_t blocks, cudaStream_t stream, int sh_bands,
+                               bool ortho, bool aa) {
+    if (dw) launch_projection_modes<INSTANCED, true>(a, ia, dw, blocks, stream, sh_bands, ortho, aa);
+    else launch_projection_modes<INSTANCED, false>(a, ia, nullptr, blocks, stream, sh_bands, ortho, aa);
 }
 
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa, uint32_t *depth_words) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho || aa) {
-        launch_projection_special<false>(a, InstanceArgs(), blocks, stream, sh_bands, ortho, aa);
+    if (ortho || aa || depth_words) {
+        launch_projection_special<false>(a, InstanceArgs(), depth_words, blocks, stream, sh_bands, ortho, aa);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }
@@ -1228,11 +1260,12 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
     return GSR_OK;
 }
 
-int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
+int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho, bool aa,
+                                uint32_t *depth_words) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho || aa) {
-        launch_projection_special<true>(a, ia, blocks, stream, sh_bands, ortho, aa);
+    if (ortho || aa || depth_words) {
+        launch_projection_special<true>(a, ia, depth_words, blocks, stream, sh_bands, ortho, aa);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }

@@ -85,7 +85,70 @@ __global__ void __launch_bounds__(HIST_THREADS) sort_hist_kernel(const uint32_t 
 }
 
 // ------------------------------------------------------------------------------------------------
+// gsr_set_depth_order: histograms of the six passes of the (tile, depth word) sort + status clear.  Reads the keys and the depth
+// words once: digits 0-3 of the depth word (the four wide passes) and digits 2-3 of the key (tile = key >> 16, the two narrow passes).
+// The wide passes cut the pairs into tiles of `wide_tile` keys, the narrow ones into tiles of `narrow_tile`.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(HIST_THREADS) sort_hist_depth_kernel(const uint32_t *__restrict__ keys, const uint32_t *__restrict__ depth,
+                                                                       const uint32_t *__restrict__ n_ptr, uint32_t n_max, uint32_t *__restrict__ hist,
+                                                                       uint32_t *__restrict__ status, uint32_t wide_tile, uint32_t narrow_tile,
+                                                                       uint32_t max_tiles) {
+    __shared__ uint32_t sh[6 * RADIX];
+    const uint32_t tid = threadIdx.x;
+    const uint32_t gtid = blockIdx.x * HIST_THREADS + tid;
+    const uint32_t gsize = gridDim.x * HIST_THREADS;
+    uint32_t n = *n_ptr;
+    n = n < n_max ? n : n_max;
+    for (uint32_t i = tid; i < 6 * RADIX; i += HIST_THREADS) sh[i] = 0;
+
+    const uint32_t wide_words = (n + wide_tile - 1) / wide_tile * RADIX;
+    const uint32_t narrow_words = (n + narrow_tile - 1) / narrow_tile * RADIX;
+    for (uint32_t i = gtid; i < wide_words; i += gsize) {
+#pragma unroll
+        for (int p = 0; p < 4; ++p) status[(size_t)p * max_tiles * RADIX + i] = 0u;
+        if (i < narrow_words) {
+            status[(size_t)4 * max_tiles * RADIX + i] = 0u;
+            status[(size_t)5 * max_tiles * RADIX + i] = 0u;
+        }
+    }
+    __syncthreads();
+
+    const uint32_t n4 = n >> 2;
+    const uint4 *k4 = reinterpret_cast<const uint4 *>(keys);
+    const uint4 *d4 = reinterpret_cast<const uint4 *>(depth);
+    for (uint32_t i = gtid; i < n4; i += gsize) {
+        const uint4 k = __ldg(k4 + i), d = __ldg(d4 + i);
+        const uint32_t kk[4] = {k.x, k.y, k.z, k.w}, dd[4] = {d.x, d.y, d.z, d.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            atomicAdd(&sh[0 * RADIX + (dd[j] & 255u)], 1u);
+            atomicAdd(&sh[1 * RADIX + ((dd[j] >> 8) & 255u)], 1u);
+            atomicAdd(&sh[2 * RADIX + ((dd[j] >> 16) & 255u)], 1u);
+            atomicAdd(&sh[3 * RADIX + (dd[j] >> 24)], 1u);
+            atomicAdd(&sh[4 * RADIX + ((kk[j] >> 16) & 255u)], 1u);
+            atomicAdd(&sh[5 * RADIX + (kk[j] >> 24)], 1u);
+        }
+    }
+    for (uint32_t i = (n4 << 2) + gtid; i < n; i += gsize) {
+        const uint32_t k = keys[i], d = depth[i];
+        atomicAdd(&sh[0 * RADIX + (d & 255u)], 1u);
+        atomicAdd(&sh[1 * RADIX + ((d >> 8) & 255u)], 1u);
+        atomicAdd(&sh[2 * RADIX + ((d >> 16) & 255u)], 1u);
+        atomicAdd(&sh[3 * RADIX + (d >> 24)], 1u);
+        atomicAdd(&sh[4 * RADIX + ((k >> 16) & 255u)], 1u);
+        atomicAdd(&sh[5 * RADIX + (k >> 24)], 1u);
+    }
+    __syncthreads();
+    for (uint32_t i = tid; i < 6 * RADIX; i += HIST_THREADS) {
+        const uint32_t v = sh[i];
+        if (v) atomicAdd(&hist[i], v);
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // one onesweep pass
+// WIDE (gsr_set_depth_order): the sorted word carries two payload words, vals_in / vals_out and vals2_in / vals2_out (PAIRS is then
+// true too).  Every wide-only statement is an `if constexpr`: WIDE = false is the pass as it always was.
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
 
@@ -99,20 +162,23 @@ __device__ __forceinline__ uint32_t warp_incl_scan(uint32_t v) {
     return v;
 }
 
-template <int THREADS, int ITEMS, bool PAIRS>
+template <int THREADS, int ITEMS, bool PAIRS, bool WIDE = false>
 __global__ void __launch_bounds__(THREADS, 1024 / THREADS) onesweep_kernel(const uint32_t *__restrict__ keys_in, uint32_t *__restrict__ keys_out,
                                                            const uint32_t *__restrict__ vals_in, uint32_t *__restrict__ vals_out,
                                                            const uint32_t *__restrict__ n_ptr, uint32_t n_max,
                                                            const uint32_t *__restrict__ hist,  // [256], this pass
                                                            uint32_t *status,                   // [tiles][256], this pass
-                                                           uint32_t *ticket, int shift) {
+                                                           uint32_t *ticket, int shift,
+                                                           const uint32_t *__restrict__ vals2_in = nullptr,  // WIDE: second payload
+                                                           uint32_t *__restrict__ vals2_out = nullptr) {
     static_assert(THREADS >= RADIX && THREADS % 32 == 0, "need one thread per digit");
+    static_assert(!WIDE || PAIRS, "a wide pass carries pairs");
     constexpr int WARPS = THREADS / 32;
     constexpr uint32_t TILE_KEYS = THREADS * ITEMS;
 #ifndef GSR_CPU_EMU
     extern __shared__ uint32_t smem[];
 #else  // tests/kernel_emu (CPU logic pre-flight): dynamic shared memory becomes a block-shared array of the same size
-    __shared__ uint32_t smem[WARPS * RADIX + 2 * TILE_KEYS];
+    __shared__ uint32_t smem[WARPS * RADIX + (WIDE ? 3 : 2) * TILE_KEYS];
 #endif
     uint32_t *s_whist = smem;                    // [WARPS][256] warp-private digit counters
     uint32_t *s_keys = s_whist + WARPS * RADIX;  // [TILE_KEYS]
@@ -157,6 +223,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) onesweep_kernel(const
         const uint32_t my_base = tile_base + warp * (32u * ITEMS) + lane;
         const bool full = (tile_base + TILE_KEYS) <= n;
         uint32_t key[ITEMS], val[ITEMS], rank[ITEMS];
+        uint32_t val2[WIDE ? ITEMS : 1];
         if (full) {
 #pragma unroll
             for (int i = 0; i < ITEMS; ++i) key[i] = keys_in[my_base + i * 32u];
@@ -164,12 +231,17 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) onesweep_kernel(const
 #pragma unroll
                 for (int i = 0; i < ITEMS; ++i) val[i] = vals_in[my_base + i * 32u];
             }
+            if constexpr (WIDE) {
+#pragma unroll
+                for (int i = 0; i < ITEMS; ++i) val2[i] = vals2_in[my_base + i * 32u];
+            }
         } else {
 #pragma unroll
             for (int i = 0; i < ITEMS; ++i) {
                 const uint32_t idx = my_base + i * 32u;
                 key[i] = idx < n ? keys_in[idx] : 0xFFFFFFFFu;  // pad keys sort last (radix_sort_downsweep.glsl:87)
                 if (PAIRS) val[i] = idx < n ? vals_in[idx] : 0u;
+                if constexpr (WIDE) val2[i] = idx < n ? vals2_in[idx] : 0u;
             }
         }
 
@@ -263,6 +335,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) onesweep_kernel(const
             const uint32_t pos = s_dstart[d] + wh[d] + rank[i];
             s_keys[pos] = key[i];
             if (PAIRS) s_vals[pos] = val[i];
+            if constexpr (WIDE) s_vals[TILE_KEYS + pos] = val2[i];
         }
 
         // ---- decoupled look-back: one thread per digit walks the predecessor tiles ----
@@ -292,6 +365,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) onesweep_kernel(const
             const uint32_t dst = s_base[(k >> shift) & 255u] + idx;
             keys_out[dst] = k;
             if (PAIRS) vals_out[dst] = s_vals[idx];
+            if constexpr (WIDE) vals2_out[dst] = s_vals[TILE_KEYS + idx];
         }
     }
 }
@@ -312,6 +386,11 @@ template <bool PAIRS>
 constexpr size_t sweep_smem() {
     return sizeof(uint32_t) * ((SWEEP_THREADS / 32) * RADIX + SWEEP_TILE * (PAIRS ? 2 : 1));
 }
+// the wide passes of the depth-order sort (three words per key): 8 keys per thread keep them within the 64 registers of two CTAs per SM
+constexpr int WIDE_ITEMS = 8;
+constexpr uint32_t WIDE_TILE = SWEEP_THREADS * WIDE_ITEMS;
+constexpr size_t wide_smem() { return sizeof(uint32_t) * ((SWEEP_THREADS / 32) * RADIX + 3 * WIDE_TILE); }
+static_assert(WIDE_TILE <= SWEEP_TILE, "the narrow passes of the depth-order sort use the wide passes' look-back slices");
 
 }  // namespace
 
@@ -324,10 +403,37 @@ int preload_sort_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, sort_hist_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, onesweep_kernel<SWEEP_THREADS, SWEEP_ITEMS, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, onesweep_kernel<SWEEP_THREADS, SWEEP_ITEMS, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, sort_hist_depth_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, onesweep_kernel<SWEEP_THREADS, WIDE_ITEMS, true, true>));
     return GSR_OK;
 }
 size_t SortWorkspace::bytes() const {
-    return sizeof(uint32_t) * (4 * RADIX + 8) + sizeof(uint32_t) * 4ull * max_tiles * RADIX + (alt_keys ? 8ull * max_n : 0);
+    return sizeof(uint32_t) * (4 * RADIX + 8) + sizeof(uint32_t) * 4ull * max_tiles * RADIX + (alt_keys ? 8ull * max_n : 0) +
+           (depth_hist ? sizeof(uint32_t) * (6 * RADIX + 8) + sizeof(uint32_t) * 6ull * depth_max_tiles * RADIX : 0);
+}
+
+int sort_workspace_enable_depth(SortWorkspace &ws) {
+    if (ws.depth_hist) return GSR_OK;
+    const uint32_t tiles = (uint32_t)((ws.max_n + WIDE_TILE - 1) / WIDE_TILE);
+    uint32_t *h = nullptr, *st = nullptr;
+    cudaError_t e = cudaMalloc((void **)&h, sizeof(uint32_t) * (6 * RADIX + 8));
+    if (e == cudaSuccess) e = cudaMalloc((void **)&st, sizeof(uint32_t) * 6ull * tiles * RADIX);
+    auto kw = onesweep_kernel<SWEEP_THREADS, WIDE_ITEMS, true, true>;
+    int occ = 0;
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(kw, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)wide_smem());
+    if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kw, SWEEP_THREADS, wide_smem());
+    if (e != cudaSuccess || occ < 1) {
+        cudaFree(h); cudaFree(st);
+        set_last_error("sorter: depth-order workspace: %s", e != cudaSuccess ? cudaGetErrorString(e) : "wide onesweep kernel does not fit on an SM");
+        return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+    }
+    int dev = 0, sm_count = 0;
+    GSR_CUDA_TRY(cudaGetDevice(&dev));
+    GSR_CUDA_TRY(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
+    ws.depth_hist = h; ws.depth_status = st; ws.depth_max_tiles = tiles;
+    const uint32_t g = (uint32_t)(sm_count * occ);
+    ws.grid_sweep_wide = (int)(g < tiles ? g : tiles);
+    return GSR_OK;
 }
 
 int sort_workspace_create(SortWorkspace &ws, uint64_t max_n, bool need_alt_buffers) {
@@ -373,6 +479,8 @@ void sort_workspace_destroy(SortWorkspace &ws) {
     cudaFree(ws.status);
     cudaFree(ws.alt_keys);
     cudaFree(ws.alt_vals);
+    cudaFree(ws.depth_hist);
+    cudaFree(ws.depth_status);
     ws = SortWorkspace();
 }
 
@@ -397,6 +505,36 @@ int sort_pairs_device(SortWorkspace &ws, uint32_t *keys, uint32_t *vals, const u
     }
     GSR_CUDA_TRY(cudaGetLastError());
     if (launches) *launches += 5;
+    return GSR_OK;
+}
+
+// (tile, depth word, input order): four wide passes over the depth word carry (key, value), then two passes of the pairs kernel over
+// the tile bits of the key carry the value.  Six passes: the result is back in keys / vals; depth is left sorted by the word alone.
+int sort_pairs_depth_device(SortWorkspace &ws, uint32_t *keys, uint32_t *vals, uint32_t *depth, const uint32_t *n_ptr, uint32_t *alt_keys,
+                            uint32_t *alt_vals, uint32_t *alt_depth, cudaStream_t stream, int *launches) {
+    if (!ws.depth_hist) { set_last_error("sorter: depth-order workspace not allocated"); return GSR_ERR_STATE; }
+    const uint32_t n_max = (uint32_t)ws.max_n;
+    const size_t slice = (size_t)ws.depth_max_tiles * RADIX;
+    GSR_CUDA_TRY(cudaMemsetAsync(ws.depth_hist, 0, sizeof(uint32_t) * (6 * RADIX + 6), stream));
+    uint32_t *tickets = ws.depth_hist + 6 * RADIX;
+    sort_hist_depth_kernel<<<ws.grid_hist, HIST_THREADS, 0, stream>>>(keys, depth, n_ptr, n_max, ws.depth_hist, ws.depth_status, WIDE_TILE,
+                                                                      SWEEP_TILE, ws.depth_max_tiles);
+    uint32_t *din = depth, *dout = alt_depth, *kin = keys, *kout = alt_keys, *vin = vals, *vout = alt_vals, *t;
+    for (int pass = 0; pass < 4; ++pass) {
+        onesweep_kernel<SWEEP_THREADS, WIDE_ITEMS, true, true><<<ws.grid_sweep_wide, SWEEP_THREADS, wide_smem(), stream>>>(
+            din, dout, kin, kout, n_ptr, n_max, ws.depth_hist + pass * RADIX, ws.depth_status + pass * slice, tickets + pass, 8 * pass, vin, vout);
+        t = din; din = dout; dout = t;
+        t = kin; kin = kout; kout = t;
+        t = vin; vin = vout; vout = t;
+    }
+    for (int pass = 4; pass < 6; ++pass) {
+        onesweep_kernel<SWEEP_THREADS, SWEEP_ITEMS, true><<<ws.grid_sweep_pairs, SWEEP_THREADS, sweep_smem<true>(), stream>>>(
+            kin, kout, vin, vout, n_ptr, n_max, ws.depth_hist + pass * RADIX, ws.depth_status + pass * slice, tickets + pass, 8 * pass - 16);
+        t = kin; kin = kout; kout = t;
+        t = vin; vin = vout; vout = t;
+    }
+    GSR_CUDA_TRY(cudaGetLastError());
+    if (launches) *launches += 7;
     return GSR_OK;
 }
 

@@ -47,12 +47,14 @@ class RenderTexture:
 class GaussianSplattingRasterizer:
     def __init__(self, point_cloud: PlyFile, output_texture_size, render_texture: RenderTexture | None, camera: Camera3D,
                  device: int = 0, flags: int = 0, dup_capacity_factor: int = 10, clock=None, sh_bands: int | None = None,
-                 antialiasing: float | None = None):
+                 antialiasing: float | None = None, depth_order: int = 0):
         """sh_bands: SH bands the context stores (gsr_config.sh_bands, 1..4 = degree + 1); None = the file's degree + 1, or 4 when its
         properties do not name a 3DGS layout.
         antialiasing: the 2D filter variance of anti-aliased trainings (include/gsr.h gsr_set_antialiasing; 0 = off); None = 0.1, the
         Mip-Splatting filter, when the file carries `filter_3D`, else off.  A file with `filter_3D` is loaded with its 3D filter folded
-        into scale and opacity (gsr_upload_ply_filtered) whatever this value is."""
+        into scale and opacity (gsr_upload_ply_filtered) whatever this value is.
+        depth_order: how each tile's splats are ordered (include/gsr.h gsr_set_depth_order): 0 = the reference's 16-bit depth key, 1 = exact
+        view depth (large or metric-scale scenes, depth compositing)."""
         self.should_enable_heatmap = [False]
         self.render_scale = [1.0]
         self.model_scale = [1.0]
@@ -70,6 +72,7 @@ class GaussianSplattingRasterizer:
         self._sh_bands = int(sh_bands) if sh_bands is not None else (self._layout.sh_degree + 1 if self._layout else 0)
         has_filter_3d = self._layout is not None and self._layout.filter_3d >= 0
         self._antialiasing = float(antialiasing) if antialiasing is not None else (0.1 if has_filter_3d else 0.0)
+        self._depth_order = int(depth_order)
         self._clock = clock or (lambda: _time.monotonic())
         self._t0 = self._clock()
         self.tile_dims = (0, 0)
@@ -120,6 +123,8 @@ class GaussianSplattingRasterizer:
         self._bind_texture()
         if self._antialiasing:
             self.set_antialiasing(self._antialiasing)
+        if self._depth_order:
+            self.set_depth_order(self._depth_order)
         self.should_terminate_thread[0] = False
         self.num_splats_loaded[0] = 0
         if not load:
@@ -189,6 +194,14 @@ class GaussianSplattingRasterizer:
         if self._ctx:
             _lib.check(_lib.lib().gsr_set_antialiasing(self._ctx, v), "gsr_set_antialiasing")
         self._antialiasing = v
+
+    def set_depth_order(self, mode: int) -> None:
+        """How the frames rendered from now on order each tile's splats (include/gsr.h gsr_set_depth_order): 0 = the reference's 16-bit
+        depth key (ties keep splat-id order), 1 = exact view depth (ties keep splat-id order only at equal float depth)."""
+        m = int(mode)
+        if self._ctx:
+            _lib.check(_lib.lib().gsr_set_depth_order(self._ctx, m), "gsr_set_depth_order")
+        self._depth_order = m
 
     def _emit_loaded(self):
         self.is_loaded = True

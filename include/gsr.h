@@ -80,8 +80,10 @@ enum {
     GSR_BUF_COMPOSITOR_TRACE_COUNT = 8, /* number of trace items written (uint32) */
     GSR_BUF_INSTANCES = 9,              /* gsr_set_instances: 24 floats per instance, to_frame as given then the library's inverse
                                            [A^-1 | -A^-1 t] rounded to float (both 3x4, column-major) */
-    GSR_BUF_SPLATS = 10                 /* the stored splat planes, plane-major: (3 + P) x plane_stride float4, plane_stride = max_splats
+    GSR_BUF_SPLATS = 10,                /* the stored splat planes, plane-major: (3 + P) x plane_stride float4, plane_stride = max_splats
                                            rounded up to 256 (gsr_config.sh_bands) */
+    GSR_BUF_DEPTH_WORDS_UNSORTED = 11   /* gsr_set_depth_order: the last mode-1 frame's ord(d) per pair in emission order, M entries
+                                           (kept with gsr_debug_keep_unsorted once mode 1 has been switched on) */
 };
 
 typedef struct gsr_ctx gsr_ctx;       /* one rasterizer = one GaussianSplattingRasterizer instance */
@@ -355,6 +357,27 @@ GSR_API int gsr_set_sh_degree(gsr_ctx *ctx, int32_t degree);
  *      GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those calls (and gsr_group_export)
  *      fail with GSR_ERR_STATE while it is on. ---- */
 GSR_API int gsr_set_antialiasing(gsr_ctx *ctx, float filter_variance);
+
+/* ---- Order splats by exact view depth (no reference counterpart: the reference sorts each frame's pairs by tile << 16 | a 16-bit
+ *      depth, so splats whose depths share a 16-bit bin -- 0.5 units wide at depth 100 with near = 0.05 -- keep splat-id order, which
+ *      pops as the camera moves and can end a depth-composited pixel on a tied splat behind the scene).
+ *      GSR_DEPTH_ORDER_KEY16 (0): the reference's order, the default.
+ *      GSR_DEPTH_ORDER_VIEW_DEPTH (1): frames enqueued afterwards sort their pairs by (tile id, ord(d), emission order), d =
+ *      -(((V[2] x + V[6] y) + V[10] z) + V[14]) in float32 with x, y, z the record's (frame-space) position and V the frame's view
+ *      matrix (view_proj[0..15]) -- the d of depth compositing -- and ord the order-preserving map of a float's bits (every finite d,
+ *      negative ones included; -0 just before +0).  Ties keep emission order (drawn-id order, tile order inside a splat's rect).  The
+ *      keys, records, M, V, C, overflow and tile bounds are those of the default frame; only the order inside each tile's range
+ *      changes, and GSR_BUF_KEYS / GSR_BUF_VALUES return it.  Works with instances, orthographic frames, anti-aliasing, reduced SH,
+ *      depth compositing, the heat map, GSR_FLAG_STATIC_CAPACITY and front / back overlap.
+ *      Cost: the projection writes 4 more bytes per pair and the sort takes six passes over 48 bits instead of four over 32 (about
+ *      twice the sort's traffic; DESIGN.md section 5.12).  The first switch to mode 1 allocates 12 bytes per pair of capacity (and may
+ *      synchronise once: GSR_ERR_OOM keeps the previous state); later switches never synchronise.  The mode is read when a frame is
+ *      enqueued: frames already enqueued keep theirs, and gsr_resize keeps the setting.  GSR_ERR_INVALID: any other mode.
+ *      Single-context only: switching mode 1 on returns GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or
+ *      row_mod > 1, and those calls (and gsr_group_export) fail with GSR_ERR_STATE while it is on. ---- */
+#define GSR_DEPTH_ORDER_KEY16 0
+#define GSR_DEPTH_ORDER_VIEW_DEPTH 1
+GSR_API int gsr_set_depth_order(gsr_ctx *ctx, int32_t mode);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
