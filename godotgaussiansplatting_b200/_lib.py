@@ -17,6 +17,10 @@ GSR_FLAG_ORTHOGRAPHIC = 0x20
 (GSR_BUF_RECORDS, GSR_BUF_KEYS, GSR_BUF_VALUES, GSR_BUF_BOUNDS, GSR_BUF_KEYS_UNSORTED, GSR_BUF_VALUES_UNSORTED,
  GSR_BUF_FRAMEBUFFER, GSR_BUF_COMPOSITOR_TRACE, GSR_BUF_COMPOSITOR_TRACE_COUNT, GSR_BUF_INSTANCES, GSR_BUF_SPLATS, GSR_BUF_DEPTH_WORDS_UNSORTED) = range(12)
 GSR_DEPTH_ORDER_KEY16, GSR_DEPTH_ORDER_VIEW_DEPTH = 0, 1
+GSR_MAX_CUTOUTS = 16
+GSR_CUTOUT_BOX, GSR_CUTOUT_ELLIPSOID = 0, 1
+GSR_CUTOUT_KEEP, GSR_CUTOUT_REMOVE = 0, 1
+GSR_CUTOUT_FRAME, GSR_CUTOUT_SOURCE = 0, 1
 GSR_MAX_INSTANCES, GSR_INSTANCE_RING = 4096, 8
 
 # every symbol include/gsr.h declares (tests/test_abi.py checks the header against this list and the .so)
@@ -24,7 +28,7 @@ EXPORTS = [
     "gsr_create", "gsr_destroy", "gsr_set_stream", "gsr_upload_splats_aos", "gsr_upload_ply_raw", "gsr_upload_ply", "gsr_resize", "gsr_set_band", "gsr_set_row_interleave", "gsr_band_sync_word", "gsr_band_fixup", "gsr_render",
     "gsr_render_async", "gsr_render_async_rgb", "gsr_render_async_fmt", "gsr_output_bytes", "gsr_present_device", "gsr_readback_async", "gsr_peer_export_framebuffers", "gsr_peer_import_framebuffers",
     "gsr_stream_join", "gsr_group_export", "gsr_group_attach", "gsr_group_detach", "gsr_group_set_present", "gsr_readback_rows_async", "gsr_sync", "gsr_framebuffer_device_ptr", "gsr_set_framebuffer_external",
-    "gsr_set_depth_compositing", "gsr_set_instances", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_upload_ply_filtered", "gsr_pick",
+    "gsr_set_depth_compositing", "gsr_set_instances", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_set_cutouts", "gsr_upload_ply_filtered", "gsr_pick",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -50,6 +54,10 @@ class GsrPlyLayout(C.Structure):
 
 class GsrInstance(C.Structure):
     _fields_ = [("first", C.c_uint64), ("count", C.c_uint64), ("to_frame", C.c_float * 12)]
+
+
+class GsrCutout(C.Structure):
+    _fields_ = [("to_local", C.c_float * 12), ("shape", C.c_int32), ("action", C.c_int32), ("space", C.c_int32)]
 
 
 GSR_HISTORY_FRAMES = 512
@@ -119,6 +127,7 @@ def lib():
         L.gsr_set_sh_degree.argtypes = [vp, C.c_int32]
         L.gsr_set_antialiasing.argtypes = [vp, C.c_float]
         L.gsr_set_depth_order.argtypes = [vp, C.c_int32]
+        L.gsr_set_cutouts.argtypes = [vp, C.POINTER(GsrCutout), u32]
         L.gsr_pick.argtypes = [vp, u32, C.c_float, fp]
         L.gsr_get_stats.argtypes = [vp, C.POINTER(GsrStats)]
         L.gsr_get_frame_history.argtypes = [vp, u32, C.POINTER(GsrFrameRecord), C.POINTER(u32)]

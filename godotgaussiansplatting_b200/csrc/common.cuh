@@ -183,8 +183,24 @@ static_assert(sizeof(ProjectionArgs) == 288 && offsetof(ProjectionArgs, lookback
 // aa: the frame is anti-aliased with a.aa_variance > 0 (gsr_set_antialiasing; read at enqueue time, single-context only)
 // depth_words: non-null = the frame is sorted by view depth (gsr_set_depth_order; single-context only): the projection also stores
 // depth_words[g] = depth_order_word(d) beside keys[g] / values[g], d the pair's splat's view depth
+// cutouts: non-null = the frame draws only the splats the set keeps (gsr_set_cutouts; single-context only); the set is copied into the
+// launch's parameters
+struct CutoutArgs;
 int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false, bool aa = false,
-                      uint32_t *depth_words = nullptr);
+                      uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr);
+
+// gsr_set_cutouts: the active set, split by action on the host so that the kernel runs one loop over the KEEP volumes and one over the
+// REMOVE volumes (vol[0, n_keep) then vol[n_keep, n_keep + n_remove)).  It travels by value as the projection's fourth __grid_constant__
+// parameter (840 B): no device buffer, no copy, and frames already enqueued keep their set.
+struct CutoutVolume {
+    float m[12];     // to_local [A | t], column-major 3x4
+    int32_t kind;    // shape (GSR_CUTOUT_BOX / _ELLIPSOID) | space << 1 (GSR_CUTOUT_FRAME / _SOURCE)
+};
+struct CutoutArgs {
+    uint32_t n_keep, n_remove;
+    CutoutVolume vol[GSR_MAX_CUTOUTS];
+};
+static_assert(sizeof(CutoutVolume) == 52 && sizeof(CutoutArgs) == 840, "CutoutArgs layout");
 
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.
@@ -208,7 +224,7 @@ struct InstanceArgs {
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false,
-                                bool aa = false, uint32_t *depth_words = nullptr);
+                                bool aa = false, uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr);
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
 // (mapped page-locked host memory on the frame path)
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream);

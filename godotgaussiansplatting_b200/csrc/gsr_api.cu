@@ -43,7 +43,8 @@ struct gsr_ctx {
     int sh_degree = -1;          // render degree (gsr_set_sh_degree); -1 = the stored degree
     float aa_variance = 0.0f;    // anti-aliasing filter of the next frames (gsr_set_antialiasing); 0 = off
     int32_t depth_order = GSR_DEPTH_ORDER_KEY16;   // sort order of the next frames (gsr_set_depth_order)
-    float4 *records = nullptr;   // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
+    CutoutArgs cutouts = {};     // cutout set of the next frames (gsr_set_cutouts), KEEP volumes first; none = off
+    float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
     uint32_t *vals = nullptr;    // 3 * capacity
@@ -194,6 +195,7 @@ float4 *framebuffer(gsr_ctx *c) { return c->fb_ext ? c->fb_ext : (c->fb_last ? c
 int render_bands(const gsr_ctx *c) { return c->sh_degree < 0 ? c->sh_bands : c->sh_degree + 1; }
 bool reduced_sh(const gsr_ctx *c) { return c->sh_bands < SH_BANDS_MAX || render_bands(c) < SH_BANDS_MAX; }
 bool view_depth_order(const gsr_ctx *c) { return c->depth_order == GSR_DEPTH_ORDER_VIEW_DEPTH; }
+bool cutouts_on(const gsr_ctx *c) { return c->cutouts.n_keep + c->cutouts.n_remove != 0u; }
 
 // The depth-order buffers at the current capacity: the depth words (3 * cap_stride), GSR_BUF_DEPTH_WORDS_UNSORTED while unsorted pairs
 // are kept, and the sorter's depth-order workspace.  On failure nothing is left half allocated.
@@ -529,6 +531,7 @@ GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod)
     if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && row_mod > 1) { set_last_error("gsr_set_row_interleave: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth order is on (single-context only)"); return GSR_ERR_STATE; }
+    if (cutouts_on(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -553,6 +556,7 @@ GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth order is on (single-context only)"); return GSR_ERR_STATE; }
+    if (cutouts_on(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
     c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
     return GSR_OK;
@@ -774,6 +778,9 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         depth_in = c->depth_words + (size_t)half * c->cap_stride;
         depth_alt = c->depth_words + 2ull * c->cap_stride;
     }
+    // gsr_set_cutouts, read here too: the set is copied into the projection's launch parameters (a group frame cannot occur: a set
+    // refuses groups)
+    const CutoutArgs *cut = cutouts_on(c) && !gf ? &c->cutouts : nullptr;
     if (gf) {
         // group mode: the projection is sharded by SPLATS.  This rank projects its slice and stores every pair and record into the
         // memory of the rank that owns it (peer stores over NVLink); the back part then waits for the other sources' flags and packs
@@ -800,10 +807,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         InstanceArgs ia;
         ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
         ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
-        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa, depth_in))) return rc;
+        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa, depth_in, cut))) return rc;
         launches += pa.num_splats ? 1 : 0;
     } else {
-        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa, depth_in))) return rc;
+        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa, depth_in, cut))) return rc;
         launches += pa.num_splats ? 1 : 0;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[1], fs));  // end of the front part
@@ -1099,6 +1106,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_export_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c)) { set_last_error("gsr_peer_export_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
+    if (cutouts_on(c)) { set_last_error("gsr_peer_export_framebuffers: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -1118,6 +1126,7 @@ GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_import_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c)) { set_last_error("gsr_peer_import_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
+    if (cutouts_on(c)) { set_last_error("gsr_peer_import_framebuffers: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -1150,6 +1159,7 @@ GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
     if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_group_export: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c)) { set_last_error("gsr_group_export: depth order is on (single-context only)"); return GSR_ERR_STATE; }
+    if (cutouts_on(c)) { set_last_error("gsr_group_export: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     if (!c->grp.arena) {
@@ -1183,6 +1193,7 @@ GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void
     if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && world > 1) { set_last_error("gsr_group_attach: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c) && world > 1) { set_last_error("gsr_group_attach: depth order is on (single-context only)"); return GSR_ERR_STATE; }
+    if (cutouts_on(c) && world > 1) { set_last_error("gsr_group_attach: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1492,6 +1503,41 @@ GSR_API int gsr_set_depth_order(gsr_ctx *c, int32_t mode) {
         if ((rc = alloc_depth_order(c))) return rc;   // the first switch only (cudaMalloc may synchronise)
     }
     c->depth_order = mode;   // read by the next render_enqueue: frames already enqueued keep their order
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_cutouts(gsr_ctx *c, const gsr_cutout *cutouts, uint32_t n) {
+    if (!c) return GSR_ERR_INVALID;
+    if (n > GSR_MAX_CUTOUTS) { set_last_error("gsr_set_cutouts: %u volumes, at most GSR_MAX_CUTOUTS = %d", n, GSR_MAX_CUTOUTS); return GSR_ERR_INVALID; }
+    if (n > 0 && !cutouts) { set_last_error("gsr_set_cutouts: cutouts == NULL with n = %u", n); return GSR_ERR_INVALID; }
+    for (uint32_t i = 0; i < n; ++i) {
+        const gsr_cutout &v = cutouts[i];
+        for (int e = 0; e < 12; ++e) {
+            if (!(fabsf(v.to_local[e]) <= 3.402823466e38f)) { set_last_error("gsr_set_cutouts: volume %u has a non-finite to_local[%d]", i, e); return GSR_ERR_INVALID; }
+        }
+        if (v.shape != GSR_CUTOUT_BOX && v.shape != GSR_CUTOUT_ELLIPSOID) { set_last_error("gsr_set_cutouts: volume %u: unknown shape %d", i, v.shape); return GSR_ERR_INVALID; }
+        if (v.action != GSR_CUTOUT_KEEP && v.action != GSR_CUTOUT_REMOVE) { set_last_error("gsr_set_cutouts: volume %u: unknown action %d", i, v.action); return GSR_ERR_INVALID; }
+        if (v.space != GSR_CUTOUT_FRAME && v.space != GSR_CUTOUT_SOURCE) { set_last_error("gsr_set_cutouts: volume %u: unknown space %d", i, v.space); return GSR_ERR_INVALID; }
+    }
+    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
+    if (n > 0 && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
+        set_last_error("gsr_set_cutouts: single-context only (no group, peer framebuffers, partial band or row interleave)");
+        return GSR_ERR_STATE;
+    }
+    // split by action, KEEP volumes first (the rule does not depend on the order): the kernel runs one loop over each list
+    CutoutArgs s = {};
+    for (int pass = 0; pass < 2; ++pass) {
+        for (uint32_t i = 0; i < n; ++i) {
+            const gsr_cutout &v = cutouts[i];
+            if (v.action != (pass ? GSR_CUTOUT_REMOVE : GSR_CUTOUT_KEEP)) continue;
+            CutoutVolume &d = s.vol[s.n_keep + s.n_remove];
+            memcpy(d.m, v.to_local, sizeof d.m);
+            d.kind = v.shape | (v.space << 1);
+            if (pass) s.n_remove += 1;
+            else s.n_keep += 1;
+        }
+    }
+    c->cutouts = s;   // read by the next render_enqueue: frames already enqueued keep their set
     return GSR_OK;
 }
 

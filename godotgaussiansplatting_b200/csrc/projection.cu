@@ -184,6 +184,43 @@ __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, flo
     }
 }
 
+// gsr_set_cutouts: is the tested position inside the unit box / sphere of volume v?  u = A p + t (one rounding per operation, in the
+// order of include/gsr.h); IEEE comparisons, so a NaN coordinate is outside.  18 FP32 operations, the volume read with a uniform index.
+__device__ __forceinline__ bool cutout_inside(const CutoutVolume &v, float x, float y, float z) {
+    const float *C = v.m;
+    const float u0 = ((C[0] * x + C[3] * y) + C[6] * z) + C[9];
+    const float u1 = ((C[1] * x + C[4] * y) + C[7] * z) + C[10];
+    const float u2 = ((C[2] * x + C[5] * y) + C[8] * z) + C[11];
+    if (v.kind & 1) return ((u0 * u0 + u1 * u1) + u2 * u2) <= 1.0f;   // GSR_CUTOUT_ELLIPSOID
+    return fabsf(u0) <= 1.0f && fabsf(u1) <= 1.0f && fabsf(u2) <= 1.0f;
+}
+// The rule of gsr_set_cutouts for source position s and frame-space position f: (no KEEP volume, or inside one) and inside no REMOVE
+// volume.  Both loops run over the warp-uniform counts of the host-split set; a lane leaves as soon as its answer is known.
+__device__ __forceinline__ bool cutout_drawn(const CutoutArgs &ct, float s0, float s1, float s2, float f0, float f1, float f2) {
+    bool keep = ct.n_keep == 0u;
+#pragma unroll 1
+    for (uint32_t i = 0; i < ct.n_keep && !keep; ++i) {
+        const CutoutVolume &v = ct.vol[i];
+        const bool src = (v.kind & 2) != 0;   // GSR_CUTOUT_SOURCE
+        keep = cutout_inside(v, src ? s0 : f0, src ? s1 : f1, src ? s2 : f2);
+    }
+    if (!keep) return false;
+    const uint32_t end = ct.n_keep + ct.n_remove;
+#pragma unroll 1
+    for (uint32_t i = ct.n_keep; i < end; ++i) {
+        const CutoutVolume &v = ct.vol[i];
+        const bool src = (v.kind & 2) != 0;
+        if (cutout_inside(v, src ? s0 : f0, src ? s1 : f1, src ? s2 : f2)) return false;
+    }
+    return true;
+}
+// The cutout parameter of a kernel: the set (CutoutArgs) for CUT = true, an empty placeholder otherwise, so that the kernels without
+// cutouts keep their parameter block as it was.
+struct NoCutouts {};
+template <bool CUT> struct CutoutParamT { using type = NoCutouts; };
+template <> struct CutoutParamT<true> { using type = CutoutArgs; };
+template <bool CUT> using CutoutParam = typename CutoutParamT<CUT>::type;
+
 struct LaneOut {  // what one splat contributes (valid when n > 0)
     uint32_t n, x0, y0, w, depth;
     int32_t last_tile;
@@ -203,9 +240,12 @@ struct LaneOut {  // what one splat contributes (valid when n > 0)
 // AA (gsr_set_antialiasing, v = a.aa_variance > 0): the 2D covariance is dilated by v instead of 0.3, and the splat's opacity is
 // multiplied by coef = sqrt(max(0.000025, det(cov_2d) / det(cov_2d + v I))) -- the compensated filter of anti-aliased trainings.  That
 // opacity drives both the radius and the record (DESIGN.md section 5.11).  AA = false is the lane as it always was.
-template <bool QUICK, bool INST = false, bool ORTHO = false, bool AA = false>
+// CUT (gsr_set_cutouts, the set `ct`): right after the frustum cull, a splat the set removes leaves exactly like a culled one (false,
+// n = 0, last_tile = -1) before any other work.  The frame-space position of an instanced splat is formed there with the record's
+// operations (DESIGN.md section 5.13).  CUT = false is the lane as it always was.
+template <bool QUICK, bool INST = false, bool ORTHO = false, bool AA = false, bool CUT = false>
 __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const float *V, const float *cam, const float *At, const float4 pt,
-                                             const float4 ca, const float4 cb, LaneOut &o) {
+                                             const float4 ca, const float4 cb, LaneOut &o, const CutoutParam<CUT> &ct = CutoutParam<CUT>()) {
     const float *P = a.vp + 16;  // X[c][r] = X[4*c + r]
     const int W = a.u.dims[0], H = a.u.dims[1];
     const uint32_t gx = (uint32_t)((W + TILE - 1) / TILE), gy = (uint32_t)((H + TILE - 1) / TILE);
@@ -224,7 +264,16 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
             } else {
             if (clip[0] < -vb || clip[1] < -vb || clip[2] < 0.0f || clip[0] > vb || clip[1] > vb || clip[2] > clip[3]) return false;
             }
-
+            if constexpr (CUT) {   // gsr_set_cutouts: a removed splat is a culled one
+                if constexpr (INST) {   // the record's frame-space position, A * sp + t (same operations as below)
+                    const float w0 = ((At[0] * sp0 + At[3] * sp1) + At[6] * sp2) + At[9];
+                    const float w1 = ((At[1] * sp0 + At[4] * sp1) + At[7] * sp2) + At[10];
+                    const float w2 = ((At[2] * sp0 + At[5] * sp1) + At[8] * sp2) + At[11];
+                    if (!cutout_drawn(ct, sp0, sp1, sp2, w0, w1, w2)) return false;
+                } else {
+                    if (!cutout_drawn(ct, sp0, sp1, sp2, sp0, sp1, sp2)) return false;
+                }
+            }
 
             // :169-174 load-in animation
             const float splat_time = a.u.time - pt.w;
@@ -419,11 +468,14 @@ __device__ __forceinline__ InstanceWarp instance_warp(const ProjectionArgs &a, c
 // record's (frame-space) position with the frame's view matrix -- the depth compositing's d, and -view[2] of project_lane without
 // instances.  The pointer travels in a third parameter, so the first two keep their offsets (a plain pointer parameter, unlike a
 // __grid_constant__ struct, changes the register allocation of the other instantiations).  Never with the compaction path (sharded only).
+// CUT (gsr_set_cutouts): every lane runs project_lane<.., CUT> with the set, which travels in a fourth parameter after DepthArgs for the
+// same reason (the first three keep their offsets); the kernels without cutouts get an empty placeholder there.  Never sharded.
 struct DepthArgs { uint32_t *words = nullptr; };
-template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false, bool DEPTH = false>
+template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false, bool DEPTH = false, bool CUT = false>
 __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
                                                                                        const __grid_constant__ InstanceArgs ia = InstanceArgs(),
-                                                                                       const __grid_constant__ DepthArgs da = DepthArgs()) {
+                                                                                       const __grid_constant__ DepthArgs da = DepthArgs(),
+                                                                                       const __grid_constant__ CutoutParam<CUT> ct = CutoutParam<CUT>()) {
 #ifndef GSR_CPU_EMU
     extern __shared__ __align__(128) unsigned char proj_smem[];
 #else
@@ -490,7 +542,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             // the instance's constants: V_k (16) | cam_k (3) | A_k | t_k (12), 128 B that every lane of the warp reads (L1 broadcasts)
             const float *sk = ia.frame + (size_t)iw.k * INSTANCE_FRAME_FLOATS;
             LaneOut o;
-            if (project_lane<false, true, ORTHO, AA>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false, true, ORTHO, AA, CUT>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], slab[64 + lane], o, ct) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -499,7 +551,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     } else if (!a.fast_reject) {
         if (id < a.num_splats) {
             LaneOut o;
-            if (project_lane<false, false, ORTHO, AA>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o) && o.n) {
+            if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o, ct) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -513,7 +565,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         //      slot, so scan and emit below are unchanged and the emission order stays the splat-id order).
         bool live = false;
         LaneOut q;
-        if (id < a.num_splats) live = project_lane<true, false, ORTHO, AA>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q);
+        if (id < a.num_splats) live = project_lane<true, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q, ct);
         s_res[tid] = make_uint4(0u, 0u, 0u, 0xFFFFFFFFu);
         const uint32_t lmask = __ballot_sync(0xffffffffu, live);
         uint32_t wbase = 0;
@@ -528,7 +580,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
-            if (project_lane<false, false, ORTHO, AA>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o) && o.n) {
+            if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o, ct) && o.n) {
                 float col[3];
                 sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
@@ -1147,20 +1199,31 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 constexpr size_t projection_smem_bytes(int sh_bands) { return proj_slab_bytes(sh_bands) * PROJ_WARPS; }
 static_assert(projection_smem_bytes(SH_BANDS_MAX) == PROJ_SMEM_BYTES, "the degree-3 slab");
 
-template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false, bool DEPTH = false>
+template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false, bool DEPTH = false, bool CUT = false>
 int preload_projection_variant() {
     cudaFuncAttributes fa;
-    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                       (int)projection_smem_bytes(B)));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT>));
     return GSR_OK;
 }
-// projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH>
-template <bool INSTANCED, bool ORTHO, bool AA = false, bool DEPTH = false>
+// projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH, CUT>
+template <bool INSTANCED, bool ORTHO, bool AA = false, bool DEPTH = false, bool CUT = false>
 int preload_projection_bands() {
     int rc;
-    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA, DEPTH>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA, DEPTH>()) ||
-        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA, DEPTH>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA, DEPTH>()))
+    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA, DEPTH, CUT>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA, DEPTH, CUT>()) ||
+        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA, DEPTH, CUT>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA, DEPTH, CUT>()))
+        return rc;
+    return GSR_OK;
+}
+// the cutout variants projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH, true> of every (ORTHO, AA, DEPTH)
+template <bool INSTANCED>
+int preload_projection_cutouts() {
+    int rc;
+    if ((rc = preload_projection_bands<INSTANCED, false, false, false, true>()) || (rc = preload_projection_bands<INSTANCED, true, false, false, true>()) ||
+        (rc = preload_projection_bands<INSTANCED, false, true, false, true>()) || (rc = preload_projection_bands<INSTANCED, true, true, false, true>()) ||
+        (rc = preload_projection_bands<INSTANCED, false, false, true, true>()) || (rc = preload_projection_bands<INSTANCED, true, false, true, true>()) ||
+        (rc = preload_projection_bands<INSTANCED, false, true, true, true>()) || (rc = preload_projection_bands<INSTANCED, true, true, true, true>()))
         return rc;
     return GSR_OK;
 }
@@ -1194,6 +1257,8 @@ int preload_projection_kernels() {
         (rc = preload_projection_bands<false, false, true, true>()) || (rc = preload_projection_bands<true, false, true, true>()) ||
         (rc = preload_projection_bands<false, true, true, true>()) || (rc = preload_projection_bands<true, true, true, true>()))
         return rc;
+    // the cutout variants (gsr_set_cutouts) of all of the above
+    if ((rc = preload_projection_cutouts<false>()) || (rc = preload_projection_cutouts<true>())) return rc;
     return GSR_OK;
 }
 uint32_t projection_scatter_blocks(uint32_t count) { return count ? (count + PROJ_THREADS - 1) / PROJ_THREADS : 1u; }   // an empty slice still publishes its flags
@@ -1207,40 +1272,48 @@ int launch_projection_scatter(const ProjectionArgs &frame_args, const ScatterPee
     return GSR_OK;
 }
 
-// projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH> for B = sh_bands (the orthographic, anti-aliased and depth-order frames: single-context
-// only, never sharded)
-template <bool INSTANCED, bool ORTHO, bool AA, bool DEPTH>
-void launch_projection_bands(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, uint32_t blocks, cudaStream_t stream, int sh_bands) {
+// projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT> for B = sh_bands (the orthographic, anti-aliased, depth-order and cutout frames:
+// single-context only, never sharded)
+template <bool INSTANCED, bool ORTHO, bool AA, bool DEPTH, bool CUT>
+void launch_projection_bands(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutParam<CUT> &ct, uint32_t blocks,
+                             cudaStream_t stream, int sh_bands) {
     switch (sh_bands) {
-        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia, DepthArgs{dw}); break;
-        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia, DepthArgs{dw}); break;
-        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia, DepthArgs{dw}); break;
-        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA, DEPTH><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia, DepthArgs{dw}); break;
+        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia, DepthArgs{dw}, ct); break;
     }
 }
-template <bool INSTANCED, bool DEPTH>
-void launch_projection_modes(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, uint32_t blocks, cudaStream_t stream, int sh_bands,
-                             bool ortho, bool aa) {
+template <bool INSTANCED, bool DEPTH, bool CUT>
+void launch_projection_modes(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutParam<CUT> &ct, uint32_t blocks,
+                             cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
     if (ortho) {
-        if (aa) launch_projection_bands<INSTANCED, true, true, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
-        else launch_projection_bands<INSTANCED, true, false, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
+        if (aa) launch_projection_bands<INSTANCED, true, true, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
+        else launch_projection_bands<INSTANCED, true, false, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
     } else {
-        if (aa) launch_projection_bands<INSTANCED, false, true, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
-        else launch_projection_bands<INSTANCED, false, false, DEPTH>(a, ia, dw, blocks, stream, sh_bands);
+        if (aa) launch_projection_bands<INSTANCED, false, true, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
+        else launch_projection_bands<INSTANCED, false, false, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
     }
+}
+template <bool INSTANCED, bool CUT>
+void launch_projection_depth(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutParam<CUT> &ct, uint32_t blocks,
+                             cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
+    if (dw) launch_projection_modes<INSTANCED, true, CUT>(a, ia, dw, ct, blocks, stream, sh_bands, ortho, aa);
+    else launch_projection_modes<INSTANCED, false, CUT>(a, ia, nullptr, ct, blocks, stream, sh_bands, ortho, aa);
 }
 template <bool INSTANCED>
-void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, uint32_t blocks, cudaStream_t stream, int sh_bands,
-                               bool ortho, bool aa) {
-    if (dw) launch_projection_modes<INSTANCED, true>(a, ia, dw, blocks, stream, sh_bands, ortho, aa);
-    else launch_projection_modes<INSTANCED, false>(a, ia, nullptr, blocks, stream, sh_bands, ortho, aa);
+void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutArgs *cut, uint32_t blocks,
+                               cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
+    if (cut) launch_projection_depth<INSTANCED, true>(a, ia, dw, *cut, blocks, stream, sh_bands, ortho, aa);
+    else launch_projection_depth<INSTANCED, false>(a, ia, dw, NoCutouts(), blocks, stream, sh_bands, ortho, aa);
 }
 
-int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa, uint32_t *depth_words) {
+int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa, uint32_t *depth_words,
+                      const CutoutArgs *cutouts) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho || aa || depth_words) {
-        launch_projection_special<false>(a, InstanceArgs(), depth_words, blocks, stream, sh_bands, ortho, aa);
+    if (ortho || aa || depth_words || cutouts) {
+        launch_projection_special<false>(a, InstanceArgs(), depth_words, cutouts, blocks, stream, sh_bands, ortho, aa);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }
@@ -1261,11 +1334,11 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
 }
 
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho, bool aa,
-                                uint32_t *depth_words) {
+                                uint32_t *depth_words, const CutoutArgs *cutouts) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho || aa || depth_words) {
-        launch_projection_special<true>(a, ia, depth_words, blocks, stream, sh_bands, ortho, aa);
+    if (ortho || aa || depth_words || cutouts) {
+        launch_projection_special<true>(a, ia, depth_words, cutouts, blocks, stream, sh_bands, ortho, aa);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }

@@ -73,6 +73,7 @@ class GaussianSplattingRasterizer:
         has_filter_3d = self._layout is not None and self._layout.filter_3d >= 0
         self._antialiasing = float(antialiasing) if antialiasing is not None else (0.1 if has_filter_3d else 0.0)
         self._depth_order = int(depth_order)
+        self._cutouts = []   # gsr_cutout entries of set_cutouts, applied again by init_gpu
         self._clock = clock or (lambda: _time.monotonic())
         self._t0 = self._clock()
         self.tile_dims = (0, 0)
@@ -125,6 +126,8 @@ class GaussianSplattingRasterizer:
             self.set_antialiasing(self._antialiasing)
         if self._depth_order:
             self.set_depth_order(self._depth_order)
+        if self._cutouts:
+            self._apply_cutouts()
         self.should_terminate_thread[0] = False
         self.num_splats_loaded[0] = 0
         if not load:
@@ -202,6 +205,25 @@ class GaussianSplattingRasterizer:
         if self._ctx:
             _lib.check(_lib.lib().gsr_set_depth_order(self._ctx, m), "gsr_set_depth_order")
         self._depth_order = m
+
+    def set_cutouts(self, cutouts) -> None:
+        """Boxes and ellipsoids that crop the cloud or cut splats away in the frames rendered from now on (include/gsr.h
+        gsr_set_cutouts).  cutouts: iterable of (transform, shape, action, space), at most GSR_MAX_CUTOUTS, where transform is a Godot
+        Transform3D in matrix form -- a (3, 4) array [basis | origin], or (4, 4) -- that maps the unit cube [-1, 1]^3
+        (GSR_CUTOUT_BOX) or the unit sphere (GSR_CUTOUT_ELLIPSOID) onto the volume: in Godot world space for GSR_CUTOUT_FRAME, in the
+        asset's own Godot space (the space of set_instances' ranges) for GSR_CUTOUT_SOURCE.  action: GSR_CUTOUT_KEEP or
+        GSR_CUTOUT_REMOVE.  A splat is kept or removed whole, by its centre.  An empty list switches cutouts off."""
+        items = list(cutouts)
+        self._cutouts = [(cutout_to_local(t, self.basis_override), int(shape), int(action), int(space)) for t, shape, action, space in items]
+        if self._ctx:
+            self._apply_cutouts()
+
+    def _apply_cutouts(self) -> None:
+        arr = (_lib.GsrCutout * max(1, len(self._cutouts)))()
+        for k, (to_local, shape, action, space) in enumerate(self._cutouts):
+            arr[k].to_local[:] = [float(v) for v in to_local.T.reshape(12)]
+            arr[k].shape, arr[k].action, arr[k].space = shape, action, space
+        _lib.check(_lib.lib().gsr_set_cutouts(self._ctx, arr, len(self._cutouts)), "gsr_set_cutouts")
 
     def _emit_loaded(self):
         self.is_loaded = True
@@ -427,6 +449,24 @@ def godot_to_frame(transform, basis_override) -> np.ndarray:
     Fb[:3, :3] = np.diag([-1.0, -1.0, 1.0]) @ np.asarray(basis_override, dtype=np.float64).T
     M = np.eye(4) + Fb @ D @ np.linalg.inv(Fb)
     return M[:3].astype(np.float32)
+
+
+def cutout_to_local(transform, basis_override) -> np.ndarray:
+    """A cutout volume's Godot Transform3D T (matrix form: a point q of the unit shape, in the volume's own Godot axes -> its Godot
+    position) -> the (3, 4) float32 [A | t] of gsr_cutout.to_local (a tested position -> q).  A Godot position p sits at F B p in frame
+    space (F = diag(-1, -1, 1), B = basis_override: the convention of godot_to_frame), so to_local = (F B T)^-1.  It is composed and
+    inverted in float64 and narrowed to float32 once.  With B a signed permutation (the identity, the usual PLY up-axis flips) this is
+    also (F B T B^-1 F)^-1, the instance convention, since F B maps the unit cube and sphere onto themselves.  A singular transform
+    raises LinAlgError."""
+    T = np.asarray(transform, dtype=np.float64)
+    if T.shape == (4, 4):
+        T = T[:3]
+    assert T.shape == (3, 4), T.shape
+    Fb = np.eye(4)
+    Fb[:3, :3] = np.diag([-1.0, -1.0, 1.0]) @ np.asarray(basis_override, dtype=np.float64).T
+    M = np.eye(4)
+    M[:3] = T
+    return np.linalg.inv(Fb @ M)[:3].astype(np.float32)
 
 
 def sort_pairs(keys: np.ndarray, values: np.ndarray | None = None, device: int = 0):

@@ -379,6 +379,42 @@ GSR_API int gsr_set_antialiasing(gsr_ctx *ctx, float filter_variance);
 #define GSR_DEPTH_ORDER_VIEW_DEPTH 1
 GSR_API int gsr_set_depth_order(gsr_ctx *ctx, int32_t mode);
 
+/* ---- Splat cutouts (no reference counterpart: the reference draws every splat of the cloud).  Up to GSR_MAX_CUTOUTS boxes and
+ *      ellipsoids that crop the cloud (KEEP) or cut splats away (REMOVE) -- backgrounds, floaters, the ground a capture stood on,
+ *      runtime cutaways -- without touching the uploaded data.  A splat is drawn iff
+ *        - no KEEP volume is set, or its tested position is inside at least one KEEP volume, and
+ *        - its tested position is inside no REMOVE volume.
+ *      The order of the volumes does not matter.  The test is on the splat's CENTRE: a splat is kept or removed whole, its footprint
+ *      is not clipped at the volume's boundary.  A removed splat is treated exactly like a frustum-culled one: no record, no pairs,
+ *      no share of M, V or the last tile: the sort and the compositor see fewer pairs (DESIGN.md section 5.7 has measured costs).
+ *      Tested position, in float32 with one rounding per operation: u[r] = ((C[r] x + C[3+r] y) + C[6+r] z) + C[9+r] with C =
+ *      to_local ([A | t], column-major 3x4 like gsr_instance.to_frame: the tested position -> the unit shape's space) and
+ *        - GSR_CUTOUT_SOURCE: (x, y, z) = the splat's source coordinates, position * model_scale (before any instance transform);
+ *        - GSR_CUTOUT_FRAME: (x, y, z) = the record's position words: the source coordinates without instances, A * sp + t with them
+ *          (the position gsr_pick returns and depth compositing uses).
+ *      Without instances the two spaces coincide; with instances a SOURCE volume is an asset-space crop that travels with every copy
+ *      of the asset, a FRAME volume a world-space cutaway.  Inside a box: |u0| <= 1 && |u1| <= 1 && |u2| <= 1 (the faces included);
+ *      inside an ellipsoid: ((u0 u0 + u1 u1) + u2 u2) <= 1.  Comparisons are IEEE: a NaN coordinate is outside every volume.  A
+ *      singular to_local is allowed (a flat slab, an infinite prism).
+ *      The array is copied and read when a frame is enqueued: frames already enqueued keep their set.  The call never synchronises,
+ *      allocates nothing and copies nothing to the device (the set travels with the projection's launch parameters).  n == 0 switches
+ *      cutouts off: the default frame, bit for bit.  gsr_resize keeps the set.  GSR_ERR_INVALID, previous set kept: n >
+ *      GSR_MAX_CUTOUTS, cutouts == NULL with n > 0, a non-finite to_local entry, an unknown shape, action or space.  Single-context
+ *      only: a non-empty set returns GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those
+ *      calls (and gsr_group_export) fail with GSR_ERR_STATE while a set is active. ---- */
+#define GSR_MAX_CUTOUTS 16
+#define GSR_CUTOUT_BOX 0        /* inside: |u0| <= 1 && |u1| <= 1 && |u2| <= 1 */
+#define GSR_CUTOUT_ELLIPSOID 1  /* inside: ((u0*u0 + u1*u1) + u2*u2) <= 1 */
+#define GSR_CUTOUT_KEEP 0       /* action: with any KEEP volume set, only splats inside one are drawn */
+#define GSR_CUTOUT_REMOVE 1     /* action: splats inside are not drawn */
+#define GSR_CUTOUT_FRAME 0      /* space: the record's frame-space position */
+#define GSR_CUTOUT_SOURCE 1     /* space: the splat's source coordinates (before an instance transform) */
+typedef struct gsr_cutout {
+    float to_local[12];         /* [A | t], column-major 3x4: tested position -> the unit shape's space */
+    int32_t shape, action, space;
+} gsr_cutout;
+GSR_API int gsr_set_cutouts(gsr_ctx *ctx, const gsr_cutout *cutouts, uint32_t n);
+
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
  *      num_tile_splats -- persistent across calls exactly like the reference's storage buffer.
