@@ -14,6 +14,7 @@ LIB_PATH = os.environ.get("GSR_LIB_PATH") or os.path.join(HERE, "libgsr.so")  # 
 GSR_OK, GSR_ERR_INVALID, GSR_ERR_CUDA, GSR_ERR_OOM, GSR_ERR_STATE, GSR_ERR_OVERFLOW = range(6)
 GSR_FLAG_REFERENCE_QUIRKS, GSR_FLAG_FIXED_RANGES, GSR_FLAG_FAST_REJECT, GSR_FLAG_STATIC_CAPACITY, GSR_FLAG_UNCONTRACTED_BLEND = 0x1, 0x2, 0x4, 0x8, 0x10
 GSR_FLAG_ORTHOGRAPHIC = 0x20
+GSR_FLAG_SH_HALF = 0x40   # SH coefficients stored as IEEE binary16 (include/gsr.h)
 (GSR_BUF_RECORDS, GSR_BUF_KEYS, GSR_BUF_VALUES, GSR_BUF_BOUNDS, GSR_BUF_KEYS_UNSORTED, GSR_BUF_VALUES_UNSORTED,
  GSR_BUF_FRAMEBUFFER, GSR_BUF_COMPOSITOR_TRACE, GSR_BUF_COMPOSITOR_TRACE_COUNT, GSR_BUF_INSTANCES, GSR_BUF_SPLATS, GSR_BUF_DEPTH_WORDS_UNSORTED,
  GSR_BUF_INSTANCE_APPEARANCE) = range(13)

@@ -15,11 +15,57 @@ constexpr int PROJ_THREADS = 256;   // gsplat_projection.glsl:31 local_size_x
 
 // SH storage by degree (gsr_config.sh_bands): B bands = degree + 1 hold K = B^2 coefficients per channel, stored coefficient-major RGB in
 // P = ceil(3K / 4) float4 planes after planes 0-2.  B = 1, 2, 3, 4 -> P = 1, 3, 7, 12 (64 / 96 / 160 / 240 B per splat).
+// A binary16 store (GSR_FLAG_SH_HALF, `half`) packs the same 3K values as IEEE halves, 8 per 16-byte plane: value i in SH plane i >> 3,
+// slot i & 7 (slot 0 = the low half of the plane's first word), slots past 3K = +0.  P_h = ceil(3K / 8) = 1, 2, 4, 6 (64 / 80 / 112 /
+// 144 B per splat).  Every plane of either format is 16 B per splat, so plane k of splat s is always float4 k * plane_stride + s.
 constexpr int SH_BANDS_MAX = 4;
 __host__ __device__ constexpr int sh_coeffs(int bands) { return bands * bands; }
-__host__ __device__ constexpr int sh_planes(int bands) { return (3 * bands * bands + 3) / 4; }
-__host__ __device__ constexpr int soa_planes(int bands) { return 3 + sh_planes(bands); }
+__host__ __device__ constexpr int sh_planes(int bands, bool half = false) { return half ? (3 * bands * bands + 7) / 8 : (3 * bands * bands + 3) / 4; }
+__host__ __device__ constexpr int soa_planes(int bands, bool half = false) { return 3 + sh_planes(bands, half); }
 static_assert(soa_planes(SH_BANDS_MAX) == NUM_PLANES, "a degree-3 store is the 60-float Splat");
+static_assert(soa_planes(SH_BANDS_MAX, true) * 16 == 144, "a degree-3 binary16 store is 144 B per splat");
+
+// binary16 SH store: h(c) = c rounded to binary16 (round to nearest even, subnormals and signed zeros kept); finite or infinite values
+// beyond +-65504 saturate to +-65504, NaN stays a NaN.  The decode of a half is exact.
+#ifndef GSR_CPU_EMU
+__device__ __forceinline__ uint32_t half_bits_rn(float x) {   // IEEE conversion: overflow gives +-inf, NaN a NaN
+    unsigned short h;
+    asm("cvt.rn.f16.f32 %0, %1;" : "=h"(h) : "f"(x));
+    return h;
+}
+__device__ __forceinline__ float half_bits_to_float(uint32_t h) {   // the low 16 bits
+    float f;
+    asm("cvt.f32.f16 %0, %1;" : "=f"(f) : "h"((unsigned short)h));
+    return f;
+}
+#else  // tests/kernel_emu (CPU logic pre-flight): the same two conversions in integer arithmetic, bit for bit
+inline uint32_t half_bits_rn(float x) {   // round to nearest even, subnormal halves kept, overflow to +-inf, NaN to a quiet NaN
+    const uint32_t u = __float_as_uint(x), s = (u >> 16) & 0x8000u, a = u & 0x7FFFFFFFu;
+    if (a > 0x7F800000u) return s | 0x7E00u | ((a >> 13) & 0x3FFu);
+    if (a >= 0x477FF000u) return s | 0x7C00u;                      // |x| >= 65520 (and inf) rounds to inf
+    if (a < 0x38800000u) {                                         // below 2^-14: a subnormal half (or zero), in units of 2^-24
+        const uint32_t m = (a >> 23) ? ((a & 0x7FFFFFu) | 0x800000u) : (a & 0x7FFFFFu);
+        const int e = (a >> 23) ? (int)(a >> 23) : 1;              // x = m * 2^(e - 150) = m * 2^(e - 126) units
+        const int sh = 126 - e;                                    // >= 14
+        if (sh > 24) return s;                                     // below 2^-25 (a tie at 2^-25 rounds to even 0 too)
+        const uint32_t q = m >> sh, rem = m & ((1u << sh) - 1u), half = 1u << (sh - 1);
+        return s | (q + ((rem > half || (rem == half && (q & 1u))) ? 1u : 0u));
+    }
+    uint32_t h = (a - 0x38000000u) >> 13;                          // rebias 127 -> 15, keep 10 mantissa bits
+    const uint32_t rem = a & 0x1FFFu;
+    if (rem > 0x1000u || (rem == 0x1000u && (h & 1u))) h += 1u;   // a carry moves into the exponent, as it should
+    return s | h;
+}
+inline float half_bits_to_float(uint32_t h) {
+    const uint32_t s = (h & 0x8000u) << 16, e = (h >> 10) & 0x1Fu, m = h & 0x3FFu;
+    if (e == 0x1Fu) return __uint_as_float(s | 0x7F800000u | (m << 13));
+    if (e == 0u) { const float f = (float)m * 0x1p-24f; return s ? -f : f; }   // exact: m < 2^10
+    return __uint_as_float(s | ((e + 112u) << 23) | (m << 13));
+}
+#endif
+// (the comparison is false for NaN, so a NaN reaches the conversion unchanged: no fminf / fmaxf, which would make it the bound)
+__device__ __forceinline__ uint32_t sh_half(float c) { return half_bits_rn(fabsf(c) > 65504.0f ? copysignf(65504.0f, c) : c); }
+__device__ __forceinline__ uint32_t sh_half2(float lo, float hi) { return sh_half(lo) | (sh_half(hi) << 16); }
 
 // ---------------------------------------------------------------------------------------------
 // error plumbing
@@ -186,8 +232,9 @@ static_assert(sizeof(ProjectionArgs) == 288 && offsetof(ProjectionArgs, lookback
 // cutouts: non-null = the frame draws only the splats the set keeps (gsr_set_cutouts; single-context only); the set is copied into the
 // launch's parameters
 struct CutoutArgs;
+// sh_half: the store holds binary16 SH planes (GSR_FLAG_SH_HALF; single-context only)
 int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false, bool aa = false,
-                      uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr);
+                      uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr, bool sh_half = false);
 
 // gsr_set_cutouts: the active set, split by action on the host so that the kernel runs one loop over the KEEP volumes and one over the
 // REMOVE volumes (vol[0, n_keep) then vol[n_keep, n_keep + n_remove)).  It travels by value as the projection's fourth __grid_constant__
@@ -228,7 +275,7 @@ struct InstanceArgs {
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false,
-                                bool aa = false, uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr);
+                                bool aa = false, uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr, bool sh_half = false);
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
 // (mapped page-locked host memory on the frame path).  With an appearance (count x 8 floats, same memory) its rows go to appearance_out.
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream,
@@ -340,16 +387,19 @@ int launch_tile_order(const uint2 *bounds, int32_t tile_begin, int32_t row_step,
 constexpr gsr_ply_layout PLY_LAYOUT_3DGS = {62u, 3u, 0, 6, 9, 54, 55, 58};
 // PLY vertices of any layout -> the first `planes` (= soa_planes(store bands)) SoA planes
 // filter_3d: index of Mip-Splatting's per-splat `filter_3D` property in a vertex (gsr_upload_ply_filtered), -1 = none
+// sh_half (GSR_FLAG_SH_HALF): the SH planes are written as packed binary16 values (then planes = soa_planes(store bands, true))
 int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
-                      uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d = -1);
+                      uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d = -1, bool sh_half = false);
 // present.cu: RGBA32F frame -> GSR_OUT_* (| GSR_OUT_SRGB_TO_LINEAR)
 int launch_present(const float4 *rgba, void *out, uint64_t pixels, int format, cudaStream_t stream);
 size_t present_bytes_per_pixel(int format);
-int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, int planes, cudaStream_t stream);
+int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, int planes, cudaStream_t stream,
+                      bool sh_half = false);
 
 // cudaFuncGetAttributes on every kernel of a file: defeats lazy module loading before the first frame
 int preload_group_kernels();
 int preload_projection_kernels();
+int preload_projection_half_kernels();   // the binary16-store variants (GSR_FLAG_SH_HALF contexts only)
 int preload_sort_kernels();
 int preload_ranges_kernels();
 int launch_frame_clear(FrameState *frame, unsigned long long *links, uint32_t n_links, uint2 *bounds, uint32_t n_bounds, cudaStream_t stream);

@@ -38,7 +38,7 @@ struct gsr_ctx {
     uint64_t max_splats = 0, capacity = 0, plane_stride = 0, num_splats = 0;
     uint64_t cap_stride = 0;     // capacity rounded up to 1024 pairs: distance between the three pair buffers (keeps each 16-byte aligned)
     cudaStream_t stream = nullptr, own_stream = nullptr;
-    float4 *soa = nullptr;       // soa_planes(sh_bands) planes x plane_stride (15 for a degree-3 store)
+    float4 *soa = nullptr;       // soa_planes(sh_bands, sh_half) planes x plane_stride (15 for a degree-3 float store)
     int sh_bands = SH_BANDS_MAX; // SH bands the store keeps (gsr_config.sh_bands)
     int sh_degree = -1;          // render degree (gsr_set_sh_degree); -1 = the stored degree
     float aa_variance = 0.0f;    // anti-aliasing filter of the next frames (gsr_set_antialiasing); 0 = off
@@ -216,8 +216,10 @@ void group_detach(gsr_ctx *c) {
 float4 *framebuffer(gsr_ctx *c) { return c->fb_ext ? c->fb_ext : (c->fb_last ? c->fb_last : c->fb); }
 
 // SH bands the next frame evaluates, and whether the context stores or renders fewer than 4 (single-context only, like depth compositing)
+// (GSR_FLAG_SH_HALF: a binary16 store is single-context only too -- the sharded, scatter and band kernels read float stores)
 int render_bands(const gsr_ctx *c) { return c->sh_degree < 0 ? c->sh_bands : c->sh_degree + 1; }
-bool reduced_sh(const gsr_ctx *c) { return c->sh_bands < SH_BANDS_MAX || render_bands(c) < SH_BANDS_MAX; }
+bool sh_half(const gsr_ctx *c) { return (c->flags & GSR_FLAG_SH_HALF) != 0u; }
+bool reduced_sh(const gsr_ctx *c) { return c->sh_bands < SH_BANDS_MAX || render_bands(c) < SH_BANDS_MAX || sh_half(c); }
 bool view_depth_order(const gsr_ctx *c) { return c->depth_order == GSR_DEPTH_ORDER_VIEW_DEPTH; }
 bool cutouts_on(const gsr_ctx *c) { return c->cutouts.n_keep + c->cutouts.n_remove != 0u; }
 
@@ -308,7 +310,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     if (!(c->flags & (GSR_FLAG_REFERENCE_QUIRKS | GSR_FLAG_FIXED_RANGES))) c->flags |= GSR_FLAG_REFERENCE_QUIRKS;
     c->max_splats = cfg->max_splats;
     c->sh_bands = cfg->sh_bands ? (int)cfg->sh_bands : SH_BANDS_MAX;
-    const uint64_t planes = (uint64_t)soa_planes(c->sh_bands);
+    const uint64_t planes = (uint64_t)soa_planes(c->sh_bands, sh_half(c));
     const uint64_t factor = cfg->dup_capacity_factor ? cfg->dup_capacity_factor : 10;  // rasterizer.gd:79
     c->dup_factor = factor;
     c->capacity_max = (1ull << 30) - 1;  // look-back words carry 30-bit counts
@@ -392,7 +394,8 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     // load every kernel now: with lazy module loading a FIRST launch may have to synchronise with the device, which must not
     // happen on the frame path (and would deadlock a group whose ranks share one process: a wait kernel spins meanwhile)
     if ((rc = preload_group_kernels()) || (rc = preload_projection_kernels()) || (rc = preload_sort_kernels()) || (rc = preload_ranges_kernels()) ||
-        (rc = preload_ingest_kernels()) || (rc = preload_present_kernels()) || (rc = preload_composite_kernels())) { free_ctx(c); return rc; }
+        (rc = preload_ingest_kernels()) || (rc = preload_present_kernels()) || (rc = preload_composite_kernels()) ||
+        (sh_half(c) && (rc = preload_projection_half_kernels()))) { free_ctx(c); return rc; }
     cudaError_t e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_last_error("init sync -> %s", cudaGetErrorString(e)); free_ctx(c); return GSR_ERR_CUDA; }
     *out = c;
@@ -426,7 +429,7 @@ GSR_API int gsr_upload_splats_aos(gsr_ctx *c, const float *splat60, uint64_t fir
     while (done < count) {
         const uint64_t m = (count - done) < per ? (count - done) : per;
         GSR_CUDA_TRY(cudaMemcpyAsync(c->staging, splat60 + (done * 60ull), m * 240ull, cudaMemcpyHostToDevice, c->stream));
-        if ((rc = launch_aos_to_soa(c->staging, m, c->soa, c->plane_stride, first + done, soa_planes(c->sh_bands), c->stream))) return rc;
+        if ((rc = launch_aos_to_soa(c->staging, m, c->soa, c->plane_stride, first + done, soa_planes(c->sh_bands, sh_half(c)), c->stream, sh_half(c)))) return rc;
         done += m;
     }
     GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));  // the caller may free/reuse splat60 (buffer_update semantics)
@@ -449,7 +452,7 @@ static int upload_ply(gsr_ctx *c, const float *ply, const gsr_ply_layout &lay, u
         const uint64_t m = (count - done) < per ? (count - done) : per;
         GSR_CUDA_TRY(cudaMemcpyAsync(c->staging, ply + done * nprops, m * nprops * sizeof(float), cudaMemcpyHostToDevice, c->stream));
         if ((rc = launch_ply_to_soa(reinterpret_cast<const float *>(c->staging), lay, m, creation_time, c->soa, c->plane_stride, first + done,
-                                    soa_planes(c->sh_bands), c->stream, filter_3d))) return rc;
+                                    soa_planes(c->sh_bands, sh_half(c)), c->stream, filter_3d, sh_half(c)))) return rc;
         done += m;
     }
     GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -552,7 +555,7 @@ GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod)
     if (!c || row_mod < 1 || row_rem < 0 || row_rem >= row_mod) { set_last_error("gsr_set_row_interleave: need 0 <= rem < mod"); return GSR_ERR_INVALID; }
     if (c->depth_out && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && row_mod > 1) { set_last_error("gsr_set_row_interleave: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && row_mod > 1) { set_last_error("gsr_set_row_interleave: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (cutouts_on(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
@@ -577,7 +580,7 @@ GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (row_begin < 0 || row_end > c->tiles_y || row_begin > row_end) { set_last_error("band [%d,%d) outside [0,%d]", row_begin, row_end, c->tiles_y); return GSR_ERR_INVALID; }
     if (c->depth_out && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (cutouts_on(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
@@ -835,10 +838,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         ia.frame = c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS;
         ia.desc = c->inst.desc; ia.warp_inst = c->inst.warps;
         ia.appearance = c->inst.app ? instance_appearance_table(c->inst, half) : nullptr;
-        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa, depth_in, cut))) return rc;
+        if ((rc = launch_projection_instanced(pa, ia, fs, render_bands(c), ortho, aa, depth_in, cut, sh_half(c)))) return rc;
         launches += pa.num_splats ? 1 : 0;
     } else {
-        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa, depth_in, cut))) return rc;
+        if ((rc = launch_projection(pa, fs, render_bands(c), ortho, aa, depth_in, cut, sh_half(c)))) return rc;
         launches += pa.num_splats ? 1 : 0;
     }
     GSR_CUDA_TRY(cudaEventRecord(ev[1], fs));  // end of the front part
@@ -1131,7 +1134,7 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
     if (c->depth_out) { set_last_error("gsr_peer_export_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n) { set_last_error("gsr_peer_export_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_export_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c)) { set_last_error("gsr_peer_export_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (cutouts_on(c)) { set_last_error("gsr_peer_export_framebuffers: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
@@ -1151,7 +1154,7 @@ GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
     if (c->depth_out) { set_last_error("gsr_peer_import_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n) { set_last_error("gsr_peer_import_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_import_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c)) { set_last_error("gsr_peer_import_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (cutouts_on(c)) { set_last_error("gsr_peer_import_framebuffers: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
@@ -1184,7 +1187,7 @@ constexpr uint32_t GROUP_MAGIC = 0x47535247u;  // "GRSG"
 GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
     if (!c || !blob) return GSR_ERR_INVALID;
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_group_export: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f) { set_last_error("gsr_group_export: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c)) { set_last_error("gsr_group_export: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (cutouts_on(c)) { set_last_error("gsr_group_export: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
@@ -1218,7 +1221,7 @@ GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void
     if (!c->grp.arena || !c->fb) { set_last_error("gsr_group_attach before gsr_group_export"); return GSR_ERR_STATE; }
     if (c->depth_out && world > 1) { set_last_error("gsr_group_attach: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
     if (c->inst.n && world > 1) { set_last_error("gsr_group_attach: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
+    if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
     if (c->aa_variance > 0.0f && world > 1) { set_last_error("gsr_group_attach: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
     if (view_depth_order(c) && world > 1) { set_last_error("gsr_group_attach: depth order is on (single-context only)"); return GSR_ERR_STATE; }
     if (cutouts_on(c) && world > 1) { set_last_error("gsr_group_attach: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
@@ -1746,7 +1749,7 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
         case GSR_BUF_FRAMEBUFFER: src = framebuffer(c); avail = sizeof(float4) * (size_t)c->width * c->height; break;
         case GSR_BUF_COMPOSITOR_TRACE: src = c->trace; avail = c->trace ? sizeof(ulonglong4) * (size_t)c->trace_cap : 0; break;
         case GSR_BUF_COMPOSITOR_TRACE_COUNT: src = c->trace_count; avail = c->trace_count ? sizeof(uint32_t) : 0; break;
-        case GSR_BUF_SPLATS: src = c->soa; avail = sizeof(float4) * (size_t)soa_planes(c->sh_bands) * c->plane_stride; break;
+        case GSR_BUF_SPLATS: src = c->soa; avail = sizeof(float4) * (size_t)soa_planes(c->sh_bands, sh_half(c)) * c->plane_stride; break;
         case GSR_BUF_INSTANCES: {   // host copy: no device involved
             avail = sizeof(float) * INSTANCE_XFORM_FLOATS * c->inst.n;
             if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }

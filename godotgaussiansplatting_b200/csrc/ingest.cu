@@ -14,6 +14,9 @@ constexpr int SPLATS_PER_BLOCK = 128;
 
 // `planes` = soa_planes(store bands): the SH planes past them are not stored, and the floats of the last stored SH plane past the store's
 // 3K coefficients are written as 0 (the AoS struct holds the next degree's coefficients there).
+// HALF (GSR_FLAG_SH_HALF; planes = soa_planes(store bands, true)): SH plane p holds the 8 values 8p .. 8p + 7 of the struct's SH floats
+// rounded to binary16 (sh_half), values past 3K as +0.
+template <bool HALF = false>
 __global__ void __launch_bounds__(256) aos_to_soa_kernel(const float4 *__restrict__ aos, uint64_t count, float4 *__restrict__ soa,
                                                          uint64_t plane_stride, uint64_t first, int planes = NUM_PLANES) {
     __shared__ float4 s[SPLATS_PER_BLOCK * NUM_PLANES];
@@ -22,6 +25,28 @@ __global__ void __launch_bounds__(256) aos_to_soa_kernel(const float4 *__restric
     const float4 *src = aos + s0 * NUM_PLANES;
     for (uint32_t i = threadIdx.x; i < here * NUM_PLANES; i += blockDim.x) s[i] = src[i];  // coalesced AoS read
     __syncthreads();
+    if constexpr (HALF) {
+        // SH values of the store: 3K = 3, 12, 27, 48 for 1..4 bands
+        const uint32_t nvals = planes == soa_planes(1, true) ? 3u : planes == soa_planes(2, true) ? 12u : planes == soa_planes(3, true) ? 27u : 48u;
+        const float *sf = reinterpret_cast<const float *>(s);
+        for (uint32_t i = threadIdx.x; i < here * (uint32_t)planes; i += blockDim.x) {
+            const uint32_t plane = i / here, k = i - plane * here;
+            float4 v;
+            if (plane < 3u) {
+                v = s[k * NUM_PLANES + plane];
+            } else {
+                const uint32_t v0 = 8u * (plane - 3u);
+                const float *c = sf + (size_t)k * (4 * NUM_PLANES) + 12u + v0;   // the struct's SH floats start at float 12
+                uint32_t w[4];
+#pragma unroll
+                for (uint32_t j = 0; j < 4; ++j)
+                    w[j] = sh_half2(v0 + 2u * j < nvals ? c[2 * j] : 0.0f, v0 + 2u * j + 1u < nvals ? c[2 * j + 1] : 0.0f);
+                v = make_float4(__uint_as_float(w[0]), __uint_as_float(w[1]), __uint_as_float(w[2]), __uint_as_float(w[3]));
+            }
+            soa[(uint64_t)plane * plane_stride + first + s0 + k] = v;
+        }
+        return;
+    }
     // valid floats of the last stored plane: 3K - 4(P - 1) = 3, 4, 3, 4 for 1..4 bands
     const uint32_t tail = (planes == soa_planes(1) || planes == soa_planes(3)) ? 3u : 4u;
     for (uint32_t i = threadIdx.x; i < here * (uint32_t)planes; i += blockDim.x) {
@@ -49,10 +74,12 @@ __device__ __forceinline__ void godot_basis_mul(const float a[3][3], const float
 
 // `lay` names the property groups of a vertex (gsr_ply_layout; default: the standard 62-property layout) and `planes` = soa_planes(store
 // bands) the planes written.  SH coefficients above the file's degree are stored as 0, those above the store's degree are dropped.
+// HALF (GSR_FLAG_SH_HALF; planes = soa_planes(store bands, true)): the SH planes are written as packed binary16 values (sh_half), 8 per
+// plane in the same coefficient-major order, values past 3K as +0.
 // FILTER3D (gsr_upload_ply_filtered): property `filter_3d` is Mip-Splatting's per-splat 3D filter f.  With f > 0 the splat is stored
 // with the filter folded in, in float64 and narrowed once: q_i = exp(scale_i)^2, q'_i = q_i + f*f, scale_i = sqrt(q'_i) and opacity =
 // sigmoid * sqrt((q_0 q_1 q_2) / (q'_0 q'_1 q'_2)).  f <= 0 or NaN: stored exactly as without the filter.
-template <bool FILTER3D = false>
+template <bool FILTER3D = false, bool HALF = false>
 __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *__restrict__ ply, uint32_t nprops, uint64_t count, float creation_time,
                                                                   float4 *__restrict__ soa, uint64_t plane_stride, uint64_t first,
                                                                   const gsr_ply_layout lay = PLY_LAYOUT_3DGS, int planes = NUM_PLANES,
@@ -110,8 +137,8 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
     soa[2 * plane_stride + id] = make_float4(Cv[1][2], Cv[2][2], opacity, 0.0f);
     // coefficient-major RGB: DC, then f_rest R | G | B (rest = K_file - 1 floats per channel) re-interleaved (:65-69)
     const uint32_t rest = (lay.sh_degree + 1u) * (lay.sh_degree + 1u) - 1u;
-    const uint32_t kept = (uint32_t)(planes - 3) == (uint32_t)sh_planes(4) ? 16u : (uint32_t)(planes - 3) == (uint32_t)sh_planes(3) ? 9u
-                        : (uint32_t)(planes - 3) == (uint32_t)sh_planes(2) ? 4u : 1u;   // K of the store
+    const uint32_t kept = (uint32_t)(planes - 3) == (uint32_t)sh_planes(4, HALF) ? 16u : (uint32_t)(planes - 3) == (uint32_t)sh_planes(3, HALF) ? 9u
+                        : (uint32_t)(planes - 3) == (uint32_t)sh_planes(2, HALF) ? 4u : 1u;   // K of the store
     const float *pf = p + (lay.f_rest < 0 ? 0 : lay.f_rest);   // every index below stays inside the vertex, also for a coefficient not read
     float sh[48];
     sh[0] = pd[0]; sh[1] = pd[1]; sh[2] = pd[2];
@@ -122,6 +149,14 @@ __global__ void __launch_bounds__(INGEST_SPLATS) ply_to_soa_kernel(const float *
         sh[3 + 3 * k + 0] = in ? pf[kr] : 0.0f;
         sh[3 + 3 * k + 1] = in ? pf[rest + kr] : 0.0f;
         sh[3 + 3 * k + 2] = in ? pf[2 * rest + kr] : 0.0f;
+    }
+    if constexpr (HALF) {   // (every value past the store's 3K is 0 already)
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+            if (k < planes - 3)
+                soa[(uint64_t)(3 + k) * plane_stride + id] = make_float4(__uint_as_float(sh_half2(sh[8 * k], sh[8 * k + 1])), __uint_as_float(sh_half2(sh[8 * k + 2], sh[8 * k + 3])),
+                                                                         __uint_as_float(sh_half2(sh[8 * k + 4], sh[8 * k + 5])), __uint_as_float(sh_half2(sh[8 * k + 6], sh[8 * k + 7])));
+        return;
     }
 #pragma unroll
     for (int k = 0; k < 12; ++k)
@@ -137,12 +172,30 @@ int preload_ingest_kernels() {
     cudaFuncAttributes fa;
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel<false>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel<true>));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, aos_to_soa_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, aos_to_soa_kernel<false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel<false, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, ply_to_soa_kernel<true, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, aos_to_soa_kernel<true>));
+    return GSR_OK;
+}
+template <bool FILTER3D, bool HALF>
+int launch_ply_variant(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
+                       uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d) {
+    const size_t smem = sizeof(float) * (size_t)INGEST_SPLATS * layout.nprops;
+    const uint32_t blocks = (uint32_t)((count + INGEST_SPLATS - 1) / INGEST_SPLATS);
+    if (smem > 48 * 1024) GSR_CUDA_TRY(cudaFuncSetAttribute(ply_to_soa_kernel<FILTER3D, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    ply_to_soa_kernel<FILTER3D, HALF><<<blocks, INGEST_SPLATS, smem, stream>>>(ply, layout.nprops, count, creation_time, soa, plane_stride, first, layout, planes,
+                                                                               filter_3d);
+    GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }
 int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t count, float creation_time, float4 *soa, uint64_t plane_stride,
-                      uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d) {
+                      uint64_t first, int planes, cudaStream_t stream, int32_t filter_3d, bool sh_half) {
     if (count == 0) return GSR_OK;
+    if (sh_half) {
+        return filter_3d >= 0 ? launch_ply_variant<true, true>(ply, layout, count, creation_time, soa, plane_stride, first, planes, stream, filter_3d)
+                              : launch_ply_variant<false, true>(ply, layout, count, creation_time, soa, plane_stride, first, planes, stream, -1);
+    }
     const size_t smem = sizeof(float) * (size_t)INGEST_SPLATS * layout.nprops;
     const uint32_t blocks = (uint32_t)((count + INGEST_SPLATS - 1) / INGEST_SPLATS);
     if (filter_3d >= 0) {
@@ -157,10 +210,12 @@ int launch_ply_to_soa(const float *ply, const gsr_ply_layout &layout, uint64_t c
     return GSR_OK;
 }
 
-int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, int planes, cudaStream_t stream) {
+int launch_aos_to_soa(const float4 *aos, uint64_t count, float4 *soa, uint64_t plane_stride, uint64_t first, int planes, cudaStream_t stream,
+                      bool sh_half) {
     if (count == 0) return GSR_OK;
     const uint32_t blocks = (uint32_t)((count + SPLATS_PER_BLOCK - 1) / SPLATS_PER_BLOCK);
-    aos_to_soa_kernel<<<blocks, 256, 0, stream>>>(aos, count, soa, plane_stride, first, planes);
+    if (sh_half) aos_to_soa_kernel<true><<<blocks, 256, 0, stream>>>(aos, count, soa, plane_stride, first, planes);
+    else aos_to_soa_kernel<false><<<blocks, 256, 0, stream>>>(aos, count, soa, plane_stride, first, planes);
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
 }

@@ -121,16 +121,37 @@ inline void mbar_wait(uint64_t *, uint32_t) {}
 // coefficients >= K set to zero adds +-0 to r for a finite view direction, and NaN (so colour 0 after the final max) for a non-finite
 // one (a splat at the camera position); `skip` = 0 * ((x + y) + z) is exactly that sum, so the frame stays bit for bit the zero-padded
 // cloud's (DESIGN.md section 5.9).
-template <bool FROM_SMEM, int SH_BANDS = SH_BANDS_MAX>
+// HALF (GSR_FLAG_SH_HALF): the planes hold binary16 values, 8 per plane.  The same two blocks of at most 8 coefficients are decoded --
+// half planes 0-2, then 3-5 -- into the same 24 registers, and the arithmetic after the decode is the float store's, so the colour is
+// bit for bit that of the float cloud holding the decoded values (the decode is exact).
+// `n` 16-byte planes from src[first * stride] on, as 8 binary16 values each, decoded into sh[0, 8n)
+template <bool FROM_SMEM>
+__device__ __forceinline__ void sh_half_block(const float4 *src, uint64_t stride, int first, int n, float sh[24]) {
+#pragma unroll
+    for (int k = 0; k < n; ++k) {
+        const float4 v = FROM_SMEM ? src[(uint64_t)(first + k) * stride] : __ldg(src + (uint64_t)(first + k) * stride);
+        const uint32_t w[4] = {__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            sh[8 * k + 2 * j] = half_bits_to_float(w[j] & 0xFFFFu);
+            sh[8 * k + 2 * j + 1] = half_bits_to_float(w[j] >> 16);
+        }
+    }
+}
+template <bool FROM_SMEM, int SH_BANDS = SH_BANDS_MAX, bool HALF = false>
 __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, float x, float y, float z, float col[3]) {
-    constexpr int K = sh_coeffs(SH_BANDS), P = sh_planes(SH_BANDS), P0 = P < 6 ? P : 6;
+    constexpr int K = sh_coeffs(SH_BANDS), P = sh_planes(SH_BANDS, HALF), P0 = P < (HALF ? 3 : 6) ? P : (HALF ? 3 : 6);
     const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
     {
         float sh[24];
+        if constexpr (HALF) {
+            sh_half_block<FROM_SMEM>(src, stride, 0, P0, sh);
+        } else {
 #pragma unroll
         for (int k = 0; k < P0; ++k) {
             const float4 v = FROM_SMEM ? src[(uint64_t)k * stride] : __ldg(src + (uint64_t)k * stride);
             sh[4 * k + 0] = v.x; sh[4 * k + 1] = v.y; sh[4 * k + 2] = v.z; sh[4 * k + 3] = v.w;
+        }
         }
 #pragma unroll
         for (int ch = 0; ch < 3; ++ch) {
@@ -153,10 +174,14 @@ __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, flo
     }
     if constexpr (K > 8) {
         float sh[24];
+        if constexpr (HALF) {
+            sh_half_block<FROM_SMEM>(src, stride, 3, P - 3, sh);
+        } else {
 #pragma unroll
         for (int k = 0; k < P - 6; ++k) {
             const float4 v = FROM_SMEM ? src[(uint64_t)(6 + k) * stride] : __ldg(src + (uint64_t)(6 + k) * stride);
             sh[4 * k + 0] = v.x; sh[4 * k + 1] = v.y; sh[4 * k + 2] = v.z; sh[4 * k + 3] = v.w;
+        }
         }
 #pragma unroll
         for (int ch = 0; ch < 3; ++ch) {
@@ -447,7 +472,7 @@ constexpr size_t PROJ_SMEM_BYTES = PROJ_SLAB_BYTES * PROJ_WARPS;                
 
 // the per-warp slab of a kernel that keeps planes 0-2 and `sh_bands` bands of SH planes (PROJ_SLAB_BYTES at 4 bands).  Used in place, never
 // as a local constant: even an unused local declaration changes the default kernel's SASS.
-__host__ __device__ constexpr size_t proj_slab_bytes(int sh_bands) { return sizeof(float4) * (size_t)soa_planes(sh_bands) * 32u; }
+__host__ __device__ constexpr size_t proj_slab_bytes(int sh_bands, bool half = false) { return sizeof(float4) * (size_t)soa_planes(sh_bands, half) * 32u; }
 static_assert(proj_slab_bytes(SH_BANDS_MAX) == PROJ_SLAB_BYTES, "the degree-3 slab");
 
 // Instanced warp: its instance k, first source splat, live lanes and the bytes of one plane slice (0 for a warp that draws nothing: a
@@ -500,8 +525,11 @@ __device__ __forceinline__ void instance_tint(const InstanceArgs &ia, uint32_t v
 // __grid_constant__ struct, changes the register allocation of the other instantiations).  Never with the compaction path (sharded only).
 // CUT (gsr_set_cutouts): every lane runs project_lane<.., CUT> with the set, which travels in a fourth parameter after DepthArgs for the
 // same reason (the first three keep their offsets); the kernels without cutouts get an empty placeholder there.  Never sharded.
+// HALF (GSR_FLAG_SH_HALF, binary16 stores): phase 2 brings sh_planes(SH_BANDS, true) planes (still 16 B per splat and plane, so the
+// slice sizes are unchanged), the warp's slab holds soa_planes(SH_BANDS, true) planes and sh_color decodes them.  Every difference is a
+// constant or an `if constexpr`: HALF = false is the float kernel.  Never sharded.
 struct DepthArgs { uint32_t *words = nullptr; };
-template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false, bool DEPTH = false, bool CUT = false>
+template <bool INSTANCED = false, int SH_BANDS = SH_BANDS_MAX, bool ORTHO = false, bool AA = false, bool DEPTH = false, bool CUT = false, bool HALF = false>
 __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_kernel(const __grid_constant__ ProjectionArgs a,
                                                                                        const __grid_constant__ InstanceParam<INSTANCED> ia = InstanceParam<INSTANCED>(),
                                                                                        const __grid_constant__ DepthArgs da = DepthArgs(),
@@ -522,7 +550,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     __shared__ uint32_t s_ncomp;
 
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
-    float4 *slab = reinterpret_cast<float4 *>(proj_smem + (size_t)warp * proj_slab_bytes(SH_BANDS));  // [SOA_PLANES][32]
+    float4 *slab = reinterpret_cast<float4 *>(proj_smem + (size_t)warp * proj_slab_bytes(SH_BANDS, HALF));  // [SOA_PLANES][32]
     if (lane == 0) {
         mbar_init(&s_bar[warp][0], 1);
         mbar_init(&s_bar[warp][1], 1);
@@ -609,13 +637,13 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         const uint32_t nsurv = s_ncomp;
         if (tid < nsurv) {
             const uint32_t li = s_list[tid];
-            const float4 *sl = reinterpret_cast<const float4 *>(proj_smem + (size_t)(li >> 5) * proj_slab_bytes(SH_BANDS));
+            const float4 *sl = reinterpret_cast<const float4 *>(proj_smem + (size_t)(li >> 5) * proj_slab_bytes(SH_BANDS, HALF));
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
             if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o, ct) && o.n) {
                 float col[3];
-                sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
+                sh_color<false, SH_BANDS, HALF>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
                 rec[0] = o.r0; rec[1] = o.r1; rec[2] = make_float4(col[0], col[1], col[2], o.opacity);
                 s_res[li] = make_uint4(o.n, o.x0 | (o.y0 << 16), o.w | (o.depth << 16), (uint32_t)o.last_tile);
@@ -659,13 +687,13 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     if (bulk && lane == 0) {
         if constexpr (INSTANCED) {   // nvis > 0: a live warp, slice_bytes > 0
             const InstanceWarp iw = instance_warp(a, ia, vwarp);
-            mbar_expect_tx(&s_bar[warp][1], (uint32_t)sh_planes(SH_BANDS) * iw.slice_bytes);
+            mbar_expect_tx(&s_bar[warp][1], (uint32_t)sh_planes(SH_BANDS, HALF) * iw.slice_bytes);
 #pragma unroll
-            for (int k = 3; k < soa_planes(SH_BANDS); ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + iw.src0, iw.slice_bytes, &s_bar[warp][1]);
+            for (int k = 3; k < soa_planes(SH_BANDS, HALF); ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + iw.src0, iw.slice_bytes, &s_bar[warp][1]);
         } else {
-        mbar_expect_tx(&s_bar[warp][1], (uint32_t)sh_planes(SH_BANDS) * 512u);
+        mbar_expect_tx(&s_bar[warp][1], (uint32_t)sh_planes(SH_BANDS, HALF) * 512u);
 #pragma unroll
-        for (int k = 3; k < soa_planes(SH_BANDS); ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + id0, 512u, &s_bar[warp][1]);
+        for (int k = 3; k < soa_planes(SH_BANDS, HALF); ++k) bulk_g2s(slab + k * 32, a.soa + (uint64_t)k * a.plane_stride + id0, 512u, &s_bar[warp][1]);
         }
     }
     if (closer) {
@@ -690,15 +718,15 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         mbar_wait(&s_bar[warp][1], 0);
         if (n) {
             float col[3];
-            sh_color<true, SH_BANDS>(slab + 3 * 32 + lane, 32, vx, vy, vz, col);
+            sh_color<true, SH_BANDS, HALF>(slab + 3 * 32 + lane, 32, vx, vy, vz, col);
             if constexpr (INSTANCED) instance_tint(ia, vwarp, col);
             float4 *rec = a.records + (uint64_t)id * 3u;
             rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
         }
     } else if (n && !colour_done) {
         float col[3];
-        if constexpr (INSTANCED) sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + instance_warp(a, ia, vwarp).src0 + lane, a.plane_stride, vx, vy, vz, col);
-        else sh_color<false, SH_BANDS>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
+        if constexpr (INSTANCED) sh_color<false, SH_BANDS, HALF>(a.soa + 3ull * a.plane_stride + instance_warp(a, ia, vwarp).src0 + lane, a.plane_stride, vx, vy, vz, col);
+        else sh_color<false, SH_BANDS, HALF>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
         if constexpr (INSTANCED) instance_tint(ia, vwarp, col);
         float4 *rec = a.records + (uint64_t)id * 3u;
         rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
@@ -1239,34 +1267,44 @@ uint32_t projection_num_blocks(uint32_t num_splats) { return (num_splats + PROJ_
 // Force-load this file's kernels (CUDA loads modules lazily; a first launch that has to load code while another context's
 // kernel spins on a flag this launch would satisfy can stall the host: see gsr_group_attach).
 // dynamic shared memory of projection_kernel<*, B>: the slabs of its eight warps
-constexpr size_t projection_smem_bytes(int sh_bands) { return proj_slab_bytes(sh_bands) * PROJ_WARPS; }
+constexpr size_t projection_smem_bytes(int sh_bands, bool half = false) { return proj_slab_bytes(sh_bands, half) * PROJ_WARPS; }
 static_assert(projection_smem_bytes(SH_BANDS_MAX) == PROJ_SMEM_BYTES, "the degree-3 slab");
 
-template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false, bool DEPTH = false, bool CUT = false>
+template <bool INSTANCED, int B, bool ORTHO = false, bool AA = false, bool DEPTH = false, bool CUT = false, bool HALF = false>
 int preload_projection_variant() {
     cudaFuncAttributes fa;
-    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)projection_smem_bytes(B)));
-    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT>));
+    GSR_CUDA_TRY(cudaFuncSetAttribute(projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      (int)projection_smem_bytes(B, HALF)));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT, HALF>));
     return GSR_OK;
 }
-// projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH, CUT>
-template <bool INSTANCED, bool ORTHO, bool AA = false, bool DEPTH = false, bool CUT = false>
+// projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH, CUT, HALF>
+template <bool INSTANCED, bool ORTHO, bool AA = false, bool DEPTH = false, bool CUT = false, bool HALF = false>
 int preload_projection_bands() {
     int rc;
-    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA, DEPTH, CUT>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA, DEPTH, CUT>()) ||
-        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA, DEPTH, CUT>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA, DEPTH, CUT>()))
+    if ((rc = preload_projection_variant<INSTANCED, 1, ORTHO, AA, DEPTH, CUT, HALF>()) || (rc = preload_projection_variant<INSTANCED, 2, ORTHO, AA, DEPTH, CUT, HALF>()) ||
+        (rc = preload_projection_variant<INSTANCED, 3, ORTHO, AA, DEPTH, CUT, HALF>()) || (rc = preload_projection_variant<INSTANCED, 4, ORTHO, AA, DEPTH, CUT, HALF>()))
         return rc;
     return GSR_OK;
 }
-// the cutout variants projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH, true> of every (ORTHO, AA, DEPTH)
-template <bool INSTANCED>
+// the variants projection_kernel<INSTANCED, 1..4, ORTHO, AA, DEPTH, CUT, HALF> of every (ORTHO, AA, DEPTH)
+template <bool INSTANCED, bool CUT = true, bool HALF = false>
 int preload_projection_cutouts() {
     int rc;
-    if ((rc = preload_projection_bands<INSTANCED, false, false, false, true>()) || (rc = preload_projection_bands<INSTANCED, true, false, false, true>()) ||
-        (rc = preload_projection_bands<INSTANCED, false, true, false, true>()) || (rc = preload_projection_bands<INSTANCED, true, true, false, true>()) ||
-        (rc = preload_projection_bands<INSTANCED, false, false, true, true>()) || (rc = preload_projection_bands<INSTANCED, true, false, true, true>()) ||
-        (rc = preload_projection_bands<INSTANCED, false, true, true, true>()) || (rc = preload_projection_bands<INSTANCED, true, true, true, true>()))
+    if ((rc = preload_projection_bands<INSTANCED, false, false, false, CUT, HALF>()) || (rc = preload_projection_bands<INSTANCED, true, false, false, CUT, HALF>()) ||
+        (rc = preload_projection_bands<INSTANCED, false, true, false, CUT, HALF>()) || (rc = preload_projection_bands<INSTANCED, true, true, false, CUT, HALF>()) ||
+        (rc = preload_projection_bands<INSTANCED, false, false, true, CUT, HALF>()) || (rc = preload_projection_bands<INSTANCED, true, false, true, CUT, HALF>()) ||
+        (rc = preload_projection_bands<INSTANCED, false, true, true, CUT, HALF>()) || (rc = preload_projection_bands<INSTANCED, true, true, true, CUT, HALF>()))
+        return rc;
+    return GSR_OK;
+}
+
+// the binary16-store variants (GSR_FLAG_SH_HALF): all 128 of them, loaded when a context with that store is created (the format is fixed
+// per context, and any of its frames may take any of them)
+int preload_projection_half_kernels() {
+    int rc;
+    if ((rc = preload_projection_cutouts<false, false, true>()) || (rc = preload_projection_cutouts<true, false, true>()) ||
+        (rc = preload_projection_cutouts<false, true, true>()) || (rc = preload_projection_cutouts<true, true, true>()))
         return rc;
     return GSR_OK;
 }
@@ -1315,48 +1353,54 @@ int launch_projection_scatter(const ProjectionArgs &frame_args, const ScatterPee
     return GSR_OK;
 }
 
-// projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT> for B = sh_bands (the orthographic, anti-aliased, depth-order and cutout frames:
-// single-context only, never sharded)
-template <bool INSTANCED, bool ORTHO, bool AA, bool DEPTH, bool CUT>
+// projection_kernel<INSTANCED, B, ORTHO, AA, DEPTH, CUT, HALF> for B = sh_bands (the orthographic, anti-aliased, depth-order, cutout and
+// binary16-store frames: single-context only, never sharded)
+template <bool INSTANCED, bool ORTHO, bool AA, bool DEPTH, bool CUT, bool HALF>
 void launch_projection_bands(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutParam<CUT> &ct, uint32_t blocks,
                              cudaStream_t stream, int sh_bands) {
     switch (sh_bands) {
-        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a, ia, DepthArgs{dw}, ct); break;
-        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a, ia, DepthArgs{dw}, ct); break;
-        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a, ia, DepthArgs{dw}, ct); break;
-        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA, DEPTH, CUT><<<blocks, PROJ_THREADS, PROJ_SMEM_BYTES, stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        case 1: projection_kernel<INSTANCED, 1, ORTHO, AA, DEPTH, CUT, HALF><<<blocks, PROJ_THREADS, projection_smem_bytes(1, HALF), stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        case 2: projection_kernel<INSTANCED, 2, ORTHO, AA, DEPTH, CUT, HALF><<<blocks, PROJ_THREADS, projection_smem_bytes(2, HALF), stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        case 3: projection_kernel<INSTANCED, 3, ORTHO, AA, DEPTH, CUT, HALF><<<blocks, PROJ_THREADS, projection_smem_bytes(3, HALF), stream>>>(a, ia, DepthArgs{dw}, ct); break;
+        default: projection_kernel<INSTANCED, SH_BANDS_MAX, ORTHO, AA, DEPTH, CUT, HALF><<<blocks, PROJ_THREADS, projection_smem_bytes(SH_BANDS_MAX, HALF), stream>>>(a, ia, DepthArgs{dw}, ct); break;
     }
 }
-template <bool INSTANCED, bool DEPTH, bool CUT>
+template <bool INSTANCED, bool DEPTH, bool CUT, bool HALF>
 void launch_projection_modes(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutParam<CUT> &ct, uint32_t blocks,
                              cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
     if (ortho) {
-        if (aa) launch_projection_bands<INSTANCED, true, true, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
-        else launch_projection_bands<INSTANCED, true, false, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
+        if (aa) launch_projection_bands<INSTANCED, true, true, DEPTH, CUT, HALF>(a, ia, dw, ct, blocks, stream, sh_bands);
+        else launch_projection_bands<INSTANCED, true, false, DEPTH, CUT, HALF>(a, ia, dw, ct, blocks, stream, sh_bands);
     } else {
-        if (aa) launch_projection_bands<INSTANCED, false, true, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
-        else launch_projection_bands<INSTANCED, false, false, DEPTH, CUT>(a, ia, dw, ct, blocks, stream, sh_bands);
+        if (aa) launch_projection_bands<INSTANCED, false, true, DEPTH, CUT, HALF>(a, ia, dw, ct, blocks, stream, sh_bands);
+        else launch_projection_bands<INSTANCED, false, false, DEPTH, CUT, HALF>(a, ia, dw, ct, blocks, stream, sh_bands);
     }
 }
-template <bool INSTANCED, bool CUT>
+template <bool INSTANCED, bool CUT, bool HALF>
 void launch_projection_depth(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutParam<CUT> &ct, uint32_t blocks,
                              cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
-    if (dw) launch_projection_modes<INSTANCED, true, CUT>(a, ia, dw, ct, blocks, stream, sh_bands, ortho, aa);
-    else launch_projection_modes<INSTANCED, false, CUT>(a, ia, nullptr, ct, blocks, stream, sh_bands, ortho, aa);
+    if (dw) launch_projection_modes<INSTANCED, true, CUT, HALF>(a, ia, dw, ct, blocks, stream, sh_bands, ortho, aa);
+    else launch_projection_modes<INSTANCED, false, CUT, HALF>(a, ia, nullptr, ct, blocks, stream, sh_bands, ortho, aa);
+}
+template <bool INSTANCED, bool HALF>
+void launch_projection_cut(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutArgs *cut, uint32_t blocks,
+                           cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
+    if (cut) launch_projection_depth<INSTANCED, true, HALF>(a, ia, dw, *cut, blocks, stream, sh_bands, ortho, aa);
+    else launch_projection_depth<INSTANCED, false, HALF>(a, ia, dw, NoCutouts(), blocks, stream, sh_bands, ortho, aa);
 }
 template <bool INSTANCED>
 void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutArgs *cut, uint32_t blocks,
-                               cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
-    if (cut) launch_projection_depth<INSTANCED, true>(a, ia, dw, *cut, blocks, stream, sh_bands, ortho, aa);
-    else launch_projection_depth<INSTANCED, false>(a, ia, dw, NoCutouts(), blocks, stream, sh_bands, ortho, aa);
+                               cudaStream_t stream, int sh_bands, bool ortho, bool aa, bool sh_half) {
+    if (sh_half) launch_projection_cut<INSTANCED, true>(a, ia, dw, cut, blocks, stream, sh_bands, ortho, aa);
+    else launch_projection_cut<INSTANCED, false>(a, ia, dw, cut, blocks, stream, sh_bands, ortho, aa);
 }
 
 int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa, uint32_t *depth_words,
-                      const CutoutArgs *cutouts) {
+                      const CutoutArgs *cutouts, bool sh_half) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho || aa || depth_words || cutouts) {
-        launch_projection_special<false>(a, InstanceArgs(), depth_words, cutouts, blocks, stream, sh_bands, ortho, aa);
+    if (ortho || aa || depth_words || cutouts || sh_half) {
+        launch_projection_special<false>(a, InstanceArgs(), depth_words, cutouts, blocks, stream, sh_bands, ortho, aa, sh_half);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }
@@ -1366,7 +1410,7 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }
-    switch (sh_bands) {   // (the sharded variant above reads a degree-3 store: reduced degrees are single-context only)
+    switch (sh_bands) {   // (the sharded variant above reads a degree-3 float store: reduced degrees and binary16 stores are single-context only)
         case 1: projection_kernel<false, 1><<<blocks, PROJ_THREADS, projection_smem_bytes(1), stream>>>(a); break;
         case 2: projection_kernel<false, 2><<<blocks, PROJ_THREADS, projection_smem_bytes(2), stream>>>(a); break;
         case 3: projection_kernel<false, 3><<<blocks, PROJ_THREADS, projection_smem_bytes(3), stream>>>(a); break;
@@ -1377,11 +1421,11 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
 }
 
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho, bool aa,
-                                uint32_t *depth_words, const CutoutArgs *cutouts) {
+                                uint32_t *depth_words, const CutoutArgs *cutouts, bool sh_half) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
-    if (ortho || aa || depth_words || cutouts) {
-        launch_projection_special<true>(a, ia, depth_words, cutouts, blocks, stream, sh_bands, ortho, aa);
+    if (ortho || aa || depth_words || cutouts || sh_half) {
+        launch_projection_special<true>(a, ia, depth_words, cutouts, blocks, stream, sh_bands, ortho, aa, sh_half);
         GSR_CUDA_TRY(cudaGetLastError());
         return GSR_OK;
     }

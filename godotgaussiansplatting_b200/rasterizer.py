@@ -47,14 +47,16 @@ class RenderTexture:
 class GaussianSplattingRasterizer:
     def __init__(self, point_cloud: PlyFile, output_texture_size, render_texture: RenderTexture | None, camera: Camera3D,
                  device: int = 0, flags: int = 0, dup_capacity_factor: int = 10, clock=None, sh_bands: int | None = None,
-                 antialiasing: float | None = None, depth_order: int = 0):
+                 antialiasing: float | None = None, depth_order: int = 0, sh_half: bool = False):
         """sh_bands: SH bands the context stores (gsr_config.sh_bands, 1..4 = degree + 1); None = the file's degree + 1, or 4 when its
         properties do not name a 3DGS layout.
         antialiasing: the 2D filter variance of anti-aliased trainings (include/gsr.h gsr_set_antialiasing; 0 = off); None = 0.1, the
         Mip-Splatting filter, when the file carries `filter_3D`, else off.  A file with `filter_3D` is loaded with its 3D filter folded
         into scale and opacity (gsr_upload_ply_filtered) whatever this value is.
         depth_order: how each tile's splats are ordered (include/gsr.h gsr_set_depth_order): 0 = the reference's 16-bit depth key, 1 = exact
-        view depth (large or metric-scale scenes, depth compositing)."""
+        view depth (large or metric-scale scenes, depth compositing).
+        sh_half: store the SH coefficients as IEEE binary16 (include/gsr.h GSR_FLAG_SH_HALF): 144 instead of 240 bytes per degree-3
+        splat, each frame exactly that of the cloud with its coefficients rounded to binary16 once."""
         self.should_enable_heatmap = [False]
         self.render_scale = [1.0]
         self.model_scale = [1.0]
@@ -64,7 +66,7 @@ class GaussianSplattingRasterizer:
         self.is_loaded = False
         self.loaded_callbacks = []  # signal `loaded`
         self._ctx = C.c_void_p(None)
-        self._device, self._flags, self._factor = device, flags, dup_capacity_factor
+        self._device, self._flags, self._factor = device, flags | (_lib.GSR_FLAG_SH_HALF if sh_half else 0), dup_capacity_factor
         try:
             self._layout = point_cloud.layout()
         except ValueError:

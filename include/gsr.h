@@ -67,6 +67,20 @@ enum {
                                       Single-context only: an orthographic frame on a context with a shard group, peer framebuffers, a
                                       partial band or row interleave returns GSR_ERR_STATE and enqueues nothing. */
 
+#define GSR_FLAG_SH_HALF 0x40u /* store the SH coefficients of the gsr_config.sh_bands bands as IEEE binary16 (no reference counterpart):
+                                   a degree-3 splat takes 144 instead of 240 bytes.  Planes 0-2 (position / time, covariance, opacity)
+                                   stay float32.  Every upload rounds each coefficient once, on the device: h(c) = c rounded to
+                                   binary16 to nearest even, subnormal halves and signed zeros kept, finite or infinite values beyond
+                                   +-65504 saturated to +-65504, NaN kept a NaN (payload and sign unspecified).  Layout: after planes
+                                   0-2 come P_h = ceil(3K / 8) planes of 16 bytes per splat (K = B^2; B = 1..4 gives 1, 2, 4, 6 planes:
+                                   64 / 80 / 112 / 144 B per splat); value i = 3k + channel sits in plane 3 + (i >> 3), slot i & 7 of its
+                                   8 halves (slot 0 = the low half of the plane's first 32-bit word), slots past 3K are +0.  Every frame
+                                   is bit for bit the frame of the same context without the flag holding the cloud whose coefficients
+                                   are float(h(c)), with every frame feature and every rendered degree (gsr_set_sh_degree reads the
+                                   first ceil(3 (d+1)^2 / 8) half planes).  Fixed at creation.  Single-context only, like a reduced
+                                   store: gsr_group_export, gsr_group_attach with world > 1, gsr_peer_*, a partial gsr_set_band and
+                                   gsr_set_row_interleave with row_mod > 1 return GSR_ERR_STATE (DESIGN.md section 5.14). */
+
 /* ---- gsr_debug_copy selectors (parity taps; not on the frame path) ---- */
 enum {
     GSR_BUF_RECORDS = 0, /* 48 B RasterizeData per splat id (gsplat_projection.glsl:42-48), max_splats entries */
@@ -81,7 +95,7 @@ enum {
     GSR_BUF_INSTANCES = 9,              /* gsr_set_instances: 24 floats per instance, to_frame as given then the library's inverse
                                            [A^-1 | -A^-1 t] rounded to float (both 3x4, column-major) */
     GSR_BUF_SPLATS = 10,                /* the stored splat planes, plane-major: (3 + P) x plane_stride float4, plane_stride = max_splats
-                                           rounded up to 256 (gsr_config.sh_bands) */
+                                           rounded up to 256 (gsr_config.sh_bands; 3 + P_h planes of binary16 SH with GSR_FLAG_SH_HALF) */
     GSR_BUF_DEPTH_WORDS_UNSORTED = 11,  /* gsr_set_depth_order: the last mode-1 frame's ord(d) per pair in emission order, M entries
                                            (kept with gsr_debug_keep_unsorted once mode 1 has been switched on) */
     GSR_BUF_INSTANCE_APPEARANCE = 12    /* gsr_set_instance_appearance: one gsr_instance_appearance per instance as stored (the default
