@@ -276,10 +276,14 @@ struct InstanceArgs {
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false,
                                 bool aa = false, uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr, bool sh_half = false);
+// Per instance and frame with motion vectors (gsr_set_motion_vectors): the previous frame's to_frame [A' | t'] (12).
+constexpr int INSTANCE_PREV_FLOATS = 12;
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats
-// (mapped page-locked host memory on the frame path).  With an appearance (count x 8 floats, same memory) its rows go to appearance_out.
+// (mapped page-locked host memory on the frame path).  With an appearance (count x 8 floats, same memory) its rows go to appearance_out,
+// with previous transforms (count x 12 floats, same memory) they go to prev_out.
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream,
-                            const float *appearance = nullptr, float *appearance_out = nullptr);
+                            const float *appearance = nullptr, float *appearance_out = nullptr, const float *prev_xf = nullptr,
+                            float *prev_out = nullptr);
 
 // ---------------------------------------------------------------------------------------------
 // multi-GPU shard group (group.cu, gsr_group_attach): flag words + receive segments + record tables in every rank's arena
@@ -373,7 +377,22 @@ struct CompositeArgs {
     const float *scene_depth;  // optional W*H linear scene depth; a pixel stops at the first splat not in front of it (nullptr: +inf)
     float *depth_out;          // W*H: D / (1 - t) of the blended splats, +inf where nothing was blended
 };
-int launch_composite(const CompositeArgs &a, cudaStream_t stream);
+// Motion vectors (gsr_set_motion_vectors, with depth compositing only): the second __grid_constant__ parameter of the motion variants
+// of the compositor.  Per staged splat m = pix(prev_vp, p') - pix(vp, p) (compositor.cu motion_of), accumulated like the depth.
+struct MotionArgs {
+    float vp[32];               // this frame's view_proj
+    float prev_vp[32];          // the previous frame's (this frame's own when there is none)
+    float fw, fh;               // (float)(W - 1), (float)(H - 1)
+    float *motion_out;          // W*H float2: M / (1 - t), (0, 0) where nothing was blended
+    // instances (warp_inst == nullptr: none, p' = p): the source splat s = desc[k].first + (v - 32 desc[k].warp0) of drawn id v and
+    // warp instance k = warp_inst[v >> 5], sp = plane0[s].xyz * model_scale, p' = A'_k * sp + t'_k
+    const uint32_t *warp_inst;
+    const InstanceDesc *desc;
+    const float *prev_xf;       // 12 floats per instance: its previous to_frame (this frame's own when there is none)
+    const float4 *plane0;       // plane 0 of the store
+    float model_scale;
+};
+int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion = nullptr);
 int composite_max_ctas_per_sm(int *out);
 // order[0 .. num_tiles) = owned-tile indices sorted by descending expected chain length: the chunk count the tile consumed in the
 // previous frame (hint[k] with bit 31 set; the bit is cleared here) or, without a hint, its list length in chunks capped at

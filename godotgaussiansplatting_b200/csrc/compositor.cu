@@ -29,6 +29,10 @@
 // scene depth Z (nothing after it contributes, as if the pixel had died), the depth is accumulated like a fourth colour channel,
 // and the outputs are premultiplied rgb, alpha = 1 - t and depth = D / (1 - t) (+inf where nothing was blended).  DEPTH = false
 // is the reference's frame and compiles to the same code as before the mode existed.
+// Motion vectors (MOTION = true, gsr_set_motion_vectors; always with DEPTH): every staged splat also carries its screen motion
+// m = pix(M', p') - pix(M, p) (motion_of below), accumulated per pixel like the depth, and the output is M / (1 - t).  The per-splat
+// loads are issued when the chunk is gathered and the arithmetic runs when it is stored to shared memory.  The constants travel in a
+// second __grid_constant__ parameter; the other variants take an empty placeholder there and compile to the code they had before.
 #include <stdlib.h>
 #include <string.h>
 
@@ -70,9 +74,29 @@ __device__ __forceinline__ Staged null_splat() {
     return s;
 }
 
+// MOTION: what the gather loads for the motion of one staged splat -- its drawn id, the record's frame-space position p and, with
+// instances, the instance of its drawn warp.  The rest (descriptor, plane 0, previous transform) is loaded at the store.
+struct MotionPending {
+    uint32_t v, k;    // drawn id; instance (0xFFFFFFFF: none -- no instances, or a null splat)
+    float p0, p1, p2; // r0.z, r0.w, r1.w
+};
+__device__ __forceinline__ MotionPending null_motion() {
+    MotionPending m;
+    m.v = 0u; m.k = 0xFFFFFFFFu; m.p0 = m.p1 = m.p2 = 0.f;
+    return m;
+}
+
+// MOTION only: the other variants carry (and declare) nothing of it
+struct NoMotion {};
+template <bool MOTION> struct MotionParamT { using type = NoMotion; using pending = NoMotion; };
+template <> struct MotionParamT<true> { using type = MotionArgs; using pending = MotionPending; };
+template <bool MOTION> using MotionParam = typename MotionParamT<MOTION>::type;
+template <bool MOTION> using Pending = typename MotionParamT<MOTION>::pending;
+
 // vz = (V[2], V[6], V[10], V[14]): the view-matrix row of the depth (DEPTH only)
-template <bool DEPTH>
-__device__ __forceinline__ Staged gather(const float4 *__restrict__ records, const uint32_t *__restrict__ values, uint32_t idx, float4 vz) {
+template <bool DEPTH, bool MOTION = false>
+__device__ __forceinline__ Staged gather(const float4 *__restrict__ records, const uint32_t *__restrict__ values, uint32_t idx, float4 vz,
+                                         Pending<MOTION> *mp = nullptr, const MotionParam<MOTION> *mo = nullptr) {
     const uint32_t v = __ldg(values + idx);
     const float4 *r = records + (uint64_t)v * 3u;
     const float4 r0 = __ldg(r + 0), r1 = __ldg(r + 1), r2 = __ldg(r + 2);
@@ -81,7 +105,47 @@ __device__ __forceinline__ Staged gather(const float4 *__restrict__ records, con
     s.b = make_float4(-r1.y, r2.w, r2.x, r2.y);
     s.c = r2.z;
     s.d = DEPTH ? -(((vz.x * r0.z + vz.y * r0.w) + vz.z * r1.w) + vz.w * 1.0f) : 0.f;   // == -view[2] of the projection
+    if constexpr (MOTION) {   // (the instance load only depends on v: it runs beside the record loads)
+        mp->v = v; mp->k = mo->warp_inst ? __ldg(mo->warp_inst + (v >> 5)) : 0xFFFFFFFFu;
+        mp->p0 = r0.z; mp->p1 = r0.w; mp->p2 = r1.w;
+    }
     return s;
+}
+
+// The pixel position of frame-space point q under the 32-float view_proj M = (V, P) of a W x H frame: the projection's image_pos
+// operations without the load-in term.  w = clip[3].
+__device__ __forceinline__ void motion_pix(const float *M, float q0, float q1, float q2, float fw, float fh, float &x, float &y, float &w) {
+    const float *V = M, *P = M + 16;
+    float view[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) view[r] = ((V[0 + r] * q0 + V[4 + r] * q1) + V[8 + r] * q2) + V[12 + r] * 1.0f;
+    const float c0 = ((P[0] * view[0] + P[4] * view[1]) + P[8] * view[2]) + P[12] * view[3];
+    const float c1 = ((P[1] * view[0] + P[5] * view[1]) + P[9] * view[2]) + P[13] * view[3];
+    w = ((P[3] * view[0] + P[7] * view[1]) + P[11] * view[2]) + P[15] * view[3];
+    x = ((c0 / w + 1.0f) * 0.5f) * fw;
+    y = ((c1 / w + 1.0f) * 0.5f) * fh;
+}
+
+// The screen motion of one staged splat, previous minus current: m = pix(M', p') - pix(M, p).  p' = p without an instance; with one,
+// p' = A' * sp + t' for the source splat's sp = plane0 * model_scale and the instance's previous to_frame A' | t' (the record's own
+// operations: an unchanged transform gives p' == p bit for bit).  (0, 0) unless clip3' > 0 and both components are finite.
+__device__ __forceinline__ float2 motion_of(const MotionArgs &mo, const MotionPending &mp) {
+    float q0 = mp.p0, q1 = mp.p1, q2 = mp.p2;
+    if (mp.k != 0xFFFFFFFFu) {
+        const InstanceDesc d = mo.desc[mp.k];
+        const float *A = mo.prev_xf + (size_t)mp.k * 12u;
+        const float4 pt = __ldg(mo.plane0 + d.first + (mp.v - 32u * d.warp0));
+        const float sp0 = pt.x * mo.model_scale, sp1 = pt.y * mo.model_scale, sp2 = pt.z * mo.model_scale;
+        q0 = ((A[0] * sp0 + A[3] * sp1) + A[6] * sp2) + A[9];
+        q1 = ((A[1] * sp0 + A[4] * sp1) + A[7] * sp2) + A[10];
+        q2 = ((A[2] * sp0 + A[5] * sp1) + A[8] * sp2) + A[11];
+    }
+    float x, y, w, xp, yp, wp;
+    motion_pix(mo.vp, mp.p0, mp.p1, mp.p2, mo.fw, mo.fh, x, y, w);
+    motion_pix(mo.prev_vp, q0, q1, q2, mo.fw, mo.fh, xp, yp, wp);
+    const float mx = xp - x, my = yp - y;
+    const bool ok = wp > 0.0f && fabsf(mx) <= 3.402823466e38f && fabsf(my) <= 3.402823466e38f;   // (false for NaN)
+    return ok ? make_float2(mx, my) : make_float2(0.f, 0.f);
 }
 
 #ifndef GSR_COMP_GROUP
@@ -180,9 +244,11 @@ __device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], 
 //      transmittance are kept by select.  `alive_mid` = "a pixel of this thread was alive after the first half of the group".
 //      DEPTH: o0/o1 = "not stopped by the scene depth" (z0/z1); a live pixel stops at the first splat with !(d < z), before blending
 //      it; a stopped pixel is dead from then on.  dd2 accumulates d * alpha * t exactly like a colour channel.
-template <bool CONTRACT, bool DEPTH>
+//      MOTION: mx2 / my2 accumulate the staged motion (s_m) exactly like the depth.
+template <bool CONTRACT, bool DEPTH, bool MOTION = false>
 __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, const float *s_d, int j, const F2 al2[GU], const F2 om2[GU], F2 &cr2,
-                                        F2 &cg2, F2 &cb2, float &t0, float &t1, bool &alive_mid, float z0, float z1, bool &o0, bool &o1, F2 &dd2) {
+                                        F2 &cg2, F2 &cb2, float &t0, float &t1, bool &alive_mid, float z0, float z1, bool &o0, bool &o1, F2 &dd2,
+                                        const float2 *s_m = nullptr, F2 *mx2 = nullptr, F2 *my2 = nullptr) {
 #pragma unroll
     for (int u = 0; u < GU; ++u) {
         const float cbl = s_c[j + u];
@@ -209,11 +275,21 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, co
             cg2 = fma2(mul2(bc(B[u].w), m2), t2, cg2);
             cb2 = fma2(mul2(bc(cbl), m2), t2, cb2);
             if constexpr (DEPTH) dd2 = fma2(mul2(bc(dj), m2), t2, dd2);
+            if constexpr (MOTION) {
+                const float2 mv = s_m[j + u];
+                *mx2 = fma2(mul2(bc(mv.x), m2), t2, *mx2);
+                *my2 = fma2(mul2(bc(mv.y), m2), t2, *my2);
+            }
         } else {
             cr2 = mul_add2_unfused(mul2(bc(B[u].z), m2), t2, cr2);
             cg2 = mul_add2_unfused(mul2(bc(B[u].w), m2), t2, cg2);
             cb2 = mul_add2_unfused(mul2(bc(cbl), m2), t2, cb2);
             if constexpr (DEPTH) dd2 = mul_add2_unfused(mul2(bc(dj), m2), t2, dd2);
+            if constexpr (MOTION) {
+                const float2 mv = s_m[j + u];
+                *mx2 = mul_add2_unfused(mul2(bc(mv.x), m2), t2, *mx2);
+                *my2 = mul_add2_unfused(mul2(bc(mv.y), m2), t2, *my2);
+            }
         }
         t0 = a0 ? pl : t0;
         t1 = a1 ? ph : t1;
@@ -226,12 +302,16 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, co
 
 // Persistent CTAs.  Ticket k of the launch renders owned tile order[k] (longest chains first) or k itself; every tile is blended
 // from its first chunk to its stop by the CTA that took it.
-template <bool CONTRACT, bool DEPTH = false>
-__global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel(const __grid_constant__ CompositeArgs p) {
+// MOTION (gsr_set_motion_vectors, with DEPTH only): the motion constants in `mo`; the other variants take an empty placeholder.
+template <bool CONTRACT, bool DEPTH = false, bool MOTION = false>
+__global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel(const __grid_constant__ CompositeArgs p,
+                                                                                 const __grid_constant__ MotionParam<MOTION> mo = MotionParam<MOTION>()) {
+    static_assert(!MOTION || DEPTH, "motion vectors are a companion of depth compositing");
     __shared__ float4 s_a[CHUNK];
     __shared__ float4 s_b[CHUNK];
     __shared__ float s_c[CHUNK];
     __shared__ float s_d[DEPTH ? CHUNK : 1];   // view depth of the staged splats
+    __shared__ float2 s_m[MOTION ? CHUNK : 1]; // MOTION: screen motion of the staged splats
     __shared__ uint32_t s_vote[THREADS / 32];
     __shared__ uint32_t s_tile;
 
@@ -271,6 +351,7 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         float t0 = 1.0f, t1 = 1.0f;                    // transmittance of the two pixels
         bool o0 = true, o1 = true;                     // DEPTH: not stopped by the scene depth
         F2 dd2 = pk(0.f, 0.f);                         // DEPTH: accumulated depth
+        F2 mx2 = pk(0.f, 0.f), my2 = mx2;              // MOTION: accumulated motion
         float z0 = __uint_as_float(0x7f800000u), z1 = z0; // DEPTH: scene depth (+inf: nothing occludes; also outside the image)
         if (DEPTH && p.scene_depth && py < p.height) {
             const float *zrow = p.scene_depth + (uint64_t)py * (uint64_t)p.width;
@@ -279,9 +360,11 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         }
 
         Staged n0 = null_splat(), n1 = null_splat();
+        Pending<MOTION> q0, q1;   // MOTION: the gathered splats' pending motion loads
+        if constexpr (MOTION) { q0 = null_motion(); q1 = null_motion(); }
         if (num_iterations > 0) {
-            if ((int)tid < num_splats) n0 = gather<DEPTH>(p.records, p.values, bounds.x + tid, vz);
-            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH>(p.records, p.values, bounds.x + tid + THREADS, vz);
+            if ((int)tid < num_splats) n0 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + tid, vz, &q0, &mo);
+            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + tid + THREADS, vz, &q1, &mo);
         }
 
         int consumed = 0;  // chunks blended before the stop rule fired (next frame's scheduling hint)
@@ -293,13 +376,15 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
             s_a[tid] = n0.a; s_b[tid] = n0.b; s_c[tid] = n0.c;
             s_a[tid + THREADS] = n1.a; s_b[tid + THREADS] = n1.b; s_c[tid + THREADS] = n1.c;
             if constexpr (DEPTH) { s_d[tid] = n0.d; s_d[tid + THREADS] = n1.d; }
+            if constexpr (MOTION) { s_m[tid] = motion_of(mo, q0); s_m[tid + THREADS] = motion_of(mo, q1); }
             __syncthreads();
             // prefetch the next chunk's records while this one is blended (slots past the list end become null splats)
             n0 = null_splat(); n1 = null_splat();
+            if constexpr (MOTION) { q0 = null_motion(); q1 = null_motion(); }
             if (i + 1 < num_iterations) {
                 const int nb = sort_offset + CHUNK;
-                if (nb + (int)tid < num_splats) n0 = gather<DEPTH>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz);
-                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz);
+                if (nb + (int)tid < num_splats) n0 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz, &q0, &mo);
+                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz, &q1, &mo);
             }
 
             // :79-91, GU splats per iteration; `chunk` rounded up to GU reads null splats (opacity 0 => exact no-op).  Software-pipelined:
@@ -322,7 +407,7 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
 #pragma unroll
                 for (int u = 0; u < GU; ++u) { A[u] = s_a[jn + u]; B[u] = s_b[jn + u]; }
                 bool alive_mid = true;
-                phase_b<CONTRACT, DEPTH>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2);
+                phase_b<CONTRACT, DEPTH, MOTION>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2, s_m, &mx2, &my2);
                 go = __any_sync(0xffffffffu, alive_mid);
             }
 
@@ -359,6 +444,13 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
                 if (px0 < p.width) drow[px0] = k0 > 0.0f ? __fdiv_rn(d0, k0) : inf;
                 if (px0 + 1 < p.width) drow[px0 + 1] = k1 > 0.0f ? __fdiv_rn(d1, k1) : inf;
             }
+            if constexpr (MOTION) {   // M / (1 - t), (0, 0) where nothing was blended
+                float mx0, mx1, my0, my1;
+                upk(mx2, mx0, mx1); upk(my2, my0, my1);
+                float2 *mrow = reinterpret_cast<float2 *>(mo.motion_out) + (uint64_t)py * (uint64_t)p.width;
+                if (px0 < p.width) mrow[px0] = k0 != 0.0f ? make_float2(__fdiv_rn(mx0, k0), __fdiv_rn(my0, k0)) : make_float2(0.f, 0.f);
+                if (px0 + 1 < p.width) mrow[px0 + 1] = k1 != 0.0f ? make_float2(__fdiv_rn(mx1, k1), __fdiv_rn(my1, k1)) : make_float2(0.f, 0.f);
+            }
         }
         // :105-110 pick: the elected (first) lane of each 32-wide subgroup of the reference's 16x16 workgroup is local
         // index 32*s = pixel (0, 2*s) of the tile = first pixel of thread 16*s here
@@ -389,27 +481,36 @@ int preload_composite_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<true, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<true, true, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false, true, true>));
     return GSR_OK;
 }
 
 int composite_max_ctas_per_sm(int *out) {
-    int a = 0, b = 0, c = 0, d = 0;
+    int a = 0, b = 0, c = 0, d = 0, e = 0, f = 0;
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, composite_kernel<true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, composite_kernel<false>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, composite_kernel<true, true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d, composite_kernel<false, true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e, composite_kernel<true, true, true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&f, composite_kernel<false, true, true>, THREADS, 0));
     if (c < a) a = c;
     if (d < b) b = d;
+    if (e < a) a = e;
+    if (f < b) b = f;
     *out = a < b ? a : b;
     if (*out < 1) *out = 1;
     return GSR_OK;
 }
 
-int launch_composite(const CompositeArgs &a, cudaStream_t stream) {
+int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion) {
     if (a.num_tiles <= 0) return GSR_OK;
     const int per_sm = a.ctas_per_sm > 0 ? a.ctas_per_sm : 1;
     const int grid = a.num_tiles < a.sm_count * per_sm ? a.num_tiles : a.sm_count * per_sm;
-    if (a.depth_out) {   // depth compositing (gsr_set_depth_compositing)
+    if (a.depth_out && motion) {   // motion vectors (gsr_set_motion_vectors)
+        if (a.contract) composite_kernel<true, true, true><<<grid, THREADS, 0, stream>>>(a, *motion);
+        else composite_kernel<false, true, true><<<grid, THREADS, 0, stream>>>(a, *motion);
+    } else if (a.depth_out) {   // depth compositing (gsr_set_depth_compositing)
         if (a.contract) composite_kernel<true, true><<<grid, THREADS, 0, stream>>>(a);
         else composite_kernel<false, true><<<grid, THREADS, 0, stream>>>(a);
     } else if (a.contract) {

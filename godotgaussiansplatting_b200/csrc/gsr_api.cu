@@ -12,6 +12,7 @@
 #include <unistd.h>
 
 #include <new>
+#include <vector>
 
 #include "common.cuh"
 
@@ -74,6 +75,19 @@ struct gsr_ctx {
     // depth compositing (gsr_set_depth_compositing): caller-owned W*H float planes; depth_out == nullptr = off
     const float *scene_depth = nullptr;
     float *depth_out = nullptr;
+    // motion vectors (gsr_set_motion_vectors, with depth compositing): caller-owned W*H float2 plane; nullptr = off
+    float *motion_out = nullptr;
+    // The camera and instance transforms of a frame, recorded for every frame enqueued by gsr_render* (motion on or off): `mot_last` is
+    // the last enqueued frame's, the previous state of the next frame; `mot_used` is the previous state the last frame was enqueued
+    // with (gsr_render's re-render of an overflowed frame uses it again).  valid == false: no previous frame (first frame, gsr_resize,
+    // gsr_reset_motion), the frame is its own previous state.
+    struct MotionState {
+        bool valid = false;
+        float vp[32] = {};
+        std::vector<uint64_t> range;   // the instance layout, 2 per instance (empty: no instances)
+        std::vector<float> to_frame;   // INSTANCE_PREV_FLOATS per instance
+    };
+    MotionState mot_last, mot_used;
     float4 *pick_strip = nullptr;   // 16 pixel rows: where gsr_pick's default-path re-dispatch writes while depth compositing is on
     float4 *fb2 = nullptr;                       // second frame for pipelined read-back (gsr_render_async)
     void *stage[2] = {nullptr, nullptr};         // converted copies of the two frames (GSR_OUT_* other than RGBA32F), lazily allocated (16 B/pixel)
@@ -136,10 +150,11 @@ struct gsr_ctx {
         InstanceDesc *desc = nullptr;    // device [n]
         uint32_t *warps = nullptr;       // device: instance of every drawn warp of the projection grid
         float *frame = nullptr;          // device [2][cap][INSTANCE_FRAME_FLOATS]: this frame's constants, by frame parity; then
-                                         // [2][cap][INSTANCE_APPEARANCE_FLOATS]: this frame's appearance rows, by frame parity
+                                         // [2][cap][INSTANCE_APPEARANCE_FLOATS]: this frame's appearance rows, by frame parity; then
+                                         // [2][cap][INSTANCE_PREV_FLOATS]: the previous transforms of its motion vectors, by parity
         uint32_t cap = 0;                // instances the device tables and the ring are sized for
-        float *ring = nullptr;           // mapped page-locked [GSR_INSTANCE_RING][cap][24 + 8]: per slot the transforms of one frame
-                                         // ([cap][24]), then its appearance rows ([cap][8])
+        float *ring = nullptr;           // mapped page-locked [GSR_INSTANCE_RING][cap][24 + 8 + 12]: per slot the transforms of one
+                                         // frame ([cap][24]), then its appearance rows ([cap][8]), then its previous transforms ([cap][12])
         float *ring_dev = nullptr;
         cudaEvent_t ev[GSR_INSTANCE_RING] = {};   // recorded after the prepare kernel that read the slot
         bool ev_used[GSR_INSTANCE_RING] = {};
@@ -156,12 +171,17 @@ struct gsr_sorter {
 
 namespace {
 
-// one slot of the instance ring, per instance of the capacity: the transforms, then the appearance rows
-constexpr size_t INSTANCE_SLOT_FLOATS = INSTANCE_XFORM_FLOATS + INSTANCE_APPEARANCE_FLOATS;
+// one slot of the instance ring, per instance of the capacity: the transforms, the appearance rows, the previous transforms
+constexpr size_t INSTANCE_SLOT_FLOATS = INSTANCE_XFORM_FLOATS + INSTANCE_APPEARANCE_FLOATS + INSTANCE_PREV_FLOATS;
 
 // the device appearance rows of the frames of parity `half` (they follow the two tables of per-frame constants)
 float *instance_appearance_table(const gsr_ctx::Instances &I, int half) {
     return I.frame + 2ull * I.cap * INSTANCE_FRAME_FLOATS + (size_t)half * I.cap * INSTANCE_APPEARANCE_FLOATS;
+}
+
+// the device previous transforms of the frames of parity `half` (motion vectors; they follow the appearance rows)
+float *instance_prev_table(const gsr_ctx::Instances &I, int half) {
+    return I.frame + 2ull * I.cap * (INSTANCE_FRAME_FLOATS + INSTANCE_APPEARANCE_FLOATS) + (size_t)half * I.cap * INSTANCE_PREV_FLOATS;
 }
 
 // The stored appearance as the kernels read it (common.cuh): tint, opacity, live_k = min(count_k, draw_count) or 0 at opacity 0, pad.
@@ -533,6 +553,7 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
     c->peer_mode = false; c->peer_fb[0] = c->peer_fb[1] = nullptr; c->peer_counter = 0; c->async_counter = 0;
     group_detach(c);   // same for a shard group: every rank resizes, exports and attaches again
     c->scene_depth = nullptr; c->depth_out = nullptr;   // the caller's depth planes have the old size: depth compositing is off
+    c->motion_out = nullptr; c->mot_last.valid = false;   // so are motion vectors, and the next frame has no previous one
     cudaFree(c->pick_strip); c->pick_strip = nullptr;
     GSR_CUDA_TRY(cudaMalloc((void **)&c->bounds, sizeof(uint2) * (size_t)tx * ty));
     GSR_CUDA_TRY(cudaMalloc((void **)&c->comp_order, sizeof(uint32_t) * (size_t)tx * ty));
@@ -707,8 +728,10 @@ static int frame_is_orthographic(const gsr_ctx *c, const float *view_proj, bool 
     return GSR_OK;
 }
 
+// same_frame: gsr_render's re-render of a frame that overflowed -- the same frame again, with the same previous state (motion vectors),
+// and the history does not advance
 static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *uniforms32, float heatmap_factor, float4 *target = nullptr,
-                          const GroupFrame *gf = nullptr) {
+                          const GroupFrame *gf = nullptr, bool same_frame = false) {
     if (!c || !view_proj || !uniforms32) return GSR_ERR_INVALID;
     if (c->width == 0) { set_last_error("gsr_render before gsr_resize"); return GSR_ERR_STATE; }
     bool ortho = false;
@@ -744,6 +767,9 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     // ---- front: rasterizer.gd:127-128 (clear M = this frame's history slot + the scan links), then the projection ----
     if (overlap && c->front_gate) GSR_CUDA_TRY(cudaStreamWaitEvent(fs, c->front_gate, 0));
     const bool inst = c->inst.n > 0 && !gf;   // (a context with instances cannot attach a group)
+    // motion vectors (gsr_set_motion_vectors, read here: frames already enqueued keep their plane): the previous state of this frame
+    const bool motion = c->motion_out && c->depth_out && !gf;
+    const gsr_ctx::MotionState &prev = same_frame ? c->mot_used : c->mot_last;
     {
         uint32_t links = projection_num_blocks((uint32_t)(inst ? c->inst.drawn : c->max_splats));
         if (gf) {
@@ -769,9 +795,22 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         memcpy(c->inst.ring + rs * per, c->inst.xf, sizeof(float) * INSTANCE_XFORM_FLOATS * c->inst.n);
         // the appearance travels in the same slot (read here: frames already enqueued keep theirs); none set: no table this frame
         if (c->inst.app) instance_appearance_rows(c->inst, c->inst.ring + rs * per + app_off);
+        // motion vectors: every instance's previous to_frame travels in the same slot -- the previous frame's where it had the same
+        // layout, else the instance's own (no instance motion, camera motion only)
+        const size_t prev_off = app_off + (size_t)c->inst.cap * INSTANCE_APPEARANCE_FLOATS;
+        if (motion) {
+            const bool same_layout = prev.valid && prev.range.size() == 2ull * c->inst.n &&
+                                     memcmp(prev.range.data(), c->inst.range, sizeof(uint64_t) * 2ull * c->inst.n) == 0;
+            float *pr = c->inst.ring + rs * per + prev_off;
+            for (uint32_t k = 0; k < c->inst.n; ++k)
+                memcpy(pr + (size_t)k * INSTANCE_PREV_FLOATS, same_layout ? prev.to_frame.data() + (size_t)k * INSTANCE_PREV_FLOATS
+                                                                          : c->inst.xf + (size_t)k * INSTANCE_XFORM_FLOATS,
+                       sizeof(float) * INSTANCE_PREV_FLOATS);
+        }
         if ((rc = launch_instance_prepare(c->inst.ring_dev + rs * per, view_proj, u.camera_pos, c->inst.n,
                                           c->inst.frame + (size_t)half * c->inst.cap * INSTANCE_FRAME_FLOATS, fs,
-                                          c->inst.app ? c->inst.ring_dev + rs * per + app_off : nullptr, instance_appearance_table(c->inst, half)))) return rc;
+                                          c->inst.app ? c->inst.ring_dev + rs * per + app_off : nullptr, instance_appearance_table(c->inst, half),
+                                          motion ? c->inst.ring_dev + rs * per + prev_off : nullptr, instance_prev_table(c->inst, half)))) return rc;
         GSR_CUDA_TRY(cudaEventRecord(c->inst.ev[rs], fs));
         c->inst.ev_used[rs] = true;
         c->inst.seq += 1;
@@ -930,7 +969,17 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         if ((rc = launch_group_wait_released(c->grp.flags[c->grp.rank], gf->seq - 2u, s))) return rc;
         launches += 1;
     }
-    if ((rc = launch_composite(ca, s))) return rc;
+    MotionArgs ma;
+    if (motion) {
+        memcpy(ma.vp, view_proj, sizeof ma.vp);
+        memcpy(ma.prev_vp, prev.valid ? prev.vp : view_proj, sizeof ma.prev_vp);
+        ma.fw = (float)(c->width - 1); ma.fh = (float)(c->height - 1);
+        ma.motion_out = c->motion_out;
+        ma.warp_inst = inst ? c->inst.warps : nullptr; ma.desc = c->inst.desc;
+        ma.prev_xf = inst ? instance_prev_table(c->inst, half) : nullptr;
+        ma.plane0 = c->soa; ma.model_scale = u.model_scale;
+    }
+    if ((rc = launch_composite(ca, s, motion ? &ma : nullptr))) return rc;
     launches += ca.num_tiles > 0 ? 1 : 0;
     if (gf && !gf->rows_local) {   // rows have landed in the presenting rank's frame: tell it (system-scope flag store after the kernel boundary)
         if ((rc = launch_group_signal_done(group_peers(c, gf->parity), 0, c->grp.rank, gf->seq, s))) return rc;
@@ -945,6 +994,16 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     c->ev_valid = true;
     c->frame_counter += 1;
     c->last_launches = (uint32_t)launches;
+    if (!same_frame) {   // the history: this frame is the next frame's previous one
+        std::swap(c->mot_used, c->mot_last);
+        gsr_ctx::MotionState &h = c->mot_last;
+        h.valid = true;
+        memcpy(h.vp, view_proj, sizeof h.vp);
+        h.range.assign(inst ? c->inst.range : nullptr, inst ? c->inst.range + 2ull * c->inst.n : nullptr);
+        h.to_frame.resize(inst ? (size_t)INSTANCE_PREV_FLOATS * c->inst.n : 0u);
+        for (uint32_t k = 0; inst && k < c->inst.n; ++k)
+            memcpy(h.to_frame.data() + (size_t)k * INSTANCE_PREV_FLOATS, c->inst.xf + (size_t)k * INSTANCE_XFORM_FLOATS, sizeof(float) * INSTANCE_PREV_FLOATS);
+    }
     return GSR_OK;
 }
 
@@ -961,7 +1020,7 @@ GSR_API int gsr_render(gsr_ctx *c, const float view_proj[32], const void *unifor
             const FrameState &fs = c->host_ring[slot];
             if (!fs.overflow || c->capacity >= c->capacity_max) break;
             if ((rc = grow_capacity(c, fs.dup_total + fs.dup_total / 4ull + 1024ull))) return rc;
-            if ((rc = render_enqueue(c, view_proj, uniforms32, heatmap_factor))) return rc;
+            if ((rc = render_enqueue(c, view_proj, uniforms32, heatmap_factor, nullptr, nullptr, true))) return rc;
         }
         GSR_CUDA_TRY(cudaMemcpyAsync(out_host, framebuffer(c), sizeof(float4) * (size_t)c->width * c->height, cudaMemcpyDeviceToHost, c->stream));
         GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));
@@ -1333,6 +1392,7 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_devic
     if (!depth_out_device) {
         if (scene_depth_device) { set_last_error("gsr_set_depth_compositing: a scene depth needs a depth output"); return GSR_ERR_INVALID; }
         c->scene_depth = nullptr; c->depth_out = nullptr;
+        c->motion_out = nullptr;   // motion vectors are a companion of the mode
         return GSR_OK;
     }
     if (c->width == 0) { set_last_error("gsr_set_depth_compositing before gsr_resize"); return GSR_ERR_STATE; }
@@ -1341,6 +1401,24 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_devic
         return GSR_ERR_STATE;
     }
     c->scene_depth = scene_depth_device; c->depth_out = depth_out_device;
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_motion_vectors(gsr_ctx *c, float *motion_out_device) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!motion_out_device) { c->motion_out = nullptr; return GSR_OK; }
+    if (!c->depth_out) { set_last_error("gsr_set_motion_vectors: depth compositing is off"); return GSR_ERR_STATE; }
+    if (motion_out_device == c->depth_out || motion_out_device == c->scene_depth) {
+        set_last_error("gsr_set_motion_vectors: the motion plane is the depth output or the scene depth");
+        return GSR_ERR_INVALID;
+    }
+    c->motion_out = motion_out_device;   // read by the next render_enqueue: frames already enqueued keep their plane
+    return GSR_OK;
+}
+
+GSR_API int gsr_reset_motion(gsr_ctx *c) {
+    if (!c) return GSR_ERR_INVALID;
+    c->mot_last.valid = false;   // the next frame is its own previous state
     return GSR_OK;
 }
 
@@ -1391,7 +1469,7 @@ static int instance_layout(gsr_ctx *c, const uint64_t *range, uint32_t n, uint64
         if (I.ring) cudaFreeHost(I.ring);
         I.ring = I.ring_dev = nullptr; I.cap = 0;
         GSR_CUDA_TRY(cudaMalloc((void **)&I.desc, sizeof(InstanceDesc) * n));
-        GSR_CUDA_TRY(cudaMalloc((void **)&I.frame, sizeof(float) * 2ull * (INSTANCE_FRAME_FLOATS + INSTANCE_APPEARANCE_FLOATS) * n));
+        GSR_CUDA_TRY(cudaMalloc((void **)&I.frame, sizeof(float) * 2ull * (INSTANCE_FRAME_FLOATS + INSTANCE_APPEARANCE_FLOATS + INSTANCE_PREV_FLOATS) * n));
         if (cudaHostAlloc((void **)&I.ring, sizeof(float) * GSR_INSTANCE_RING * INSTANCE_SLOT_FLOATS * (size_t)n, cudaHostAllocMapped | cudaHostAllocPortable) != cudaSuccess) {
             cudaGetLastError(); I.ring = nullptr; set_last_error("cudaHostAlloc(instance ring) failed"); return GSR_ERR_OOM;
         }

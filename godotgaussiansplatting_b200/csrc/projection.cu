@@ -1229,6 +1229,8 @@ struct InstancePrepareArgs {
     float *out;           // count x INSTANCE_FRAME_FLOATS
     const float *appearance = nullptr;   // count x INSTANCE_APPEARANCE_FLOATS, or null: no appearance table this frame
     float *appearance_out = nullptr;
+    const float *prev_xf = nullptr;      // count x INSTANCE_PREV_FLOATS (motion vectors), or null: no previous transforms this frame
+    float *prev_out = nullptr;
 };
 
 __global__ void __launch_bounds__(256) instance_prepare_kernel(const __grid_constant__ InstancePrepareArgs p) {
@@ -1257,6 +1259,9 @@ __global__ void __launch_bounds__(256) instance_prepare_kernel(const __grid_cons
         uint32_t *dst = reinterpret_cast<uint32_t *>(p.appearance_out);
         for (uint32_t e = threadIdx.x; e < p.count * (uint32_t)INSTANCE_APPEARANCE_FLOATS; e += blockDim.x) dst[e] = src[e];
     }
+    // the previous transforms of the frame's motion vectors, as the host wrote them
+    if (p.prev_xf)
+        for (uint32_t e = threadIdx.x; e < p.count * (uint32_t)INSTANCE_PREV_FLOATS; e += blockDim.x) p.prev_out[e] = p.prev_xf[e];
 }
 
 }  // namespace
@@ -1440,7 +1445,7 @@ int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia,
 }
 
 int launch_instance_prepare(const float *xf, const float *vp, const float *cam, uint32_t count, float *out, cudaStream_t stream,
-                            const float *appearance, float *appearance_out) {
+                            const float *appearance, float *appearance_out, const float *prev_xf, float *prev_out) {
     if (count == 0) return GSR_OK;
     InstancePrepareArgs p;
     p.xf = xf;
@@ -1448,6 +1453,7 @@ int launch_instance_prepare(const float *xf, const float *vp, const float *cam, 
     memcpy(p.cam, cam, sizeof p.cam);
     p.count = count; p.out = out;
     p.appearance = appearance; p.appearance_out = appearance_out;
+    p.prev_xf = prev_xf; p.prev_out = prev_out;
     instance_prepare_kernel<<<1, 256, 0, stream>>>(p);
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;

@@ -243,6 +243,16 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_set_depth_compositing(self._ctx, C.c_void_p(scene_depth_ptr or None), C.c_void_p(depth_out_ptr or None)),
                    "gsr_set_depth_compositing")
 
+    def set_motion_vectors(self, motion_out_ptr: int | None) -> None:
+        """Write the splats' per-pixel screen motion since the previous frame (include/gsr.h gsr_set_motion_vectors): motion_out_ptr =
+        device float[h*w*2], (x, y) in pixels per pixel, previous position minus current; None switches it off.  Needs depth
+        compositing (set_depth_compositing first)."""
+        _lib.check(_lib.lib().gsr_set_motion_vectors(self._ctx, C.c_void_p(motion_out_ptr or None)), "gsr_set_motion_vectors")
+
+    def reset_motion(self) -> None:
+        """A camera cut: the next frame reports no motion (include/gsr.h gsr_reset_motion)."""
+        _lib.check(_lib.lib().gsr_reset_motion(self._ctx), "gsr_reset_motion")
+
     def set_instances(self, instances) -> None:
         """Draw placed, moving and repeated ranges of the splat buffer in one sorted frame (include/gsr.h gsr_set_instances).
         instances: iterable of (first, count, transform), where transform is a Godot Transform3D in matrix form -- a (3, 4) array

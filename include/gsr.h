@@ -317,6 +317,36 @@ GSR_API int gsr_set_framebuffer_external(gsr_ctx *ctx, void *device_ptr);
  *      gsr_pick keeps the default path (and leaves the depth-composited frame as it is).  GSR_ERR_STATE before gsr_resize. ---- */
 GSR_API int gsr_set_depth_compositing(gsr_ctx *ctx, const float *scene_depth_device, float *depth_out_device);
 
+/* ---- Motion vectors: the per-pixel screen motion of the splats since the previous frame, for a host's temporal anti-aliasing,
+ *      upscaler or motion blur (no reference counterpart).  motion_out_device: caller-owned device float[2*width*height], (x, y) per
+ *      pixel, row-major like the frame; NULL switches the mode off.  A companion of depth compositing: GSR_ERR_STATE while depth
+ *      compositing is off (a NULL scene depth is enough), and gsr_set_depth_compositing(ctx, NULL, NULL) and gsr_resize switch it off;
+ *      its single-context rules are those of depth compositing.  GSR_ERR_INVALID, previous state kept: a pointer equal to depth_out or
+ *      scene_depth.  The pointer is read when a frame is enqueued (frames already enqueued keep theirs: a host may double-buffer its
+ *      velocity textures).  The call never synchronises, allocates or copies.
+ *      Motion of one staged splat (float32, one rounding per operation, no contraction):
+ *        - p is the record's frame-space position, the one gsr_pick returns and depth compositing uses; p' its position in the previous
+ *          frame: p' = p without instances (uploads and the load-in animation are not motion); for drawn id v of instance k the source
+ *          splat is s = first_k + (v - 32 w_k), sp = (x_s ms, y_s ms, z_s ms) with this frame's model_scale ms, and
+ *          p'[r] = ((A'[r] sp0 + A'[3+r] sp1) + A'[6+r] sp2) + A'[9+r] with A' instance k's previous to_frame (an unchanged transform
+ *          gives p' == p bit for bit);
+ *        - pix(M, q) for a view_proj M = (V, P): view[r] = ((V[r] q0 + V[4+r] q1) + V[8+r] q2) + V[12+r],
+ *          clip[r] = ((P[r] view0 + P[4+r] view1) + P[8+r] view2) + P[12+r] view3 (r = 0, 1, 3), and
+ *          pix = (((clip0/clip3 + 1) 0.5) (W-1), ((clip1/clip3 + 1) 0.5) (H-1)): the projection's image_pos without the load-in term;
+ *        - m = pix(M', p') - pix(M, p), previous minus current, in the frame's pixel axes (column, row; y grows downwards); (0, 0) unless
+ *          clip3' > 0 and both components are finite.
+ *      Per pixel m.x and m.y accumulate exactly like depth_out (same stop rule and transmittance: fma(m alpha, t, M), unfused under
+ *      GSR_FLAG_UNCONTRACTED_BLEND), and motion_out = (Mx / (1 - t), My / (1 - t)), (0, 0) where 1 - t == 0.  rgba and depth_out are
+ *      bit-identical to the frame without motion vectors.
+ *      Previous state: the context records the view_proj and the instance transforms of every frame enqueued by gsr_render* (motion on
+ *      or off); a frame's previous state is the last enqueued frame's, except that it is the frame's own for the context's first frame,
+ *      the first frame after gsr_resize and the first after gsr_reset_motion (a camera cut), and, per instance, when the previous frame
+ *      had a different instance layout (another (first, count) sequence, or no instances).  gsr_render's re-render of a frame that
+ *      overflowed is the same frame with the same previous state; gsr_pick neither reads nor updates the history and leaves
+ *      motion_out as it is. ---- */
+GSR_API int gsr_set_motion_vectors(gsr_ctx *ctx, float *motion_out_device);
+GSR_API int gsr_reset_motion(gsr_ctx *ctx);
+
 /* ---- Splat instances (no reference counterpart: the reference draws one cloud at the origin).  An instance draws the source range
  *      [first, first + count) of the uploaded splats with its own affine transform `to_frame` = [A | t] (3x4, column-major: columns
  *      a0, a1, a2, t) from the range's splat coordinates (position * model_scale) into FRAME space, the space the uploaded splats, the
