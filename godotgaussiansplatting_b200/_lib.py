@@ -26,13 +26,14 @@ GSR_CUTOUT_FRAME, GSR_CUTOUT_SOURCE = 0, 1
 GSR_MAX_INSTANCES, GSR_INSTANCE_RING = 4096, 8
 GSR_TINT_MAX = 16.0
 GSR_DRAW_ALL = 0xFFFFFFFFFFFFFFFF   # gsr_instance_appearance.draw_count: every splat of the range
+GSR_NO_ID = 0xFFFFFFFF              # gsr_set_splat_ids: no splat / no instance
 
 # every symbol include/gsr.h declares (tests/test_abi.py checks the header against this list and the .so)
 EXPORTS = [
     "gsr_create", "gsr_destroy", "gsr_set_stream", "gsr_upload_splats_aos", "gsr_upload_ply_raw", "gsr_upload_ply", "gsr_resize", "gsr_set_band", "gsr_set_row_interleave", "gsr_band_sync_word", "gsr_band_fixup", "gsr_render",
     "gsr_render_async", "gsr_render_async_rgb", "gsr_render_async_fmt", "gsr_output_bytes", "gsr_present_device", "gsr_readback_async", "gsr_peer_export_framebuffers", "gsr_peer_import_framebuffers",
     "gsr_stream_join", "gsr_group_export", "gsr_group_attach", "gsr_group_detach", "gsr_group_set_present", "gsr_readback_rows_async", "gsr_sync", "gsr_framebuffer_device_ptr", "gsr_set_framebuffer_external",
-    "gsr_set_depth_compositing", "gsr_set_motion_vectors", "gsr_reset_motion", "gsr_set_instances", "gsr_set_instance_appearance", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_set_cutouts", "gsr_upload_ply_filtered", "gsr_pick",
+    "gsr_set_depth_compositing", "gsr_set_motion_vectors", "gsr_reset_motion", "gsr_set_splat_ids", "gsr_set_instances", "gsr_set_instance_appearance", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_set_cutouts", "gsr_upload_ply_filtered", "gsr_pick",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -133,6 +134,7 @@ def lib():
         L.gsr_set_depth_compositing.argtypes = [vp, vp, vp]
         L.gsr_set_motion_vectors.argtypes = [vp, vp]
         L.gsr_reset_motion.argtypes = [vp]
+        L.gsr_set_splat_ids.argtypes = [vp, vp]
         L.gsr_set_instances.argtypes = [vp, C.POINTER(GsrInstance), u32]
         L.gsr_set_instance_appearance.argtypes = [vp, C.POINTER(GsrInstanceAppearance), u32]
         L.gsr_set_sh_degree.argtypes = [vp, C.c_int32]

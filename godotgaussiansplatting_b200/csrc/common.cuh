@@ -392,7 +392,15 @@ struct MotionArgs {
     const float4 *plane0;       // plane 0 of the store
     float model_scale;
 };
-int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion = nullptr);
+// Splat and instance IDs (gsr_set_splat_ids, with depth compositing only): carried in the second __grid_constant__ parameter of the ID
+// variants of the compositor, beside the motion constants when both are on.  Per pixel, the drawn id v of the blended splat with the
+// largest t - t * (1 - alpha) (the first in sorted order on a tie) and warp_inst[v >> 5].
+constexpr uint32_t NO_ID = 0xFFFFFFFFu;
+struct SplatIdArgs {
+    uint32_t *ids_out;          // W*H uint2 (v, k); (NO_ID, NO_ID) where no splat has t - t' > 0
+    const uint32_t *warp_inst;  // instance of every drawn warp; nullptr: no instances, k = NO_ID
+};
+int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion = nullptr, const SplatIdArgs *ids = nullptr);
 int composite_max_ctas_per_sm(int *out);
 // order[0 .. num_tiles) = owned-tile indices sorted by descending expected chain length: the chunk count the tile consumed in the
 // previous frame (hint[k] with bit 31 set; the bit is cleared here) or, without a hint, its list length in chunks capped at

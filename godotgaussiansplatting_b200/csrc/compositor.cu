@@ -33,6 +33,11 @@
 // m = pix(M', p') - pix(M, p) (motion_of below), accumulated per pixel like the depth, and the output is M / (1 - t).  The per-splat
 // loads are issued when the chunk is gathered and the arithmetic runs when it is stored to shared memory.  The constants travel in a
 // second __grid_constant__ parameter; the other variants take an empty placeholder there and compile to the code they had before.
+// Splat IDs (composite_ids_kernel, IDS = true in composite_tiles, gsr_set_splat_ids; always with DEPTH, with or without MOTION): the
+// staged chunk also carries each splat's drawn id v (s_v), and every pixel tracks the blended splat with the largest w = t - t'
+// (t' = t * (1 - alpha), the value the blend stores), replaced only by a strictly larger w.  The compare and selects sit beside the
+// transmittance chain, not on it.  The output is (v, warp_inst[v >> 5]) per pixel, (NO_ID, NO_ID) where no w was > 0.  Its pointers
+// travel in the second parameter too.
 #include <stdlib.h>
 #include <string.h>
 
@@ -91,12 +96,21 @@ struct NoMotion {};
 template <bool MOTION> struct MotionParamT { using type = NoMotion; using pending = NoMotion; };
 template <> struct MotionParamT<true> { using type = MotionArgs; using pending = MotionPending; };
 template <bool MOTION> using MotionParam = typename MotionParamT<MOTION>::type;
-template <bool MOTION> using Pending = typename MotionParamT<MOTION>::pending;
+// IDS without MOTION: the gather keeps only the drawn id (MotionPending carries it too)
+struct IdPending { uint32_t v; };
+template <bool MOTION, bool IDS> struct PendingT { using type = typename MotionParamT<MOTION>::pending; };
+template <> struct PendingT<false, true> { using type = IdPending; };
+template <bool MOTION, bool IDS = false> using Pending = typename PendingT<MOTION, IDS>::type;
+// IDS: the second parameter is the motion one (or the placeholder) extended by the ID pointers, so the motion code reads it unchanged
+template <bool MOTION> struct WithIds : MotionParam<MOTION> { SplatIdArgs ids; };
+template <bool MOTION, bool IDS> struct SecondParamT { using type = MotionParam<MOTION>; };
+template <bool MOTION> struct SecondParamT<MOTION, true> { using type = WithIds<MOTION>; };
+template <bool MOTION, bool IDS> using SecondParam = typename SecondParamT<MOTION, IDS>::type;
 
 // vz = (V[2], V[6], V[10], V[14]): the view-matrix row of the depth (DEPTH only)
-template <bool DEPTH, bool MOTION = false>
+template <bool DEPTH, bool MOTION = false, bool IDS = false>
 __device__ __forceinline__ Staged gather(const float4 *__restrict__ records, const uint32_t *__restrict__ values, uint32_t idx, float4 vz,
-                                         Pending<MOTION> *mp = nullptr, const MotionParam<MOTION> *mo = nullptr) {
+                                         Pending<MOTION, IDS> *mp = nullptr, const MotionParam<MOTION> *mo = nullptr) {
     const uint32_t v = __ldg(values + idx);
     const float4 *r = records + (uint64_t)v * 3u;
     const float4 r0 = __ldg(r + 0), r1 = __ldg(r + 1), r2 = __ldg(r + 2);
@@ -108,6 +122,8 @@ __device__ __forceinline__ Staged gather(const float4 *__restrict__ records, con
     if constexpr (MOTION) {   // (the instance load only depends on v: it runs beside the record loads)
         mp->v = v; mp->k = mo->warp_inst ? __ldg(mo->warp_inst + (v >> 5)) : 0xFFFFFFFFu;
         mp->p0 = r0.z; mp->p1 = r0.w; mp->p2 = r1.w;
+    } else if constexpr (IDS) {
+        mp->v = v;
     }
     return s;
 }
@@ -245,10 +261,19 @@ __device__ __forceinline__ void phase_a(const float4 A[GU], const float4 B[GU], 
 //      DEPTH: o0/o1 = "not stopped by the scene depth" (z0/z1); a live pixel stops at the first splat with !(d < z), before blending
 //      it; a stopped pixel is dead from then on.  dd2 accumulates d * alpha * t exactly like a colour channel.
 //      MOTION: mx2 / my2 accumulate the staged motion (s_m) exactly like the depth.
-template <bool CONTRACT, bool DEPTH, bool MOTION = false>
+//      IDS: a blended splat with w = t - t' > the pixel's best w so far becomes the pixel's splat (s_v).
+struct IdState {   // IDS: the two pixels' largest w and its drawn id
+    float best0, best1;
+    uint32_t id0, id1;
+};
+template <bool IDS> struct IdStateT { using type = NoMotion; };
+template <> struct IdStateT<true> { using type = IdState; };
+template <bool IDS> using IdStateOf = typename IdStateT<IDS>::type;
+template <bool CONTRACT, bool DEPTH, bool MOTION = false, bool IDS = false>
 __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, const float *s_d, int j, const F2 al2[GU], const F2 om2[GU], F2 &cr2,
                                         F2 &cg2, F2 &cb2, float &t0, float &t1, bool &alive_mid, float z0, float z1, bool &o0, bool &o1, F2 &dd2,
-                                        const float2 *s_m = nullptr, F2 *mx2 = nullptr, F2 *my2 = nullptr) {
+                                        const float2 *s_m = nullptr, F2 *mx2 = nullptr, F2 *my2 = nullptr, const uint32_t *s_v = nullptr,
+                                        IdStateOf<IDS> *ids = nullptr) {
 #pragma unroll
     for (int u = 0; u < GU; ++u) {
         const float cbl = s_c[j + u];
@@ -291,6 +316,13 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, co
                 *my2 = mul_add2_unfused(mul2(bc(mv.y), m2), t2, *my2);
             }
         }
+        if constexpr (IDS) {
+            const uint32_t vj = s_v[j + u];
+            const float w0 = __fsub_rn(t0, pl), w1 = __fsub_rn(t1, ph);
+            const bool b0 = a0 && w0 > ids->best0, b1 = a1 && w1 > ids->best1;
+            ids->best0 = b0 ? w0 : ids->best0; ids->id0 = b0 ? vj : ids->id0;
+            ids->best1 = b1 ? w1 : ids->best1; ids->id1 = b1 ? vj : ids->id1;
+        }
         t0 = a0 ? pl : t0;
         t1 = a1 ? ph : t1;
     }
@@ -301,17 +333,21 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, co
 #endif
 
 // Persistent CTAs.  Ticket k of the launch renders owned tile order[k] (longest chains first) or k itself; every tile is blended
-// from its first chunk to its stop by the CTA that took it.
+// from its first chunk to its stop by the CTA that took it.  The body of composite_kernel and composite_ids_kernel; p and mo are
+// their __grid_constant__ parameters (p taken by value: the inlined copy folds away, and composite_kernel compiles to the same
+// code as when this body was its own).
 // MOTION (gsr_set_motion_vectors, with DEPTH only): the motion constants in `mo`; the other variants take an empty placeholder.
-template <bool CONTRACT, bool DEPTH = false, bool MOTION = false>
-__global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel(const __grid_constant__ CompositeArgs p,
-                                                                                 const __grid_constant__ MotionParam<MOTION> mo = MotionParam<MOTION>()) {
+// IDS (gsr_set_splat_ids, with DEPTH only): `mo` also carries the ID pointers (mo.ids).
+template <bool CONTRACT, bool DEPTH, bool MOTION, bool IDS>
+__device__ __forceinline__ void composite_tiles(const CompositeArgs p, const SecondParam<MOTION, IDS> &mo) {
     static_assert(!MOTION || DEPTH, "motion vectors are a companion of depth compositing");
+    static_assert(!IDS || DEPTH, "splat IDs are a companion of depth compositing");
     __shared__ float4 s_a[CHUNK];
     __shared__ float4 s_b[CHUNK];
     __shared__ float s_c[CHUNK];
     __shared__ float s_d[DEPTH ? CHUNK : 1];   // view depth of the staged splats
     __shared__ float2 s_m[MOTION ? CHUNK : 1]; // MOTION: screen motion of the staged splats
+    __shared__ uint32_t s_v[IDS ? CHUNK : 1];  // IDS: drawn id of the staged splats
     __shared__ uint32_t s_vote[THREADS / 32];
     __shared__ uint32_t s_tile;
 
@@ -352,6 +388,8 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         bool o0 = true, o1 = true;                     // DEPTH: not stopped by the scene depth
         F2 dd2 = pk(0.f, 0.f);                         // DEPTH: accumulated depth
         F2 mx2 = pk(0.f, 0.f), my2 = mx2;              // MOTION: accumulated motion
+        IdStateOf<IDS> ids;                              // IDS: largest w so far (0: none) and its drawn id
+        if constexpr (IDS) ids = IdState{0.f, 0.f, NO_ID, NO_ID};
         float z0 = __uint_as_float(0x7f800000u), z1 = z0; // DEPTH: scene depth (+inf: nothing occludes; also outside the image)
         if (DEPTH && p.scene_depth && py < p.height) {
             const float *zrow = p.scene_depth + (uint64_t)py * (uint64_t)p.width;
@@ -360,11 +398,12 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
         }
 
         Staged n0 = null_splat(), n1 = null_splat();
-        Pending<MOTION> q0, q1;   // MOTION: the gathered splats' pending motion loads
+        Pending<MOTION, IDS> q0, q1;   // MOTION: the gathered splats' pending motion loads; IDS: their drawn ids
         if constexpr (MOTION) { q0 = null_motion(); q1 = null_motion(); }
+        else if constexpr (IDS) { q0.v = NO_ID; q1.v = NO_ID; }
         if (num_iterations > 0) {
-            if ((int)tid < num_splats) n0 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + tid, vz, &q0, &mo);
-            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + tid + THREADS, vz, &q1, &mo);
+            if ((int)tid < num_splats) n0 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + tid, vz, &q0, &mo);
+            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + tid + THREADS, vz, &q1, &mo);
         }
 
         int consumed = 0;  // chunks blended before the stop rule fired (next frame's scheduling hint)
@@ -377,14 +416,16 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
             s_a[tid + THREADS] = n1.a; s_b[tid + THREADS] = n1.b; s_c[tid + THREADS] = n1.c;
             if constexpr (DEPTH) { s_d[tid] = n0.d; s_d[tid + THREADS] = n1.d; }
             if constexpr (MOTION) { s_m[tid] = motion_of(mo, q0); s_m[tid + THREADS] = motion_of(mo, q1); }
+            if constexpr (IDS) { s_v[tid] = q0.v; s_v[tid + THREADS] = q1.v; }   // (a null splat: alpha 0, w = 0, never the pixel's)
             __syncthreads();
             // prefetch the next chunk's records while this one is blended (slots past the list end become null splats)
             n0 = null_splat(); n1 = null_splat();
             if constexpr (MOTION) { q0 = null_motion(); q1 = null_motion(); }
+            else if constexpr (IDS) { q0.v = NO_ID; q1.v = NO_ID; }
             if (i + 1 < num_iterations) {
                 const int nb = sort_offset + CHUNK;
-                if (nb + (int)tid < num_splats) n0 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz, &q0, &mo);
-                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz, &q1, &mo);
+                if (nb + (int)tid < num_splats) n0 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz, &q0, &mo);
+                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz, &q1, &mo);
             }
 
             // :79-91, GU splats per iteration; `chunk` rounded up to GU reads null splats (opacity 0 => exact no-op).  Software-pipelined:
@@ -407,7 +448,8 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
 #pragma unroll
                 for (int u = 0; u < GU; ++u) { A[u] = s_a[jn + u]; B[u] = s_b[jn + u]; }
                 bool alive_mid = true;
-                phase_b<CONTRACT, DEPTH, MOTION>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2, s_m, &mx2, &my2);
+                phase_b<CONTRACT, DEPTH, MOTION, IDS>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2, s_m, &mx2, &my2,
+                                                      s_v, &ids);
                 go = __any_sync(0xffffffffu, alive_mid);
             }
 
@@ -451,6 +493,14 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
                 if (px0 < p.width) mrow[px0] = k0 != 0.0f ? make_float2(__fdiv_rn(mx0, k0), __fdiv_rn(my0, k0)) : make_float2(0.f, 0.f);
                 if (px0 + 1 < p.width) mrow[px0 + 1] = k1 != 0.0f ? make_float2(__fdiv_rn(mx1, k1), __fdiv_rn(my1, k1)) : make_float2(0.f, 0.f);
             }
+            if constexpr (IDS) {   // (v, instance of v's warp), (NO_ID, NO_ID) where no splat had w > 0
+                const uint32_t *wi = mo.ids.warp_inst;
+                uint2 *irow = reinterpret_cast<uint2 *>(mo.ids.ids_out) + (uint64_t)py * (uint64_t)p.width;
+                if (px0 < p.width)
+                    irow[px0] = ids.best0 > 0.0f ? make_uint2(ids.id0, wi ? __ldg(wi + (ids.id0 >> 5)) : NO_ID) : make_uint2(NO_ID, NO_ID);
+                if (px0 + 1 < p.width)
+                    irow[px0 + 1] = ids.best1 > 0.0f ? make_uint2(ids.id1, wi ? __ldg(wi + (ids.id1 >> 5)) : NO_ID) : make_uint2(NO_ID, NO_ID);
+            }
         }
         // :105-110 pick: the elected (first) lane of each 32-wide subgroup of the reference's 16x16 workgroup is local
         // index 32*s = pixel (0, 2*s) of the tile = first pixel of thread 16*s here
@@ -472,6 +522,21 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel
     if (tid == 0 && staged && p.count_staged) atomicAdd(&p.frame->staged, (unsigned long long)staged);
 }
 
+template <bool CONTRACT, bool DEPTH = false, bool MOTION = false>
+__global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_kernel(const __grid_constant__ CompositeArgs p,
+                                                                                 const __grid_constant__ MotionParam<MOTION> mo = MotionParam<MOTION>()) {
+    composite_tiles<CONTRACT, DEPTH, MOTION, false>(p, mo);
+}
+
+// Splat IDs (gsr_set_splat_ids): the depth-compositing frame, with or without motion vectors, plus the ID plane.  The same body as
+// composite_kernel<CONTRACT, true, MOTION>; a kernel of its own, so the set of composite_kernel instantiations stays one per frame
+// variant of the colour / depth / motion outputs.
+template <bool CONTRACT, bool MOTION>
+__global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_ids_kernel(const __grid_constant__ CompositeArgs p,
+                                                                                     const __grid_constant__ WithIds<MOTION> mo) {
+    composite_tiles<CONTRACT, true, MOTION, true>(p, mo);
+}
+
 }  // namespace
 
 #ifndef GSR_CPU_EMU
@@ -483,31 +548,54 @@ int preload_composite_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<true, true, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_kernel<false, true, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<true, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<false, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<true, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<false, true>));
     return GSR_OK;
 }
 
 int composite_max_ctas_per_sm(int *out) {
-    int a = 0, b = 0, c = 0, d = 0, e = 0, f = 0;
+    int a = 0, b = 0, c = 0, d = 0, e = 0, f = 0, g = 0, h = 0, i = 0, j = 0;
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, composite_kernel<true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, composite_kernel<false>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, composite_kernel<true, true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&d, composite_kernel<false, true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&e, composite_kernel<true, true, true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&f, composite_kernel<false, true, true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&g, composite_ids_kernel<true, false>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h, composite_ids_kernel<false, false>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&i, composite_ids_kernel<true, true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&j, composite_ids_kernel<false, true>, THREADS, 0));
     if (c < a) a = c;
     if (d < b) b = d;
     if (e < a) a = e;
     if (f < b) b = f;
+    if (g < a) a = g;
+    if (h < b) b = h;
+    if (i < a) a = i;
+    if (j < b) b = j;
     *out = a < b ? a : b;
     if (*out < 1) *out = 1;
     return GSR_OK;
 }
 
-int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion) {
+int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion, const SplatIdArgs *ids) {
     if (a.num_tiles <= 0) return GSR_OK;
     const int per_sm = a.ctas_per_sm > 0 ? a.ctas_per_sm : 1;
     const int grid = a.num_tiles < a.sm_count * per_sm ? a.num_tiles : a.sm_count * per_sm;
-    if (a.depth_out && motion) {   // motion vectors (gsr_set_motion_vectors)
+    if (a.depth_out && ids && motion) {   // splat IDs and motion vectors (gsr_set_splat_ids + gsr_set_motion_vectors)
+        WithIds<true> x;
+        static_cast<MotionArgs &>(x) = *motion;
+        x.ids = *ids;
+        if (a.contract) composite_ids_kernel<true, true><<<grid, THREADS, 0, stream>>>(a, x);
+        else composite_ids_kernel<false, true><<<grid, THREADS, 0, stream>>>(a, x);
+    } else if (a.depth_out && ids) {   // splat IDs (gsr_set_splat_ids)
+        WithIds<false> x;
+        x.ids = *ids;
+        if (a.contract) composite_ids_kernel<true, false><<<grid, THREADS, 0, stream>>>(a, x);
+        else composite_ids_kernel<false, false><<<grid, THREADS, 0, stream>>>(a, x);
+    } else if (a.depth_out && motion) {   // motion vectors (gsr_set_motion_vectors)
         if (a.contract) composite_kernel<true, true, true><<<grid, THREADS, 0, stream>>>(a, *motion);
         else composite_kernel<false, true, true><<<grid, THREADS, 0, stream>>>(a, *motion);
     } else if (a.depth_out) {   // depth compositing (gsr_set_depth_compositing)

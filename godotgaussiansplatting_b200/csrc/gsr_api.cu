@@ -77,6 +77,8 @@ struct gsr_ctx {
     float *depth_out = nullptr;
     // motion vectors (gsr_set_motion_vectors, with depth compositing): caller-owned W*H float2 plane; nullptr = off
     float *motion_out = nullptr;
+    // splat IDs (gsr_set_splat_ids, with depth compositing): caller-owned W*H uint32 pair plane; nullptr = off
+    uint32_t *ids_out = nullptr;
     // The camera and instance transforms of a frame, recorded for every frame enqueued by gsr_render* (motion on or off): `mot_last` is
     // the last enqueued frame's, the previous state of the next frame; `mot_used` is the previous state the last frame was enqueued
     // with (gsr_render's re-render of an overflowed frame uses it again).  valid == false: no previous frame (first frame, gsr_resize,
@@ -554,6 +556,7 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
     group_detach(c);   // same for a shard group: every rank resizes, exports and attaches again
     c->scene_depth = nullptr; c->depth_out = nullptr;   // the caller's depth planes have the old size: depth compositing is off
     c->motion_out = nullptr; c->mot_last.valid = false;   // so are motion vectors, and the next frame has no previous one
+    c->ids_out = nullptr;                                  // and splat IDs
     cudaFree(c->pick_strip); c->pick_strip = nullptr;
     GSR_CUDA_TRY(cudaMalloc((void **)&c->bounds, sizeof(uint2) * (size_t)tx * ty));
     GSR_CUDA_TRY(cudaMalloc((void **)&c->comp_order, sizeof(uint32_t) * (size_t)tx * ty));
@@ -770,6 +773,8 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     // motion vectors (gsr_set_motion_vectors, read here: frames already enqueued keep their plane): the previous state of this frame
     const bool motion = c->motion_out && c->depth_out && !gf;
     const gsr_ctx::MotionState &prev = same_frame ? c->mot_used : c->mot_last;
+    // splat IDs (gsr_set_splat_ids), read here as well
+    const bool ids = c->ids_out && c->depth_out && !gf;
     {
         uint32_t links = projection_num_blocks((uint32_t)(inst ? c->inst.drawn : c->max_splats));
         if (gf) {
@@ -979,7 +984,10 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         ma.prev_xf = inst ? instance_prev_table(c->inst, half) : nullptr;
         ma.plane0 = c->soa; ma.model_scale = u.model_scale;
     }
-    if ((rc = launch_composite(ca, s, motion ? &ma : nullptr))) return rc;
+    SplatIdArgs sa;
+    sa.ids_out = c->ids_out;
+    sa.warp_inst = inst ? c->inst.warps : nullptr;
+    if ((rc = launch_composite(ca, s, motion ? &ma : nullptr, ids ? &sa : nullptr))) return rc;
     launches += ca.num_tiles > 0 ? 1 : 0;
     if (gf && !gf->rows_local) {   // rows have landed in the presenting rank's frame: tell it (system-scope flag store after the kernel boundary)
         if ((rc = launch_group_signal_done(group_peers(c, gf->parity), 0, c->grp.rank, gf->seq, s))) return rc;
@@ -1393,6 +1401,7 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_devic
         if (scene_depth_device) { set_last_error("gsr_set_depth_compositing: a scene depth needs a depth output"); return GSR_ERR_INVALID; }
         c->scene_depth = nullptr; c->depth_out = nullptr;
         c->motion_out = nullptr;   // motion vectors are a companion of the mode
+        c->ids_out = nullptr;      // and so are splat IDs
         return GSR_OK;
     }
     if (c->width == 0) { set_last_error("gsr_set_depth_compositing before gsr_resize"); return GSR_ERR_STATE; }
@@ -1412,7 +1421,24 @@ GSR_API int gsr_set_motion_vectors(gsr_ctx *c, float *motion_out_device) {
         set_last_error("gsr_set_motion_vectors: the motion plane is the depth output or the scene depth");
         return GSR_ERR_INVALID;
     }
+    if (c->ids_out && (const void *)motion_out_device == (const void *)c->ids_out) {
+        set_last_error("gsr_set_motion_vectors: the motion plane is the splat ID plane");
+        return GSR_ERR_INVALID;
+    }
     c->motion_out = motion_out_device;   // read by the next render_enqueue: frames already enqueued keep their plane
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_splat_ids(gsr_ctx *c, uint32_t *ids_out_device) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!ids_out_device) { c->ids_out = nullptr; return GSR_OK; }
+    if (!c->depth_out) { set_last_error("gsr_set_splat_ids: depth compositing is off"); return GSR_ERR_STATE; }
+    const void *p = ids_out_device;
+    if (p == (const void *)c->depth_out || p == (const void *)c->scene_depth || p == (const void *)c->motion_out) {
+        set_last_error("gsr_set_splat_ids: the ID plane is the depth output, the scene depth or the motion plane");
+        return GSR_ERR_INVALID;
+    }
+    c->ids_out = ids_out_device;   // read by the next render_enqueue: frames already enqueued keep their plane
     return GSR_OK;
 }
 

@@ -76,6 +76,7 @@ class GaussianSplattingRasterizer:
         self._antialiasing = float(antialiasing) if antialiasing is not None else (0.1 if has_filter_3d else 0.0)
         self._depth_order = int(depth_order)
         self._cutouts = []   # gsr_cutout entries of set_cutouts, applied again by init_gpu
+        self._instance_ranges = None   # (first, count) per instance of the current set_instances layout; None: no instances
         self._clock = clock or (lambda: _time.monotonic())
         self._t0 = self._clock()
         self.tile_dims = (0, 0)
@@ -253,6 +254,17 @@ class GaussianSplattingRasterizer:
         """A camera cut: the next frame reports no motion (include/gsr.h gsr_reset_motion)."""
         _lib.check(_lib.lib().gsr_reset_motion(self._ctx), "gsr_reset_motion")
 
+    def set_splat_ids(self, ids_out_ptr: int | None) -> None:
+        """Write, per pixel, the splat and the instance that dominate the blend (include/gsr.h gsr_set_splat_ids): ids_out_ptr = device
+        uint32[h*w*2], (drawn id v, instance k) per pixel, GSR_NO_ID where no splat covers it; None switches it off.  Needs depth
+        compositing (set_depth_compositing first).  splat_sources maps the array to source splat indices."""
+        _lib.check(_lib.lib().gsr_set_splat_ids(self._ctx, C.c_void_p(ids_out_ptr or None)), "gsr_set_splat_ids")
+
+    def splat_sources(self, ids: np.ndarray) -> np.ndarray:
+        """The source splat index of every pixel of an (h, w, 2) array read back from set_splat_ids' plane, under the current instance
+        layout (set_instances): GSR_NO_ID where the pixel has no splat.  Valid for frames rendered with that layout."""
+        return splat_sources(ids, self._instance_ranges)
+
     def set_instances(self, instances) -> None:
         """Draw placed, moving and repeated ranges of the splat buffer in one sorted frame (include/gsr.h gsr_set_instances).
         instances: iterable of (first, count, transform), where transform is a Godot Transform3D in matrix form -- a (3, 4) array
@@ -265,6 +277,7 @@ class GaussianSplattingRasterizer:
             arr[k].first, arr[k].count = int(first), int(count)
             arr[k].to_frame[:] = [float(v) for v in godot_to_frame(transform, self.basis_override).T.reshape(12)]
         _lib.check(_lib.lib().gsr_set_instances(self._ctx, arr, len(items)), "gsr_set_instances")
+        self._instance_ranges = [(int(first), int(count)) for first, count, _ in items] if items else None
 
     def set_instance_appearance(self, appearance) -> None:
         """Show, hide, fade, tint and shorten the instances of set_instances, per frame and without a host synchronisation (include/gsr.h
@@ -317,6 +330,7 @@ class GaussianSplattingRasterizer:
         if self._ctx:
             _lib.lib().gsr_destroy(self._ctx)
             self._ctx = C.c_void_p(None)
+            self._instance_ranges = None
         if self.render_texture:
             self.render_texture.device_ptr = 0
 
@@ -464,6 +478,26 @@ def pack_instance_appearance(appearance):
         arr[k].opacity = float(opacity)
         arr[k].draw_count = _lib.GSR_DRAW_ALL if draw_count is None else int(draw_count)
     return arr
+
+
+def splat_sources(ids: np.ndarray, ranges=None) -> np.ndarray:
+    """(h, w, 2) uint32 (v, k) of gsr_set_splat_ids -> (h, w) uint32 source splat indices.  ranges: the (first, count) per instance of
+    the frame's gsr_set_instances layout, or None without instances (the source is v).  Instance k's drawn ids start at warp
+    w_k = sum of ceil(count_j / 32) over j < k, so v maps to first_k + (v - 32 w_k).  GSR_NO_ID stays GSR_NO_ID."""
+    ids = np.asarray(ids, dtype=np.uint32)
+    assert ids.shape[-1] == 2, ids.shape
+    v, k = ids[..., 0], ids[..., 1]
+    out = np.full(v.shape, _lib.GSR_NO_ID, dtype=np.uint32)
+    hit = v != _lib.GSR_NO_ID
+    if not ranges:
+        out[hit] = v[hit]
+        return out
+    counts = np.array([int(c) for _, c in ranges], dtype=np.int64)
+    w0 = np.concatenate([[0], np.cumsum((counts + 31) // 32)[:-1]])
+    first = np.array([int(f) for f, _ in ranges], dtype=np.int64)
+    kk = k[hit].astype(np.int64)
+    out[hit] = (first[kk] + (v[hit].astype(np.int64) - 32 * w0[kk])).astype(np.uint32)
+    return out
 
 
 def godot_to_frame(transform, basis_override) -> np.ndarray:

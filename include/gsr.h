@@ -347,6 +347,29 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *ctx, const float *scene_depth_dev
 GSR_API int gsr_set_motion_vectors(gsr_ctx *ctx, float *motion_out_device);
 GSR_API int gsr_reset_motion(gsr_ctx *ctx);
 
+/* ---- Splat and instance IDs: per pixel, which splat and which instance dominate the depth-composited blend, for click picking,
+ *      selection outlines and any post effect that needs to know which object owns a pixel (no reference counterpart).
+ *      ids_out_device: caller-owned device uint32_t[2*width*height], (v, k) per pixel, row-major like the frame; NULL switches the
+ *      mode off.  A companion of depth compositing: GSR_ERR_STATE while depth compositing is off (a NULL scene depth is enough), and
+ *      gsr_set_depth_compositing(ctx, NULL, NULL) and gsr_resize switch it off; its single-context rules are those of depth
+ *      compositing.  GSR_ERR_INVALID, previous state kept: a pointer equal to depth_out, scene_depth or motion_out
+ *      (gsr_set_motion_vectors likewise refuses the ID plane while IDs are on).  The pointer is read when a frame is enqueued (frames
+ *      already enqueued keep theirs: a host may double-buffer).  The call never synchronises, allocates or copies.
+ *      Rule: a pixel's splats are those its depth-composited blend blends (same stop rule at the scene depth, same dead-pixel rule
+ *      t > 1/255, same sorted order).  For each, w = t - t' in float32 (one subtraction), with t the pixel's transmittance before the
+ *      splat and t' = t * (1 - alpha) the value the blend stores after it; alpha is that of the context's blend (contracted, or
+ *      GSR_FLAG_UNCONTRACTED_BLEND).  The pixel's splat is the first in sorted order with the largest w: a later splat replaces it
+ *      only when its w is strictly greater.
+ *        v = its drawn id, the sort value: the splat index without instances; with instances, drawn id v of instance k maps to source
+ *            splat first_k + (v - 32 w_k) (see gsr_set_instances);
+ *        k = the instance that owns drawn warp v >> 5, GSR_NO_ID without instances.
+ *      A pixel where no splat has w > 0 (exactly where the coverage alpha 1 - t is 0) holds (GSR_NO_ID, GSR_NO_ID).  Hidden
+ *      instances and splats beyond an instance's draw_count are never blended, so they never appear.  rgba, depth_out and motion_out
+ *      are bit-identical to the frame without IDs; pixels outside the image are not written.  gsr_render's re-render of a frame
+ *      that overflowed writes the same IDs; gsr_pick keeps the default path and leaves the ID plane as it is. ---- */
+#define GSR_NO_ID 0xFFFFFFFFu
+GSR_API int gsr_set_splat_ids(gsr_ctx *ctx, uint32_t *ids_out_device);
+
 /* ---- Splat instances (no reference counterpart: the reference draws one cloud at the origin).  An instance draws the source range
  *      [first, first + count) of the uploaded splats with its own affine transform `to_frame` = [A | t] (3x4, column-major: columns
  *      a0, a1, a2, t) from the range's splat coordinates (position * model_scale) into FRAME space, the space the uploaded splats, the
