@@ -245,6 +245,31 @@ bool reduced_sh(const gsr_ctx *c) { return c->sh_bands < SH_BANDS_MAX || render_
 bool view_depth_order(const gsr_ctx *c) { return c->depth_order == GSR_DEPTH_ORDER_VIEW_DEPTH; }
 bool cutouts_on(const gsr_ctx *c) { return c->cutouts.n_keep + c->cutouts.n_remove != 0u; }
 
+// The single-context rule (gsr.h, "Single-context features") is decided by these two functions only: a call that would shard the
+// context refuses while single_context_feature() names a feature, and a call that would turn a feature on refuses while sharded().
+// So no frame of a shard group, of peer framebuffers, of a partial band or of row interleave has any of these features.
+//
+// The reason text of the first feature that is on, or nullptr.  for_group_export skips depth compositing and instances:
+// gsr_group_export accepts them, and only gsr_group_attach with world > 1 refuses them.
+const char *single_context_feature(const gsr_ctx *c, bool for_group_export) {
+    if (!for_group_export && c->depth_out) return "depth compositing is on";
+    if (!for_group_export && c->inst.n) return "instances are set";
+    if (reduced_sh(c)) return "SH stored as binary16, or stored or rendered below degree 3";
+    if (c->aa_variance > 0.0f) return "anti-aliasing is on";
+    if (view_depth_order(c)) return "depth order is on";
+    if (cutouts_on(c)) return "cutouts are set";
+    return nullptr;
+}
+
+// Whether the context is sharded: an attached shard group, exported or imported peer framebuffers, row interleave, or a band short of
+// the full frame (there is no band before gsr_resize).
+bool sharded(const gsr_ctx *c) {
+    const bool partial = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
+    return c->grp.world > 1 || c->peer_mode || c->row_mod > 1 || partial;
+}
+
+constexpr char SINGLE_CONTEXT_ONLY[] = "single-context only (no group, peer framebuffers, partial band or row interleave)";
+
 // The depth-order buffers at the current capacity: the depth words (3 * cap_stride), GSR_BUF_DEPTH_WORDS_UNSORTED while unsorted pairs
 // are kept, and the sorter's depth-order workspace.  On failure nothing is left half allocated.
 int alloc_depth_order(gsr_ctx *c) {
@@ -577,12 +602,8 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
 
 GSR_API int gsr_set_row_interleave(gsr_ctx *c, int32_t row_rem, int32_t row_mod) {
     if (!c || row_mod < 1 || row_rem < 0 || row_rem >= row_mod) { set_last_error("gsr_set_row_interleave: need 0 <= rem < mod"); return GSR_ERR_INVALID; }
-    if (c->depth_out && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (c->inst.n && row_mod > 1) { set_last_error("gsr_set_row_interleave: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
-    if (c->aa_variance > 0.0f && row_mod > 1) { set_last_error("gsr_set_row_interleave: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (view_depth_order(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: depth order is on (single-context only)"); return GSR_ERR_STATE; }
-    if (cutouts_on(c) && row_mod > 1) { set_last_error("gsr_set_row_interleave: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
+    const char *why = row_mod > 1 ? single_context_feature(c, false) : nullptr;
+    if (why) { set_last_error("gsr_set_row_interleave: %s (single-context only)", why); return GSR_ERR_STATE; }
     c->row_mod = row_mod; c->row_rem = row_rem;
     return GSR_OK;
 }
@@ -602,14 +623,11 @@ GSR_API int gsr_band_fixup(gsr_ctx *c) {
 GSR_API int gsr_set_band(gsr_ctx *c, int32_t row_begin, int32_t row_end) {
     if (!c || c->tiles_y == 0) { set_last_error("gsr_set_band before gsr_resize"); return GSR_ERR_STATE; }
     if (row_begin < 0 || row_end > c->tiles_y || row_begin > row_end) { set_last_error("band [%d,%d) outside [0,%d]", row_begin, row_end, c->tiles_y); return GSR_ERR_INVALID; }
-    if (c->depth_out && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (c->inst.n && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
-    if (c->aa_variance > 0.0f && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (view_depth_order(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: depth order is on (single-context only)"); return GSR_ERR_STATE; }
-    if (cutouts_on(c) && !(row_begin == 0 && row_end == c->tiles_y)) { set_last_error("gsr_set_band: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
+    const bool partial = !(row_begin == 0 && row_end == c->tiles_y);
+    const char *why = partial ? single_context_feature(c, false) : nullptr;
+    if (why) { set_last_error("gsr_set_band: %s (single-context only)", why); return GSR_ERR_STATE; }
     c->band_y0 = row_begin; c->band_y1 = row_end;
-    c->band_set = !(row_begin == 0 && row_end == c->tiles_y);
+    c->band_set = partial;
     return GSR_OK;
 }
 
@@ -720,14 +738,10 @@ static GroupPeers group_peers(const gsr_ctx *c, int parity) {
 }
 
 // GSR_FLAG_ORTHOGRAPHIC: whether the frame takes the orthographic projection path (its projection's w row is exactly (0, 0, 0, 1)), and
-// GSR_ERR_STATE when it does on a context that is not single-context (checked before anything of the frame is enqueued).
+// GSR_ERR_STATE when it does on a sharded context (checked before anything of the frame is enqueued).
 static int frame_is_orthographic(const gsr_ctx *c, const float *view_proj, bool *ortho) {
     *ortho = (c->flags & GSR_FLAG_ORTHOGRAPHIC) && view_proj[19] == 0.0f && view_proj[23] == 0.0f && view_proj[27] == 0.0f && view_proj[31] == 1.0f;
-    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
-    if (*ortho && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
-        set_last_error("orthographic frame: single-context only (no group, peer framebuffers, partial band or row interleave)");
-        return GSR_ERR_STATE;
-    }
+    if (*ortho && sharded(c)) { set_last_error("orthographic frame: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
     return GSR_OK;
 }
 
@@ -769,12 +783,13 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
 
     // ---- front: rasterizer.gd:127-128 (clear M = this frame's history slot + the scan links), then the projection ----
     if (overlap && c->front_gate) GSR_CUDA_TRY(cudaStreamWaitEvent(fs, c->front_gate, 0));
-    const bool inst = c->inst.n > 0 && !gf;   // (a context with instances cannot attach a group)
+    // A group frame (gf) has none of the single-context features read below: single_context_feature() and sharded() keep them apart.
+    const bool inst = c->inst.n > 0;
     // motion vectors (gsr_set_motion_vectors, read here: frames already enqueued keep their plane): the previous state of this frame
-    const bool motion = c->motion_out && c->depth_out && !gf;
+    const bool motion = c->motion_out && c->depth_out;
     const gsr_ctx::MotionState &prev = same_frame ? c->mot_used : c->mot_last;
     // splat IDs (gsr_set_splat_ids), read here as well
-    const bool ids = c->ids_out && c->depth_out && !gf;
+    const bool ids = c->ids_out && c->depth_out;
     {
         uint32_t links = projection_num_blocks((uint32_t)(inst ? c->inst.drawn : c->max_splats));
         if (gf) {
@@ -846,15 +861,14 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     pa.aa_variance = c->aa_variance;   // read here: frames already enqueued keep their filter
     const bool aa = c->aa_variance > 0.0f;
     // gsr_set_depth_order, read here like the filter: the projection stores every pair's depth word beside its key, and the sort orders
-    // the pairs by (tile, depth word) instead of by the key (a group frame cannot occur: the mode refuses groups)
+    // the pairs by (tile, depth word) instead of by the key
     uint32_t *depth_in = nullptr, *depth_alt = nullptr;
-    if (view_depth_order(c) && !gf) {
+    if (view_depth_order(c)) {
         depth_in = c->depth_words + (size_t)half * c->cap_stride;
         depth_alt = c->depth_words + 2ull * c->cap_stride;
     }
-    // gsr_set_cutouts, read here too: the set is copied into the projection's launch parameters (a group frame cannot occur: a set
-    // refuses groups)
-    const CutoutArgs *cut = cutouts_on(c) && !gf ? &c->cutouts : nullptr;
+    // gsr_set_cutouts, read here too: the set is copied into the projection's launch parameters
+    const CutoutArgs *cut = cutouts_on(c) ? &c->cutouts : nullptr;
     if (gf) {
         // group mode: the projection is sharded by SPLATS.  This rank projects its slice and stores every pair and record into the
         // memory of the rank that owns it (peer stores over NVLink); the back part then waits for the other sources' flags and packs
@@ -1199,12 +1213,8 @@ GSR_API int gsr_readback_rows_async(gsr_ctx *c, void *host_frame) {
 
 GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
-    if (c->depth_out) { set_last_error("gsr_peer_export_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (c->inst.n) { set_last_error("gsr_peer_export_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c)) { set_last_error("gsr_peer_export_framebuffers: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
-    if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_export_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (view_depth_order(c)) { set_last_error("gsr_peer_export_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
-    if (cutouts_on(c)) { set_last_error("gsr_peer_export_framebuffers: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
+    const char *why = single_context_feature(c, false);
+    if (why) { set_last_error("gsr_peer_export_framebuffers: %s (single-context only)", why); return GSR_ERR_STATE; }
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_peer_export_framebuffers: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
@@ -1219,12 +1229,8 @@ GSR_API int gsr_peer_export_framebuffers(gsr_ctx *c, void *handles128) {
 
 GSR_API int gsr_peer_import_framebuffers(gsr_ctx *c, const void *handles128) {
     if (!c || !handles128) return GSR_ERR_INVALID;
-    if (c->depth_out) { set_last_error("gsr_peer_import_framebuffers: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (c->inst.n) { set_last_error("gsr_peer_import_framebuffers: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c)) { set_last_error("gsr_peer_import_framebuffers: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
-    if (c->aa_variance > 0.0f) { set_last_error("gsr_peer_import_framebuffers: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (view_depth_order(c)) { set_last_error("gsr_peer_import_framebuffers: depth order is on (single-context only)"); return GSR_ERR_STATE; }
-    if (cutouts_on(c)) { set_last_error("gsr_peer_import_framebuffers: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
+    const char *why = single_context_feature(c, false);
+    if (why) { set_last_error("gsr_peer_import_framebuffers: %s (single-context only)", why); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     cudaIpcMemHandle_t h[2];
@@ -1254,10 +1260,8 @@ constexpr uint32_t GROUP_MAGIC = 0x47535247u;  // "GRSG"
 GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
     if (!c || !blob) return GSR_ERR_INVALID;
     if (!c->fb || !c->fb2 || c->fb_ext) { set_last_error("gsr_group_export: call gsr_resize first (library-owned frames only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c)) { set_last_error("gsr_group_export: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
-    if (c->aa_variance > 0.0f) { set_last_error("gsr_group_export: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (view_depth_order(c)) { set_last_error("gsr_group_export: depth order is on (single-context only)"); return GSR_ERR_STATE; }
-    if (cutouts_on(c)) { set_last_error("gsr_group_export: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
+    const char *why = single_context_feature(c, true);
+    if (why) { set_last_error("gsr_group_export: %s (single-context only)", why); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     if (!c->grp.arena) {
@@ -1286,12 +1290,8 @@ GSR_API int gsr_group_export(gsr_ctx *c, void *blob) {
 GSR_API int gsr_group_attach(gsr_ctx *c, int32_t rank, int32_t world, const void *blobs) {
     if (!c || !blobs || world < 1 || world > GROUP_MAX || rank < 0 || rank >= world) { set_last_error("gsr_group_attach: need 0 <= rank < world <= %d", GROUP_MAX); return GSR_ERR_INVALID; }
     if (!c->grp.arena || !c->fb) { set_last_error("gsr_group_attach before gsr_group_export"); return GSR_ERR_STATE; }
-    if (c->depth_out && world > 1) { set_last_error("gsr_group_attach: depth compositing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (c->inst.n && world > 1) { set_last_error("gsr_group_attach: instances are set (single-context only)"); return GSR_ERR_STATE; }
-    if (reduced_sh(c) && world > 1) { set_last_error("gsr_group_attach: SH stored as binary16, or stored or rendered below degree 3 (single-context only)"); return GSR_ERR_STATE; }
-    if (c->aa_variance > 0.0f && world > 1) { set_last_error("gsr_group_attach: anti-aliasing is on (single-context only)"); return GSR_ERR_STATE; }
-    if (view_depth_order(c) && world > 1) { set_last_error("gsr_group_attach: depth order is on (single-context only)"); return GSR_ERR_STATE; }
-    if (cutouts_on(c) && world > 1) { set_last_error("gsr_group_attach: cutouts are set (single-context only)"); return GSR_ERR_STATE; }
+    const char *why = world > 1 ? single_context_feature(c, false) : nullptr;
+    if (why) { set_last_error("gsr_group_attach: %s (single-context only)", why); return GSR_ERR_STATE; }
     int rc = use_device(c->device);
     if (rc) return rc;
     group_detach(c);
@@ -1405,10 +1405,7 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_devic
         return GSR_OK;
     }
     if (c->width == 0) { set_last_error("gsr_set_depth_compositing before gsr_resize"); return GSR_ERR_STATE; }
-    if (c->grp.world > 1 || c->peer_mode || c->row_mod > 1 || !(c->band_y0 == 0 && c->band_y1 == c->tiles_y)) {
-        set_last_error("gsr_set_depth_compositing: single-context only (no group, peer framebuffers, partial band or row interleave)");
-        return GSR_ERR_STATE;
-    }
+    if (sharded(c)) { set_last_error("gsr_set_depth_compositing: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
     c->scene_depth = scene_depth_device; c->depth_out = depth_out_device;
     return GSR_OK;
 }
@@ -1542,10 +1539,7 @@ GSR_API int gsr_set_instances(gsr_ctx *c, const gsr_instance *instances, uint32_
     }
     if (!instances) { set_last_error("gsr_set_instances: NULL array with n = %u", n); return GSR_ERR_INVALID; }
     if (n > GSR_MAX_INSTANCES) { set_last_error("gsr_set_instances: %u instances exceed GSR_MAX_INSTANCES (%d)", n, GSR_MAX_INSTANCES); return GSR_ERR_INVALID; }
-    if (c->grp.world > 1 || c->peer_mode || c->row_mod > 1 || !(c->band_y0 == 0 && c->band_y1 == c->tiles_y)) {
-        set_last_error("gsr_set_instances: single-context only (no group, peer framebuffers, partial band or row interleave)");
-        return GSR_ERR_STATE;
-    }
+    if (sharded(c)) { set_last_error("gsr_set_instances: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
     float *xf = new (std::nothrow) float[(size_t)INSTANCE_XFORM_FLOATS * n];
     uint64_t *range = new (std::nothrow) uint64_t[2ull * n];
     if (!xf || !range) { delete[] xf; delete[] range; return GSR_ERR_OOM; }
@@ -1627,11 +1621,7 @@ GSR_API int gsr_set_sh_degree(gsr_ctx *c, int32_t degree) {
         set_last_error("gsr_set_sh_degree: degree %d outside -1..%d (the stored degree)", degree, c->sh_bands - 1);
         return GSR_ERR_INVALID;
     }
-    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
-    if (degree >= 0 && degree < SH_BANDS_MAX - 1 && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
-        set_last_error("gsr_set_sh_degree: single-context only below degree 3 (no group, peer framebuffers, partial band or row interleave)");
-        return GSR_ERR_STATE;
-    }
+    if (degree >= 0 && degree < SH_BANDS_MAX - 1 && sharded(c)) { set_last_error("gsr_set_sh_degree: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
     c->sh_degree = degree;   // read by the next render_enqueue: frames already enqueued keep their degree
     return GSR_OK;
 }
@@ -1642,11 +1632,7 @@ GSR_API int gsr_set_antialiasing(gsr_ctx *c, float filter_variance) {
         set_last_error("gsr_set_antialiasing: filter variance %g outside 0..64 px^2", (double)filter_variance);
         return GSR_ERR_INVALID;
     }
-    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
-    if (filter_variance > 0.0f && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
-        set_last_error("gsr_set_antialiasing: single-context only (no group, peer framebuffers, partial band or row interleave)");
-        return GSR_ERR_STATE;
-    }
+    if (filter_variance > 0.0f && sharded(c)) { set_last_error("gsr_set_antialiasing: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
     c->aa_variance = filter_variance;   // read by the next render_enqueue: frames already enqueued keep their filter
     return GSR_OK;
 }
@@ -1658,11 +1644,7 @@ GSR_API int gsr_set_depth_order(gsr_ctx *c, int32_t mode) {
         return GSR_ERR_INVALID;
     }
     if (mode == GSR_DEPTH_ORDER_VIEW_DEPTH) {
-        const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
-        if (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1) {
-            set_last_error("gsr_set_depth_order: single-context only (no group, peer framebuffers, partial band or row interleave)");
-            return GSR_ERR_STATE;
-        }
+        if (sharded(c)) { set_last_error("gsr_set_depth_order: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
         int rc = use_device(c->device);
         if (rc) return rc;
         if ((rc = alloc_depth_order(c))) return rc;   // the first switch only (cudaMalloc may synchronise)
@@ -1684,11 +1666,7 @@ GSR_API int gsr_set_cutouts(gsr_ctx *c, const gsr_cutout *cutouts, uint32_t n) {
         if (v.action != GSR_CUTOUT_KEEP && v.action != GSR_CUTOUT_REMOVE) { set_last_error("gsr_set_cutouts: volume %u: unknown action %d", i, v.action); return GSR_ERR_INVALID; }
         if (v.space != GSR_CUTOUT_FRAME && v.space != GSR_CUTOUT_SOURCE) { set_last_error("gsr_set_cutouts: volume %u: unknown space %d", i, v.space); return GSR_ERR_INVALID; }
     }
-    const bool partial_band = c->tiles_y != 0 && !(c->band_y0 == 0 && c->band_y1 == c->tiles_y);
-    if (n > 0 && (c->grp.world > 1 || c->peer_mode || c->peer_opened || partial_band || c->row_mod > 1)) {
-        set_last_error("gsr_set_cutouts: single-context only (no group, peer framebuffers, partial band or row interleave)");
-        return GSR_ERR_STATE;
-    }
+    if (n > 0 && sharded(c)) { set_last_error("gsr_set_cutouts: %s", SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
     // split by action, KEEP volumes first (the rule does not depend on the order): the kernel runs one loop over each list
     CutoutArgs s = {};
     for (int pass = 0; pass < 2; ++pass) {

@@ -64,8 +64,8 @@ enum {
                                       (far - near) / 65536: set near / far around the content.  Every other frame (perspective and
                                       frustum matrices, anything the reference's packing produces: it writes (0, 0, -1, 0)) takes the
                                       perspective path unchanged.  The choice is made per frame when it is enqueued, without a sync.
-                                      Single-context only: an orthographic frame on a context with a shard group, peer framebuffers, a
-                                      partial band or row interleave returns GSR_ERR_STATE and enqueues nothing. */
+                                      A single-context feature (see "Single-context features"): an orthographic frame on a sharded
+                                      context returns GSR_ERR_STATE and enqueues nothing. */
 
 #define GSR_FLAG_SH_HALF 0x40u /* store the SH coefficients of the gsr_config.sh_bands bands as IEEE binary16 (no reference counterpart):
                                    a degree-3 splat takes 144 instead of 240 bytes.  Planes 0-2 (position / time, covariance, opacity)
@@ -77,9 +77,8 @@ enum {
                                    8 halves (slot 0 = the low half of the plane's first 32-bit word), slots past 3K are +0.  Every frame
                                    is bit for bit the frame of the same context without the flag holding the cloud whose coefficients
                                    are float(h(c)), with every frame feature and every rendered degree (gsr_set_sh_degree reads the
-                                   first ceil(3 (d+1)^2 / 8) half planes).  Fixed at creation.  Single-context only, like a reduced
-                                   store: gsr_group_export, gsr_group_attach with world > 1, gsr_peer_*, a partial gsr_set_band and
-                                   gsr_set_row_interleave with row_mod > 1 return GSR_ERR_STATE (DESIGN.md section 5.14). */
+                                   first ceil(3 (d+1)^2 / 8) half planes).  Fixed at creation.  A single-context feature, like a
+                                   reduced store (see "Single-context features"; DESIGN.md section 5.14). */
 
 /* ---- gsr_debug_copy selectors (parity taps; not on the frame path) ---- */
 enum {
@@ -112,8 +111,8 @@ typedef struct gsr_config {
     uint32_t dup_capacity_factor; /* initial sort capacity = factor * max_splats; 0 -> 10 (rasterizer.gd:79); grows on demand */
     uint32_t sh_bands;            /* SH bands the context stores = SH degree + 1: 1 (DC only) .. 4 (degree 3); 0 -> 4.  The splat buffer holds
                                      3 + P float4 planes per splat, P = ceil(3 B^2 / 4) = 1, 3, 7, 12: 64 / 96 / 160 / 240 bytes.  Uploads drop
-                                     the coefficients the store does not keep.  > 4: GSR_ERR_INVALID.  A store of fewer than 4 bands is
-                                     single-context only (see gsr_set_sh_degree). */
+                                     the coefficients the store does not keep.  > 4: GSR_ERR_INVALID.  A store of fewer than 4 bands is a
+                                     single-context feature (see "Single-context features"). */
 } gsr_config;
 
 typedef struct gsr_stats {
@@ -215,6 +214,29 @@ GSR_API int gsr_band_fixup(gsr_ctx *ctx);
 GSR_API int gsr_peer_export_framebuffers(gsr_ctx *ctx, void *handles128);
 GSR_API int gsr_peer_import_framebuffers(gsr_ctx *ctx, const void *handles128);
 
+/* ---- Single-context features: frame features that work only on a context that renders the whole frame by itself.
+ *        - depth compositing (gsr_set_depth_compositing), with its companions motion vectors and splat IDs;
+ *        - instances (gsr_set_instances with n > 0);
+ *        - a store of fewer than 4 SH bands (gsr_config.sh_bands), a binary16 store (GSR_FLAG_SH_HALF), and a rendered SH degree
+ *          below 3 (gsr_set_sh_degree 0..2);
+ *        - anti-aliasing (gsr_set_antialiasing > 0);
+ *        - view-depth order (gsr_set_depth_order GSR_DEPTH_ORDER_VIEW_DEPTH);
+ *        - cutouts (gsr_set_cutouts with n > 0);
+ *        - orthographic frames (GSR_FLAG_ORTHOGRAPHIC; the flag alone is no feature, each orthographic frame is).
+ *      A context is sharded while any of these holds:
+ *        - a shard group is attached (gsr_group_attach with world > 1);
+ *        - it exported or imported peer framebuffers (gsr_peer_export_framebuffers / gsr_peer_import_framebuffers);
+ *        - its band is not the full frame (gsr_set_band other than (0, tiles_y));
+ *        - row_mod > 1 (gsr_set_row_interleave).
+ *      gsr_resize detaches the group and drops the peer framebuffers.  The rule holds in both directions, with GSR_ERR_STATE and
+ *      the context left as it was:
+ *        - on a sharded context, every call that would turn a feature on is refused, and an orthographic frame enqueues nothing;
+ *        - while a feature is on, every call that would shard the context is refused: gsr_set_band with a partial band,
+ *          gsr_set_row_interleave with row_mod > 1, gsr_group_attach with world > 1, and both gsr_peer_* calls.
+ *      The calls that turn a feature off, gsr_set_band(0, tiles_y) and gsr_set_row_interleave(0, 1) are never refused by the rule.
+ *      gsr_group_export is refused as well while a feature is on, except for depth compositing and instances: a context with
+ *      those may export, but not attach with world > 1. ---- */
+
 /* ---- rasterize() (rasterizer.gd:122-160).
  *      view_proj: the 128-byte push constant of update_camera_matrices (rasterizer.gd:181-193):
  *                 view_matrix then projection_matrix, GLSL column-major.
@@ -312,8 +334,7 @@ GSR_API int gsr_set_framebuffer_external(gsr_ctx *ctx, void *device_ptr);
  *      and depth_out the coverage-weighted linear view depth of the blended splats, +inf where nothing was blended.
  *      depth_out is written by every frame's compositor on the render stream; the caller orders its reads like those of an
  *      external framebuffer.  GSR_OUT_RGB32F drops the coverage; GSR_OUT_SRGB_TO_LINEAR converts the premultiplied values as
- *      they are.  Single-context only: GSR_ERR_STATE on a context with an attached group, peer framebuffers, a partial band
- *      or row_mod > 1, and those calls fail with GSR_ERR_STATE while the mode is on.  gsr_resize switches the mode off;
+ *      they are.  A single-context feature (see "Single-context features").  gsr_resize switches the mode off;
  *      gsr_pick keeps the default path (and leaves the depth-composited frame as it is).  GSR_ERR_STATE before gsr_resize. ---- */
 GSR_API int gsr_set_depth_compositing(gsr_ctx *ctx, const float *scene_depth_device, float *depth_out_device);
 
@@ -391,9 +412,8 @@ GSR_API int gsr_set_splat_ids(gsr_ctx *ctx, uint32_t *ids_out_device);
  *      GSR_INSTANCE_RING frames ahead of the GPU waits for a slot).  Any other call re-lays out the drawn ids: it synchronises and may
  *      reallocate (record tables for max(max_splats, D) ids; the sort capacity is raised to factor * D when D > max_splats).
  *      n == 0 switches instancing off: the default frame.  GSR_ERR_INVALID, previous state kept: n > GSR_MAX_INSTANCES, a range beyond
- *      max_splats, a non-finite entry, a singular A, D >= 2^32 - 256.  Single-context only: GSR_ERR_STATE with an attached group, peer
- *      framebuffers, a partial band or row_mod > 1, and those calls fail with GSR_ERR_STATE while instances are set.  gsr_resize
- *      keeps the instances. ---- */
+ *      max_splats, a non-finite entry, a singular A, D >= 2^32 - 256.  A single-context feature (see "Single-context features").
+ *      gsr_resize keeps the instances. ---- */
 #define GSR_MAX_INSTANCES 4096
 #define GSR_INSTANCE_RING 8
 typedef struct gsr_instance {
@@ -433,9 +453,8 @@ GSR_API int gsr_set_instance_appearance(gsr_ctx *ctx, const gsr_instance_appeara
  *      SH planes, so a lower degree also reads fewer bytes.  -1 = the stored degree (gsr_config.sh_bands - 1), the default.  The degree
  *      is read when a frame is enqueued: frames already enqueued keep theirs, and the call never synchronises.  A frame drawn at
  *      degree d is bit for bit the frame of the same cloud with every coefficient above degree d set to zero (DESIGN.md section 5.9).
- *      GSR_ERR_INVALID: a degree below -1 or above the stored one.  A degree below 3, like a store of fewer than 4 bands, is
- *      single-context only: GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those calls
- *      (and gsr_group_export) fail with GSR_ERR_STATE on such a store or while a degree below 3 is set. ---- */
+ *      GSR_ERR_INVALID: a degree below -1 or above the stored one.  A degree below 3, like a store of fewer than 4 bands, is a
+ *      single-context feature (see "Single-context features"). ---- */
 GSR_API int gsr_set_sh_degree(gsr_ctx *ctx, int32_t degree);
 
 /* ---- Anti-aliased trainings (no reference counterpart: the reference dilates the 2D covariance by a fixed 0.3 px^2 and keeps the
@@ -448,9 +467,8 @@ GSR_API int gsr_set_sh_degree(gsr_ctx *ctx, int32_t degree);
  *      opacity also sets the splat's radius.  0.3 = 3DGS --antialiasing / gsplat "antialiased"; 0.1 = Mip-Splatting's 2D filter.
  *      The value is read when a frame is enqueued: frames already enqueued keep theirs, and the call never synchronises.  Back at 0
  *      the frame is bit for bit that of a context that never used the filter.  gsr_resize keeps the setting.  GSR_ERR_INVALID,
- *      previous state kept: a negative, NaN or infinite variance, or one above 64.  Single-context only: turning the filter on returns
- *      GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those calls (and gsr_group_export)
- *      fail with GSR_ERR_STATE while it is on. ---- */
+ *      previous state kept: a negative, NaN or infinite variance, or one above 64.  A single-context feature while the filter is on
+ *      (see "Single-context features"). ---- */
 GSR_API int gsr_set_antialiasing(gsr_ctx *ctx, float filter_variance);
 
 /* ---- Order splats by exact view depth (no reference counterpart: the reference sorts each frame's pairs by tile << 16 | a 16-bit
@@ -468,8 +486,7 @@ GSR_API int gsr_set_antialiasing(gsr_ctx *ctx, float filter_variance);
  *      twice the sort's traffic; DESIGN.md section 5.12).  The first switch to mode 1 allocates 12 bytes per pair of capacity (and may
  *      synchronise once: GSR_ERR_OOM keeps the previous state); later switches never synchronise.  The mode is read when a frame is
  *      enqueued: frames already enqueued keep theirs, and gsr_resize keeps the setting.  GSR_ERR_INVALID: any other mode.
- *      Single-context only: switching mode 1 on returns GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or
- *      row_mod > 1, and those calls (and gsr_group_export) fail with GSR_ERR_STATE while it is on. ---- */
+ *      Mode 1 is a single-context feature (see "Single-context features"). ---- */
 #define GSR_DEPTH_ORDER_KEY16 0
 #define GSR_DEPTH_ORDER_VIEW_DEPTH 1
 GSR_API int gsr_set_depth_order(gsr_ctx *ctx, int32_t mode);
@@ -494,9 +511,8 @@ GSR_API int gsr_set_depth_order(gsr_ctx *ctx, int32_t mode);
  *      The array is copied and read when a frame is enqueued: frames already enqueued keep their set.  The call never synchronises,
  *      allocates nothing and copies nothing to the device (the set travels with the projection's launch parameters).  n == 0 switches
  *      cutouts off: the default frame, bit for bit.  gsr_resize keeps the set.  GSR_ERR_INVALID, previous set kept: n >
- *      GSR_MAX_CUTOUTS, cutouts == NULL with n > 0, a non-finite to_local entry, an unknown shape, action or space.  Single-context
- *      only: a non-empty set returns GSR_ERR_STATE with an attached group, peer framebuffers, a partial band or row_mod > 1, and those
- *      calls (and gsr_group_export) fail with GSR_ERR_STATE while a set is active. ---- */
+ *      GSR_MAX_CUTOUTS, cutouts == NULL with n > 0, a non-finite to_local entry, an unknown shape, action or space.  A non-empty set
+ *      is a single-context feature (see "Single-context features"). ---- */
 #define GSR_MAX_CUTOUTS 16
 #define GSR_CUTOUT_BOX 0        /* inside: |u0| <= 1 && |u1| <= 1 && |u2| <= 1 */
 #define GSR_CUTOUT_ELLIPSOID 1  /* inside: ((u0*u0 + u1*u1) + u2*u2) <= 1 */
