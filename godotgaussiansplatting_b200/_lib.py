@@ -27,6 +27,8 @@ GSR_MAX_INSTANCES, GSR_INSTANCE_RING = 4096, 8
 GSR_TINT_MAX = 16.0
 GSR_DRAW_ALL = 0xFFFFFFFFFFFFFFFF   # gsr_instance_appearance.draw_count: every splat of the range
 GSR_NO_ID = 0xFFFFFFFF              # gsr_set_splat_ids: no splat / no instance
+GSR_MAX_SELECT_VERTICES = 64
+GSR_SELECT_SET, GSR_SELECT_ADD, GSR_SELECT_SUBTRACT, GSR_SELECT_TOGGLE = range(4)
 
 # every symbol include/gsr.h declares (tests/test_abi.py checks the header against this list and the .so)
 EXPORTS = [
@@ -34,6 +36,8 @@ EXPORTS = [
     "gsr_render_async", "gsr_render_async_rgb", "gsr_render_async_fmt", "gsr_output_bytes", "gsr_present_device", "gsr_readback_async", "gsr_peer_export_framebuffers", "gsr_peer_import_framebuffers",
     "gsr_stream_join", "gsr_group_export", "gsr_group_attach", "gsr_group_detach", "gsr_group_set_present", "gsr_readback_rows_async", "gsr_sync", "gsr_framebuffer_device_ptr", "gsr_set_framebuffer_external",
     "gsr_set_depth_compositing", "gsr_set_motion_vectors", "gsr_reset_motion", "gsr_set_splat_ids", "gsr_set_instances", "gsr_set_instance_appearance", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_set_cutouts", "gsr_upload_ply_filtered", "gsr_pick",
+    "gsr_select_all", "gsr_select_polygon", "gsr_select_volume", "gsr_select_ids", "gsr_hide_selection", "gsr_unhide_all", "gsr_clear_splat_masks",
+    "gsr_get_splat_masks", "gsr_set_splat_masks", "gsr_splat_mask_counts", "gsr_set_selection_style",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -142,6 +146,18 @@ def lib():
         L.gsr_set_depth_order.argtypes = [vp, C.c_int32]
         L.gsr_set_cutouts.argtypes = [vp, C.POINTER(GsrCutout), u32]
         L.gsr_pick.argtypes = [vp, u32, C.c_float, fp]
+        u32p, u64 = C.POINTER(C.c_uint32), C.c_uint64
+        L.gsr_select_all.argtypes = [vp, C.c_int32]
+        L.gsr_select_polygon.argtypes = [vp, fp, C.c_float, C.c_int32, fp, u32, C.c_int32]
+        L.gsr_select_volume.argtypes = [vp, C.POINTER(GsrCutout), C.c_float, C.c_int32, C.c_int32]
+        L.gsr_select_ids.argtypes = [vp, vp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]
+        L.gsr_hide_selection.argtypes = [vp]
+        L.gsr_unhide_all.argtypes = [vp]
+        L.gsr_clear_splat_masks.argtypes = [vp]
+        L.gsr_get_splat_masks.argtypes = [vp, u32p, u32p, u64]
+        L.gsr_set_splat_masks.argtypes = [vp, u32p, u32p, u64]
+        L.gsr_splat_mask_counts.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
+        L.gsr_set_selection_style.argtypes = [vp, fp, C.c_float]
         L.gsr_get_stats.argtypes = [vp, C.POINTER(GsrStats)]
         L.gsr_get_frame_history.argtypes = [vp, u32, C.POINTER(GsrFrameRecord), C.POINTER(u32)]
         L.gsr_debug_copy.argtypes = [vp, C.c_int, vp, C.c_size_t]

@@ -229,12 +229,13 @@ static_assert(sizeof(ProjectionArgs) == 288 && offsetof(ProjectionArgs, lookback
 // aa: the frame is anti-aliased with a.aa_variance > 0 (gsr_set_antialiasing; read at enqueue time, single-context only)
 // depth_words: non-null = the frame is sorted by view depth (gsr_set_depth_order; single-context only): the projection also stores
 // depth_words[g] = depth_order_word(d) beside keys[g] / values[g], d the pair's splat's view depth
-// cutouts: non-null = the frame draws only the splats the set keeps (gsr_set_cutouts; single-context only); the set is copied into the
-// launch's parameters
-struct CutoutArgs;
+// cut: non-null = the frame takes the CUT = true kernels: it draws only the splats the cutout set keeps (gsr_set_cutouts) and, with the
+// splat masks in use (gsr_select_*), drops hidden splats and highlights selected ones (single-context only); copied into the launch's
+// parameters
+struct CutParams;
 // sh_half: the store holds binary16 SH planes (GSR_FLAG_SH_HALF; single-context only)
 int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false, bool aa = false,
-                      uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr, bool sh_half = false);
+                      uint32_t *depth_words = nullptr, const CutParams *cut = nullptr, bool sh_half = false);
 
 // gsr_set_cutouts: the active set, split by action on the host so that the kernel runs one loop over the KEEP volumes and one over the
 // REMOVE volumes (vol[0, n_keep) then vol[n_keep, n_keep + n_remove)).  It travels by value as the projection's fourth __grid_constant__
@@ -248,6 +249,72 @@ struct CutoutArgs {
     CutoutVolume vol[GSR_MAX_CUTOUTS];
 };
 static_assert(sizeof(CutoutVolume) == 52 && sizeof(CutoutArgs) == 840, "CutoutArgs layout");
+
+// gsr_set_cutouts / gsr_select_volume: is the tested position inside the unit box / sphere of volume v?  u = A p + t (one rounding per
+// operation, in the order of include/gsr.h); IEEE comparisons, so a NaN coordinate is outside.  18 FP32 operations.
+__device__ __forceinline__ bool cutout_inside(const CutoutVolume &v, float x, float y, float z) {
+    const float *C = v.m;
+    const float u0 = ((C[0] * x + C[3] * y) + C[6] * z) + C[9];
+    const float u1 = ((C[1] * x + C[4] * y) + C[7] * z) + C[10];
+    const float u2 = ((C[2] * x + C[5] * y) + C[8] * z) + C[11];
+    if (v.kind & 1) return ((u0 * u0 + u1 * u1) + u2 * u2) <= 1.0f;   // GSR_CUTOUT_ELLIPSOID
+    return fabsf(u0) <= 1.0f && fabsf(u1) <= 1.0f && fabsf(u2) <= 1.0f;
+}
+
+// Splat masks (gsr_select_*, gsr_hide_selection): one bit per SOURCE splat, 32 per word, over [0, max_splats).  hidden == nullptr: the
+// masks are not in use.  A hidden splat leaves the projection like a cutout-removed one; a selected one, with `highlight`, has its colour
+// replaced by c * keep + add per channel (an FMUL, then an FADD) after the SH clamp and the instance tint.
+struct SplatMaskArgs {
+    const uint32_t *hidden = nullptr;
+    const uint32_t *selected = nullptr;
+    float keep = 1.0f;              // 1 - strength
+    float add[3] = {0.0f, 0.0f, 0.0f};   // rgb * strength
+    uint32_t highlight = 0u;        // strength > 0
+};
+// The parameter of the CUT = true projection kernels: the cutout set and the splat masks (either may be empty).  It converts from a bare
+// cutout set (no masks).
+struct CutParams {
+    CutoutArgs set;
+    SplatMaskArgs masks;
+    CutParams() = default;
+    __host__ __device__ CutParams(const CutoutArgs &s) : set(s) {}
+};
+__device__ __forceinline__ bool mask_bit(const uint32_t *m, uint64_t s) { return ((m[s >> 5] >> (uint32_t)(s & 31u)) & 1u) != 0u; }
+
+// ---- selection operations (selection.cu) ----
+constexpr int SELECT_MAX_VERTICES = GSR_MAX_SELECT_VERTICES;
+// One region operation: inside(s) for the source splats s of [first, first + count) (every other splat is outside), combined into the
+// selected mask by `op`, then selected &= ~hidden.  Polygon: q of splat s is sp = plane0[s].xyz * model_scale, or A sp + t with
+// `instanced`, and inside = clip3 > 0 and the even-odd test of pix(vp, q) against xy[0, n).  Volume: cutout_inside(vol, sp or q).
+struct SelectArgs {
+    uint32_t *selected;
+    const uint32_t *hidden;
+    uint32_t words, op;
+    uint64_t max_splats, first, count;
+    const float4 *plane0;
+    float model_scale;
+    int32_t instanced;
+    float A[12];
+    float vp[32];
+    float fw, fh;              // (float)(W - 1), (float)(H - 1)
+    CutoutVolume vol;
+    uint32_t n;
+    float2 xy[SELECT_MAX_VERTICES];
+};
+enum SelectKind { SELECT_ALL = 0, SELECT_POLYGON = 1, SELECT_VOLUME = 2 };
+struct InstanceDesc;
+int launch_select_region(const SelectArgs &a, int kind, cudaStream_t stream);
+// "select what you see": every pixel of [x0, x1) x [y0, y1) of an ID plane (gsr_set_splat_ids layout) marks the source splat of its
+// drawn id in `scratch` (zero on entry), then selected = op(selected, scratch) & ~hidden and scratch is zeroed again.  warp_inst ==
+// nullptr: no instances (ids below max_splats are sources); else the layout's `drawn_warps` warps of desc / warp_inst.
+int launch_select_ids(const uint32_t *ids, int32_t width, int32_t x0, int32_t y0, int32_t x1, int32_t y1, const uint32_t *warp_inst,
+                      const InstanceDesc *desc, uint32_t drawn_warps, uint64_t max_splats, uint32_t *scratch, uint32_t *selected,
+                      const uint32_t *hidden, uint32_t words, uint32_t op, cudaStream_t stream);
+// hidden |= selected, selected = 0
+int launch_hide_selection(uint32_t *hidden, uint32_t *selected, uint32_t words, cudaStream_t stream);
+// counts[0] += popcount(selected), counts[1] += popcount(hidden)
+int launch_mask_counts(const uint32_t *selected, const uint32_t *hidden, uint32_t words, unsigned long long *counts, cudaStream_t stream);
+int preload_selection_kernels();
 
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.
@@ -275,7 +342,7 @@ struct InstanceArgs {
 };
 // a.num_splats = D (drawn ids), a.records indexed by drawn id
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands = SH_BANDS_MAX, bool ortho = false,
-                                bool aa = false, uint32_t *depth_words = nullptr, const CutoutArgs *cutouts = nullptr, bool sh_half = false);
+                                bool aa = false, uint32_t *depth_words = nullptr, const CutParams *cut = nullptr, bool sh_half = false);
 // Per instance and frame with motion vectors (gsr_set_motion_vectors): the previous frame's to_frame [A' | t'] (12).
 constexpr int INSTANCE_PREV_FLOATS = 12;
 // one CTA: out[k] = the constants of instance k for the frame's view matrix vp[0..15] and camera_pos cam[0..2]; xf = k x 24 floats

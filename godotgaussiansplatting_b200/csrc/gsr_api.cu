@@ -45,6 +45,17 @@ struct gsr_ctx {
     float aa_variance = 0.0f;    // anti-aliasing filter of the next frames (gsr_set_antialiasing); 0 = off
     int32_t depth_order = GSR_DEPTH_ORDER_KEY16;   // sort order of the next frames (gsr_set_depth_order)
     CutoutArgs cutouts = {};     // cutout set of the next frames (gsr_set_cutouts), KEEP volumes first; none = off
+    // splat masks (gsr_select_*): one device allocation of [hidden | selected | scratch] words, then two 64-bit counters; allocated by
+    // the first call that can set a bit and kept until gsr_destroy.  on == false: not in use (the frames take their usual kernels).
+    struct Masks {
+        bool on = false;
+        uint32_t words = 0;               // ceil(max_splats / 32)
+        uint32_t *hidden = nullptr, *selected = nullptr, *scratch = nullptr;
+        unsigned long long *counts = nullptr;
+        cudaEvent_t ids_ready = nullptr;  // gsr_select_ids with front / back overlap: the render stream's work that wrote the ID plane
+        float rgb[3] = {1.0f, 0.5f, 0.0f};
+        float strength = 0.5f;
+    } masks;
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -258,6 +269,7 @@ const char *single_context_feature(const gsr_ctx *c, bool for_group_export) {
     if (c->aa_variance > 0.0f) return "anti-aliasing is on";
     if (view_depth_order(c)) return "depth order is on";
     if (cutouts_on(c)) return "cutouts are set";
+    if (c->masks.on) return "splat masks are in use";
     return nullptr;
 }
 
@@ -303,6 +315,8 @@ void free_ctx(gsr_ctx *c) {
     cudaFree(c->unsorted_keys); cudaFree(c->unsorted_vals); cudaFree(c->trace); cudaFree(c->trace_count);
     cudaFree(c->depth_words); cudaFree(c->unsorted_depth);
     cudaFree(c->inst.desc); cudaFree(c->inst.warps); cudaFree(c->inst.frame);
+    cudaFree(c->masks.counts);   // the base of the mask allocation
+    if (c->masks.ids_ready) cudaEventDestroy(c->masks.ids_ready);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
     for (int i = 0; i < GSR_INSTANCE_RING; ++i) if (c->inst.ev[i]) cudaEventDestroy(c->inst.ev[i]);
     delete[] c->inst.range; delete[] c->inst.xf; delete[] c->inst.app;
@@ -441,7 +455,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     // load every kernel now: with lazy module loading a FIRST launch may have to synchronise with the device, which must not
     // happen on the frame path (and would deadlock a group whose ranks share one process: a wait kernel spins meanwhile)
     if ((rc = preload_group_kernels()) || (rc = preload_projection_kernels()) || (rc = preload_sort_kernels()) || (rc = preload_ranges_kernels()) ||
-        (rc = preload_ingest_kernels()) || (rc = preload_present_kernels()) || (rc = preload_composite_kernels()) ||
+        (rc = preload_ingest_kernels()) || (rc = preload_present_kernels()) || (rc = preload_composite_kernels()) || (rc = preload_selection_kernels()) ||
         (sh_half(c) && (rc = preload_projection_half_kernels()))) { free_ctx(c); return rc; }
     cudaError_t e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_last_error("init sync -> %s", cudaGetErrorString(e)); free_ctx(c); return GSR_ERR_CUDA; }
@@ -867,8 +881,18 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
         depth_in = c->depth_words + (size_t)half * c->cap_stride;
         depth_alt = c->depth_words + 2ull * c->cap_stride;
     }
-    // gsr_set_cutouts, read here too: the set is copied into the projection's launch parameters
-    const CutoutArgs *cut = cutouts_on(c) ? &c->cutouts : nullptr;
+    // gsr_set_cutouts and the splat masks (gsr_select_*, gsr_set_selection_style), read here too: the set, the mask pointers and the
+    // highlight are copied into the projection's launch parameters
+    CutParams cut_params(c->cutouts);
+    if (c->masks.on) {
+        SplatMaskArgs &m = cut_params.masks;
+        m.hidden = c->masks.hidden; m.selected = c->masks.selected;
+        const volatile float sh = c->masks.strength;   // float32 on the host, once per frame
+        m.keep = 1.0f - sh;
+        for (int i = 0; i < 3; ++i) { const volatile float h = c->masks.rgb[i] * sh; m.add[i] = h; }
+        m.highlight = sh > 0.0f ? 1u : 0u;
+    }
+    const CutParams *cut = (cutouts_on(c) || c->masks.on) ? &cut_params : nullptr;
     if (gf) {
         // group mode: the projection is sharded by SPLATS.  This rank projects its slice and stores every pair and record into the
         // memory of the rank that owns it (peer stores over NVLink); the back part then waits for the other sources' flags and packs
@@ -1681,6 +1705,229 @@ GSR_API int gsr_set_cutouts(gsr_ctx *c, const gsr_cutout *cutouts, uint32_t n) {
         }
     }
     c->cutouts = s;   // read by the next render_enqueue: frames already enqueued keep their set
+    return GSR_OK;
+}
+
+// ---- splat selection (gsr_select_*): the masks live on the device; every operation is enqueued on the projections' stream ----------
+// The stream the projections run on (the front stream with front / back overlap): every mask operation is enqueued there, so it is
+// ordered after the projections of the frames enqueued before it and before those of the frames after it.  The sort and the
+// compositor never read the masks, so an operation does not hold the next frame's projection behind the previous frame's compositor.
+// (gsr_debug_pipeline synchronises both streams, so a switch of the overlap mode never leaves an operation behind.)
+static cudaStream_t mask_stream(const gsr_ctx *c) { return (c->overlap > 0 && c->front_stream) ? c->front_stream : c->stream; }
+
+static bool select_op_valid(int32_t op) { return op >= GSR_SELECT_SET && op <= GSR_SELECT_TOGGLE; }
+
+// The first call that can set a bit puts the masks in use: allocated and zeroed once (GSR_ERR_OOM / GSR_ERR_CUDA keep the state as it
+// was), zeroed again by gsr_clear_splat_masks, so a later first call only switches them on.
+static int masks_use(gsr_ctx *c, const char *where) {
+    if (sharded(c)) { set_last_error("%s: %s", where, SINGLE_CONTEXT_ONLY); return GSR_ERR_STATE; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    gsr_ctx::Masks &m = c->masks;
+    if (!m.hidden) {
+        const uint32_t words = (uint32_t)((c->max_splats + 31ull) / 32ull);
+        const size_t bytes = 2 * sizeof(unsigned long long) + sizeof(uint32_t) * 3ull * words;
+        void *buf = nullptr;
+        cudaEvent_t ev = nullptr;
+        cudaError_t e = cudaMalloc(&buf, bytes);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaMemsetAsync(buf, 0, bytes, mask_stream(c));
+        if (e != cudaSuccess) {
+            cudaFree(buf);
+            if (ev) cudaEventDestroy(ev);
+            set_last_error("%s: splat masks of %llu B -> %s", where, (unsigned long long)bytes, cudaGetErrorString(e));
+            return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+        }
+        m.counts = static_cast<unsigned long long *>(buf);
+        m.hidden = reinterpret_cast<uint32_t *>(m.counts + 2);
+        m.selected = m.hidden + words;
+        m.scratch = m.selected + words;
+        m.words = words;
+        m.ids_ready = ev;
+    }
+    m.on = true;
+    return GSR_OK;
+}
+
+// The tested range and transform of instance `instance` (-1: every splat, no transform)
+static int select_range(const gsr_ctx *c, const char *where, int32_t instance, SelectArgs &a) {
+    if (instance < -1 || instance >= (int32_t)c->inst.n) {
+        set_last_error("%s: instance %d outside the current layout (-1 or 0..%u)", where, instance, c->inst.n ? c->inst.n - 1u : 0u);
+        return GSR_ERR_INVALID;
+    }
+    if (instance < 0) { a.first = 0; a.count = c->max_splats; a.instanced = 0; return GSR_OK; }
+    a.first = c->inst.range[2 * instance]; a.count = c->inst.range[2 * instance + 1]; a.instanced = 1;
+    memcpy(a.A, c->inst.xf + (size_t)instance * INSTANCE_XFORM_FLOATS, sizeof a.A);
+    return GSR_OK;
+}
+
+static int select_region(gsr_ctx *c, const char *where, SelectArgs &a, int kind, int32_t op) {
+    int rc = masks_use(c, where);
+    if (rc) return rc;
+    a.selected = c->masks.selected; a.hidden = c->masks.hidden; a.words = c->masks.words; a.op = (uint32_t)op;
+    a.max_splats = c->max_splats; a.plane0 = c->soa;
+    return launch_select_region(a, kind, mask_stream(c));
+}
+
+GSR_API int gsr_select_all(gsr_ctx *c, int32_t op) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!select_op_valid(op)) { set_last_error("gsr_select_all: unknown op %d", op); return GSR_ERR_INVALID; }
+    SelectArgs a;
+    memset(&a, 0, sizeof a);
+    a.first = 0; a.count = c->max_splats;
+    return select_region(c, "gsr_select_all", a, SELECT_ALL, op);
+}
+
+GSR_API int gsr_select_polygon(gsr_ctx *c, const float view_proj[32], float model_scale, int32_t instance, const float *xy, uint32_t n,
+                               int32_t op) {
+    if (!c || !view_proj || !xy) { set_last_error("gsr_select_polygon: NULL argument"); return GSR_ERR_INVALID; }
+    if (!select_op_valid(op)) { set_last_error("gsr_select_polygon: unknown op %d", op); return GSR_ERR_INVALID; }
+    if (n < 3 || n > GSR_MAX_SELECT_VERTICES) { set_last_error("gsr_select_polygon: %u vertices, need 3..%d", n, GSR_MAX_SELECT_VERTICES); return GSR_ERR_INVALID; }
+    for (uint32_t i = 0; i < 2 * n; ++i) {
+        if (!(fabsf(xy[i]) <= 3.402823466e38f)) { set_last_error("gsr_select_polygon: vertex %u is not finite", i / 2); return GSR_ERR_INVALID; }
+    }
+    if (c->width == 0) { set_last_error("gsr_select_polygon before gsr_resize"); return GSR_ERR_STATE; }
+    SelectArgs a;
+    memset(&a, 0, sizeof a);
+    int rc = select_range(c, "gsr_select_polygon", instance, a);
+    if (rc) return rc;
+    a.model_scale = model_scale;
+    memcpy(a.vp, view_proj, sizeof a.vp);
+    a.fw = (float)(c->width - 1); a.fh = (float)(c->height - 1);
+    a.n = n;
+    for (uint32_t i = 0; i < n; ++i) a.xy[i] = make_float2(xy[2 * i], xy[2 * i + 1]);
+    return select_region(c, "gsr_select_polygon", a, SELECT_POLYGON, op);
+}
+
+GSR_API int gsr_select_volume(gsr_ctx *c, const gsr_cutout *volume, float model_scale, int32_t instance, int32_t op) {
+    if (!c || !volume) { set_last_error("gsr_select_volume: NULL argument"); return GSR_ERR_INVALID; }
+    if (!select_op_valid(op)) { set_last_error("gsr_select_volume: unknown op %d", op); return GSR_ERR_INVALID; }
+    for (int e = 0; e < 12; ++e) {
+        if (!(fabsf(volume->to_local[e]) <= 3.402823466e38f)) { set_last_error("gsr_select_volume: non-finite to_local[%d]", e); return GSR_ERR_INVALID; }
+    }
+    if (volume->shape != GSR_CUTOUT_BOX && volume->shape != GSR_CUTOUT_ELLIPSOID) { set_last_error("gsr_select_volume: unknown shape %d", volume->shape); return GSR_ERR_INVALID; }
+    if (volume->space != GSR_CUTOUT_FRAME && volume->space != GSR_CUTOUT_SOURCE) { set_last_error("gsr_select_volume: unknown space %d", volume->space); return GSR_ERR_INVALID; }
+    SelectArgs a;
+    memset(&a, 0, sizeof a);
+    int rc = select_range(c, "gsr_select_volume", instance, a);
+    if (rc) return rc;
+    a.model_scale = model_scale;
+    memcpy(a.vol.m, volume->to_local, sizeof a.vol.m);
+    a.vol.kind = volume->shape | (volume->space << 1);
+    return select_region(c, "gsr_select_volume", a, SELECT_VOLUME, op);
+}
+
+GSR_API int gsr_select_ids(gsr_ctx *c, const uint32_t *ids_device, int32_t x0, int32_t y0, int32_t x1, int32_t y1, int32_t op) {
+    if (!c || !ids_device) { set_last_error("gsr_select_ids: NULL argument"); return GSR_ERR_INVALID; }
+    if (!select_op_valid(op)) { set_last_error("gsr_select_ids: unknown op %d", op); return GSR_ERR_INVALID; }
+    if (c->width == 0) { set_last_error("gsr_select_ids before gsr_resize"); return GSR_ERR_STATE; }
+    if (x0 < 0 || y0 < 0 || x1 < x0 || y1 < y0 || x1 > c->width || y1 > c->height) {
+        set_last_error("gsr_select_ids: rectangle [%d,%d) x [%d,%d) outside the %dx%d image", x0, x1, y0, y1, c->width, c->height);
+        return GSR_ERR_INVALID;
+    }
+    int rc = masks_use(c, "gsr_select_ids");
+    if (rc) return rc;
+    cudaStream_t ms = mask_stream(c);
+    if (ms != c->stream) {   // the ID plane is written by the compositor of an earlier frame, on the render stream
+        GSR_CUDA_TRY(cudaEventRecord(c->masks.ids_ready, c->stream));
+        GSR_CUDA_TRY(cudaStreamWaitEvent(ms, c->masks.ids_ready, 0));
+    }
+    const bool inst = c->inst.n > 0;
+    if ((rc = launch_select_ids(ids_device, c->width, x0, y0, x1, y1, inst ? c->inst.warps : nullptr, c->inst.desc,
+                                inst ? (uint32_t)(c->inst.drawn / 32ull) : 0u, c->max_splats, c->masks.scratch, c->masks.selected,
+                                c->masks.hidden, c->masks.words, (uint32_t)op, ms))) return rc;
+    return GSR_OK;
+}
+
+GSR_API int gsr_hide_selection(gsr_ctx *c) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!c->masks.on) return GSR_OK;   // nothing is selected
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    return launch_hide_selection(c->masks.hidden, c->masks.selected, c->masks.words, mask_stream(c));
+}
+
+GSR_API int gsr_unhide_all(gsr_ctx *c) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!c->masks.on) return GSR_OK;   // nothing is hidden
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    GSR_CUDA_TRY(cudaMemsetAsync(c->masks.hidden, 0, sizeof(uint32_t) * c->masks.words, mask_stream(c)));
+    return GSR_OK;
+}
+
+GSR_API int gsr_clear_splat_masks(gsr_ctx *c) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!c->masks.on) return GSR_OK;
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    GSR_CUDA_TRY(cudaMemsetAsync(c->masks.hidden, 0, sizeof(uint32_t) * 2ull * c->masks.words, mask_stream(c)));   // hidden | selected
+    c->masks.on = false;
+    return GSR_OK;
+}
+
+static int check_mask_words(const gsr_ctx *c, const char *where, const void *hidden, const void *selected, uint64_t words) {
+    if (!hidden || !selected) { set_last_error("%s: NULL array", where); return GSR_ERR_INVALID; }
+    const uint64_t want = (c->max_splats + 31ull) / 32ull;
+    if (words != want) { set_last_error("%s: %llu words, need ceil(max_splats / 32) = %llu", where, (unsigned long long)words, (unsigned long long)want); return GSR_ERR_INVALID; }
+    return GSR_OK;
+}
+
+GSR_API int gsr_get_splat_masks(gsr_ctx *c, uint32_t *hidden, uint32_t *selected, uint64_t words) {
+    if (!c) return GSR_ERR_INVALID;
+    int rc = check_mask_words(c, "gsr_get_splat_masks", hidden, selected, words);
+    if (rc) return rc;
+    if (!c->masks.on) {
+        memset(hidden, 0, sizeof(uint32_t) * words);
+        memset(selected, 0, sizeof(uint32_t) * words);
+        return GSR_OK;
+    }
+    if ((rc = use_device(c->device))) return rc;
+    cudaStream_t ms = mask_stream(c);
+    GSR_CUDA_TRY(cudaMemcpyAsync(hidden, c->masks.hidden, sizeof(uint32_t) * words, cudaMemcpyDeviceToHost, ms));
+    GSR_CUDA_TRY(cudaMemcpyAsync(selected, c->masks.selected, sizeof(uint32_t) * words, cudaMemcpyDeviceToHost, ms));
+    GSR_CUDA_TRY(cudaStreamSynchronize(ms));
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_splat_masks(gsr_ctx *c, const uint32_t *hidden, const uint32_t *selected, uint64_t words) {
+    if (!c) return GSR_ERR_INVALID;
+    int rc = check_mask_words(c, "gsr_set_splat_masks", hidden, selected, words);
+    if (rc) return rc;
+    const uint32_t tail = (uint32_t)(c->max_splats & 31ull), past = tail ? ~((1u << tail) - 1u) : 0u;   // bits past max_splats
+    for (uint64_t w = 0; w < words; ++w) {
+        if (hidden[w] & selected[w]) { set_last_error("gsr_set_splat_masks: word %llu has splats both hidden and selected", (unsigned long long)w); return GSR_ERR_INVALID; }
+    }
+    if ((hidden[words - 1] | selected[words - 1]) & past) { set_last_error("gsr_set_splat_masks: bits past max_splats"); return GSR_ERR_INVALID; }
+    if ((rc = masks_use(c, "gsr_set_splat_masks"))) return rc;
+    // pageable host memory: each copy has read its source when it returns
+    GSR_CUDA_TRY(cudaMemcpyAsync(c->masks.hidden, hidden, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, mask_stream(c)));
+    GSR_CUDA_TRY(cudaMemcpyAsync(c->masks.selected, selected, sizeof(uint32_t) * words, cudaMemcpyHostToDevice, mask_stream(c)));
+    return GSR_OK;
+}
+
+GSR_API int gsr_splat_mask_counts(gsr_ctx *c, uint64_t *selected, uint64_t *hidden) {
+    if (!c || !selected || !hidden) { set_last_error("gsr_splat_mask_counts: NULL argument"); return GSR_ERR_INVALID; }
+    *selected = 0; *hidden = 0;
+    if (!c->masks.on) return GSR_OK;
+    int rc = use_device(c->device);
+    cudaStream_t ms = mask_stream(c);
+    if (rc || (rc = launch_mask_counts(c->masks.selected, c->masks.hidden, c->masks.words, c->masks.counts, ms))) return rc;
+    unsigned long long n[2] = {0ull, 0ull};
+    GSR_CUDA_TRY(cudaMemcpyAsync(n, c->masks.counts, sizeof n, cudaMemcpyDeviceToHost, ms));
+    GSR_CUDA_TRY(cudaStreamSynchronize(ms));
+    *selected = n[0]; *hidden = n[1];
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_selection_style(gsr_ctx *c, const float rgb[3], float strength) {
+    if (!c || !rgb) { set_last_error("gsr_set_selection_style: NULL argument"); return GSR_ERR_INVALID; }
+    for (int i = 0; i < 3; ++i) {
+        if (!(rgb[i] >= 0.0f && rgb[i] <= GSR_TINT_MAX)) { set_last_error("gsr_set_selection_style: rgb[%d] = %g outside [0, GSR_TINT_MAX]", i, (double)rgb[i]); return GSR_ERR_INVALID; }
+    }
+    if (!(strength >= 0.0f && strength <= 1.0f)) { set_last_error("gsr_set_selection_style: strength %g outside [0, 1]", (double)strength); return GSR_ERR_INVALID; }
+    memcpy(c->masks.rgb, rgb, sizeof c->masks.rgb);
+    c->masks.strength = strength;   // read by the next render_enqueue
     return GSR_OK;
 }
 

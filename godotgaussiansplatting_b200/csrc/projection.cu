@@ -209,19 +209,12 @@ __device__ __forceinline__ void sh_color(const float4 *src, uint64_t stride, flo
     }
 }
 
-// gsr_set_cutouts: is the tested position inside the unit box / sphere of volume v?  u = A p + t (one rounding per operation, in the
-// order of include/gsr.h); IEEE comparisons, so a NaN coordinate is outside.  18 FP32 operations, the volume read with a uniform index.
-__device__ __forceinline__ bool cutout_inside(const CutoutVolume &v, float x, float y, float z) {
-    const float *C = v.m;
-    const float u0 = ((C[0] * x + C[3] * y) + C[6] * z) + C[9];
-    const float u1 = ((C[1] * x + C[4] * y) + C[7] * z) + C[10];
-    const float u2 = ((C[2] * x + C[5] * y) + C[8] * z) + C[11];
-    if (v.kind & 1) return ((u0 * u0 + u1 * u1) + u2 * u2) <= 1.0f;   // GSR_CUTOUT_ELLIPSOID
-    return fabsf(u0) <= 1.0f && fabsf(u1) <= 1.0f && fabsf(u2) <= 1.0f;
-}
 // The rule of gsr_set_cutouts for source position s and frame-space position f: (no KEEP volume, or inside one) and inside no REMOVE
-// volume.  Both loops run over the warp-uniform counts of the host-split set; a lane leaves as soon as its answer is known.
-__device__ __forceinline__ bool cutout_drawn(const CutoutArgs &ct, float s0, float s1, float s2, float f0, float f1, float f2) {
+// volume.  Both loops run over the warp-uniform counts of the host-split set; a lane leaves as soon as its answer is known.  With the
+// splat masks in use (gsr_select_*), source splat `sid` must not be hidden either (tested first: one word that the warp shares).
+__device__ __forceinline__ bool cutout_drawn(const CutParams &cp, uint64_t sid, float s0, float s1, float s2, float f0, float f1, float f2) {
+    if (cp.masks.hidden && mask_bit(cp.masks.hidden, sid)) return false;
+    const CutoutArgs &ct = cp.set;
     bool keep = ct.n_keep == 0u;
 #pragma unroll 1
     for (uint32_t i = 0; i < ct.n_keep && !keep; ++i) {
@@ -239,11 +232,11 @@ __device__ __forceinline__ bool cutout_drawn(const CutoutArgs &ct, float s0, flo
     }
     return true;
 }
-// The cutout parameter of a kernel: the set (CutoutArgs) for CUT = true, an empty placeholder otherwise, so that the kernels without
-// cutouts keep their parameter block as it was.
+// The cutout parameter of a kernel: the set and the splat masks (CutParams) for CUT = true, an empty placeholder otherwise, so that the
+// kernels without cutouts keep their parameter block as it was.
 struct NoCutouts {};
 template <bool CUT> struct CutoutParamT { using type = NoCutouts; };
-template <> struct CutoutParamT<true> { using type = CutoutArgs; };
+template <> struct CutoutParamT<true> { using type = CutParams; };
 template <bool CUT> using CutoutParam = typename CutoutParamT<CUT>::type;
 // The instance parameter of a kernel: InstanceArgs for INSTANCED = true; otherwise a placeholder of the three pointers InstanceArgs
 // used to be, which nothing reads, so that the parameters after it keep their offsets in the kernels without instances.
@@ -278,10 +271,12 @@ struct LaneOut {  // what one splat contributes (valid when n > 0)
 // opacity drives both the radius and the record (DESIGN.md section 5.11).  AA = false is the lane as it always was.
 // CUT (gsr_set_cutouts, the set `ct`): right after the frustum cull, a splat the set removes leaves exactly like a culled one (false,
 // n = 0, last_tile = -1) before any other work.  The frame-space position of an instanced splat is formed there with the record's
-// operations (DESIGN.md section 5.13).  CUT = false is the lane as it always was.
+// operations (DESIGN.md section 5.13).  A hidden source splat `src` (gsr_select_*, DESIGN.md section 5.17) leaves there too.  CUT = false
+// is the lane as it always was.
 template <bool QUICK, bool INST = false, bool ORTHO = false, bool AA = false, bool CUT = false>
 __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const float *V, const float *cam, const float *At, const float4 pt,
-                                             const float4 ca, const float4 cb, LaneOut &o, const CutoutParam<CUT> &ct = CutoutParam<CUT>()) {
+                                             const float4 ca, const float4 cb, LaneOut &o, const CutoutParam<CUT> &ct = CutoutParam<CUT>(),
+                                             uint64_t src = 0u) {
     const float *P = a.vp + 16;  // X[c][r] = X[4*c + r]
     const int W = a.u.dims[0], H = a.u.dims[1];
     const uint32_t gx = (uint32_t)((W + TILE - 1) / TILE), gy = (uint32_t)((H + TILE - 1) / TILE);
@@ -305,9 +300,9 @@ __device__ __forceinline__ bool project_lane(const ProjectionArgs &a, const floa
                     const float w0 = ((At[0] * sp0 + At[3] * sp1) + At[6] * sp2) + At[9];
                     const float w1 = ((At[1] * sp0 + At[4] * sp1) + At[7] * sp2) + At[10];
                     const float w2 = ((At[2] * sp0 + At[5] * sp1) + At[8] * sp2) + At[11];
-                    if (!cutout_drawn(ct, sp0, sp1, sp2, w0, w1, w2)) return false;
+                    if (!cutout_drawn(ct, src, sp0, sp1, sp2, w0, w1, w2)) return false;
                 } else {
-                    if (!cutout_drawn(ct, sp0, sp1, sp2, sp0, sp1, sp2)) return false;
+                    if (!cutout_drawn(ct, src, sp0, sp1, sp2, sp0, sp1, sp2)) return false;
                 }
             }
 
@@ -507,6 +502,16 @@ __device__ __forceinline__ void instance_tint(const InstanceArgs &ia, uint32_t v
 #pragma unroll
     for (int i = 0; i < 3; ++i) col[i] = col[i] * ap[i];
 }
+// gsr_set_selection_style: a selected source splat `src` gets c * keep + add per channel (an FMUL, then an FADD), after the SH clamp and
+// the instance tint.  Read at the record write, like the tint.  CUT = false: nothing.
+template <bool CUT>
+__device__ __forceinline__ void selection_highlight(const CutoutParam<CUT> &ct, uint64_t src, float col[3]) {
+    if constexpr (CUT) {
+        if (!ct.masks.highlight || !mask_bit(ct.masks.selected, src)) return;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) col[i] = col[i] * ct.masks.keep + ct.masks.add[i];
+    }
+}
 
 // INSTANCED (gsr_set_instances): the grid runs over DRAWN ids.  Instance k owns the drawn warps [warp0_k, warp0_k + ceil(count_k/32));
 // drawn warp warp0_k + j projects source splats first_k + 32 j + lane (lanes past count_k are dead) with the instance's V_k / cam_k and
@@ -603,7 +608,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             float4 cb = slab[64 + lane];
             if (ia.appearance) cb.z = cb.z * instance_appearance(ia, iw.k)[3];
             LaneOut o;
-            if (project_lane<false, true, ORTHO, AA, CUT>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], cb, o, ct) && o.n) {
+            if (project_lane<false, true, ORTHO, AA, CUT>(a, sk, sk + 16, sk + 19, slab[lane], slab[32 + lane], cb, o, ct, iw.src0 + lane) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -612,7 +617,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
     } else if (!a.fast_reject) {
         if (id < a.num_splats) {
             LaneOut o;
-            if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o, ct) && o.n) {
+            if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], o, ct, id) && o.n) {
                 n = o.n; x0u = o.x0; y0u = o.y0; wu = o.w; depth = o.depth;
                 r0 = o.r0; r1 = o.r1; splat_opacity = o.opacity; vx = o.vx; vy = o.vy; vz = o.vz;
             }
@@ -626,7 +631,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         //      slot, so scan and emit below are unchanged and the emission order stays the splat-id order).
         bool live = false;
         LaneOut q;
-        if (id < a.num_splats) live = project_lane<true, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q, ct);
+        if (id < a.num_splats) live = project_lane<true, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, slab[lane], slab[32 + lane], slab[64 + lane], q, ct, id);
         s_res[tid] = make_uint4(0u, 0u, 0u, 0xFFFFFFFFu);
         const uint32_t lmask = __ballot_sync(0xffffffffu, live);
         uint32_t wbase = 0;
@@ -641,9 +646,10 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             const uint32_t l2 = li & 31u;
             const uint32_t gid = bid * PROJ_THREADS + li;
             LaneOut o;
-            if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o, ct) && o.n) {
+            if (project_lane<false, false, ORTHO, AA, CUT>(a, a.vp, a.u.camera_pos, nullptr, sl[l2], sl[32 + l2], sl[64 + l2], o, ct, gid) && o.n) {
                 float col[3];
                 sh_color<false, SH_BANDS, HALF>(a.soa + 3ull * a.plane_stride + gid, a.plane_stride, o.vx, o.vy, o.vz, col);
+                selection_highlight<CUT>(ct, gid, col);
                 float4 *rec = a.records + (uint64_t)gid * 3u;
                 rec[0] = o.r0; rec[1] = o.r1; rec[2] = make_float4(col[0], col[1], col[2], o.opacity);
                 s_res[li] = make_uint4(o.n, o.x0 | (o.y0 << 16), o.w | (o.depth << 16), (uint32_t)o.last_tile);
@@ -720,6 +726,8 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
             float col[3];
             sh_color<true, SH_BANDS, HALF>(slab + 3 * 32 + lane, 32, vx, vy, vz, col);
             if constexpr (INSTANCED) instance_tint(ia, vwarp, col);
+            if constexpr (INSTANCED && CUT) selection_highlight<CUT>(ct, instance_warp(a, ia, vwarp).src0 + lane, col);
+            else selection_highlight<CUT>(ct, id, col);
             float4 *rec = a.records + (uint64_t)id * 3u;
             rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
         }
@@ -728,6 +736,8 @@ __global__ void __launch_bounds__(PROJ_THREADS, GSR_PROJ_MIN_BLOCKS) projection_
         if constexpr (INSTANCED) sh_color<false, SH_BANDS, HALF>(a.soa + 3ull * a.plane_stride + instance_warp(a, ia, vwarp).src0 + lane, a.plane_stride, vx, vy, vz, col);
         else sh_color<false, SH_BANDS, HALF>(a.soa + 3ull * a.plane_stride + id, a.plane_stride, vx, vy, vz, col);
         if constexpr (INSTANCED) instance_tint(ia, vwarp, col);
+        if constexpr (INSTANCED && CUT) selection_highlight<CUT>(ct, instance_warp(a, ia, vwarp).src0 + lane, col);
+        else selection_highlight<CUT>(ct, id, col);
         float4 *rec = a.records + (uint64_t)id * 3u;
         rec[0] = r0; rec[1] = r1; rec[2] = make_float4(col[0], col[1], col[2], splat_opacity);
     }
@@ -1388,20 +1398,20 @@ void launch_projection_depth(const ProjectionArgs &a, const InstanceArgs &ia, ui
     else launch_projection_modes<INSTANCED, false, CUT, HALF>(a, ia, nullptr, ct, blocks, stream, sh_bands, ortho, aa);
 }
 template <bool INSTANCED, bool HALF>
-void launch_projection_cut(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutArgs *cut, uint32_t blocks,
+void launch_projection_cut(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutParams *cut, uint32_t blocks,
                            cudaStream_t stream, int sh_bands, bool ortho, bool aa) {
     if (cut) launch_projection_depth<INSTANCED, true, HALF>(a, ia, dw, *cut, blocks, stream, sh_bands, ortho, aa);
     else launch_projection_depth<INSTANCED, false, HALF>(a, ia, dw, NoCutouts(), blocks, stream, sh_bands, ortho, aa);
 }
 template <bool INSTANCED>
-void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutoutArgs *cut, uint32_t blocks,
+void launch_projection_special(const ProjectionArgs &a, const InstanceArgs &ia, uint32_t *dw, const CutParams *cut, uint32_t blocks,
                                cudaStream_t stream, int sh_bands, bool ortho, bool aa, bool sh_half) {
     if (sh_half) launch_projection_cut<INSTANCED, true>(a, ia, dw, cut, blocks, stream, sh_bands, ortho, aa);
     else launch_projection_cut<INSTANCED, false>(a, ia, dw, cut, blocks, stream, sh_bands, ortho, aa);
 }
 
 int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands, bool ortho, bool aa, uint32_t *depth_words,
-                      const CutoutArgs *cutouts, bool sh_half) {
+                      const CutParams *cutouts, bool sh_half) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
     if (ortho || aa || depth_words || cutouts || sh_half) {
@@ -1426,7 +1436,7 @@ int launch_projection(const ProjectionArgs &a, cudaStream_t stream, int sh_bands
 }
 
 int launch_projection_instanced(const ProjectionArgs &a, const InstanceArgs &ia, cudaStream_t stream, int sh_bands, bool ortho, bool aa,
-                                uint32_t *depth_words, const CutoutArgs *cutouts, bool sh_half) {
+                                uint32_t *depth_words, const CutParams *cutouts, bool sh_half) {
     const uint32_t blocks = projection_num_blocks(a.num_splats);
     if (blocks == 0) return GSR_OK;
     if (ortho || aa || depth_words || cutouts || sh_half) {

@@ -120,7 +120,8 @@ class GaussianSplattingRasterizer:
         device_ingest=True runs the per-splat preprocessing of ply_file.gd:44-69 on the GPU instead of in numpy."""
         assert self.render_texture is not None, "An output Texture2DRD must be set!"
         L = _lib.lib()
-        cfg = _lib.GsrConfig(self._device, self._flags, max(1, self.point_cloud.size), self._factor, self._sh_bands)
+        self._max_splats = max(1, self.point_cloud.size)
+        cfg = _lib.GsrConfig(self._device, self._flags, self._max_splats, self._factor, self._sh_bands)
         _lib.check(L.gsr_create(C.byref(cfg), C.byref(self._ctx)), "gsr_create")
         w, h = self._texture_size
         _lib.check(L.gsr_resize(self._ctx, w, h), "gsr_resize")
@@ -290,6 +291,76 @@ class GaussianSplattingRasterizer:
             return
         arr = pack_instance_appearance(appearance)
         _lib.check(_lib.lib().gsr_set_instance_appearance(self._ctx, arr, len(arr)), "gsr_set_instance_appearance")
+
+    # ---- splat selection (include/gsr.h "Splat selection"): per-splat selected / hidden masks set on the GPU ----
+    def select_polygon(self, xy, op: int = _lib.GSR_SELECT_SET, instance: int = -1) -> None:
+        """Select the splats whose centres the current camera (update_camera_matrices) projects inside a screen lasso or rectangle: xy =
+        (n, 2) pixel positions (column, row) at the current texture size, 3 <= n <= GSR_MAX_SELECT_VERTICES.  instance = -1 tests every
+        splat, k only instance k's range at its current transform.  op: GSR_SELECT_SET / _ADD / _SUBTRACT / _TOGGLE."""
+        if self.camera_push_constants is None:
+            self.update_camera_matrices()
+        v = np.ascontiguousarray(xy, dtype=np.float32).reshape(-1, 2)
+        fp = C.POINTER(C.c_float)
+        _lib.check(_lib.lib().gsr_select_polygon(self._ctx, self.camera_push_constants.ctypes.data_as(fp), float(self.model_scale[0]),
+                                                 int(instance), v.ctypes.data_as(fp), v.shape[0], int(op)), "gsr_select_polygon")
+
+    def select_volume(self, transform, shape: int, space: int = _lib.GSR_CUTOUT_FRAME, op: int = _lib.GSR_SELECT_SET,
+                      instance: int = -1) -> None:
+        """Select the splats whose centres lie in a box or ellipsoid given like set_cutouts' volumes (a Godot Transform3D of the unit
+        shape, in world space for GSR_CUTOUT_FRAME, in the asset's space for GSR_CUTOUT_SOURCE)."""
+        vol = _lib.GsrCutout()
+        vol.to_local[:] = [float(x) for x in cutout_to_local(transform, self.basis_override).T.reshape(12)]
+        vol.shape, vol.action, vol.space = int(shape), _lib.GSR_CUTOUT_KEEP, int(space)
+        _lib.check(_lib.lib().gsr_select_volume(self._ctx, C.byref(vol), float(self.model_scale[0]), int(instance), int(op)),
+                   "gsr_select_volume")
+
+    def select_ids(self, ids_ptr: int, rect=None, op: int = _lib.GSR_SELECT_SET) -> None:
+        """"Select what you see": the splats of every pixel of rect = (x0, y0, x1, y1) (None: the whole frame) of a device ID plane
+        written by set_splat_ids."""
+        w, h = self._texture_size
+        x0, y0, x1, y1 = (0, 0, w, h) if rect is None else (int(r) for r in rect)
+        _lib.check(_lib.lib().gsr_select_ids(self._ctx, C.c_void_p(ids_ptr), x0, y0, x1, y1, int(op)), "gsr_select_ids")
+
+    def select_all(self, op: int = _lib.GSR_SELECT_SET) -> None:
+        """SET: select every splat; SUBTRACT: select none; TOGGLE: invert the selection."""
+        _lib.check(_lib.lib().gsr_select_all(self._ctx, int(op)), "gsr_select_all")
+
+    def hide_selection(self) -> None:
+        _lib.check(_lib.lib().gsr_hide_selection(self._ctx), "gsr_hide_selection")
+
+    def unhide_all(self) -> None:
+        _lib.check(_lib.lib().gsr_unhide_all(self._ctx), "gsr_unhide_all")
+
+    def clear_splat_masks(self) -> None:
+        """No splat selected or hidden, and the masks out of use: frames take their usual kernels again."""
+        _lib.check(_lib.lib().gsr_clear_splat_masks(self._ctx), "gsr_clear_splat_masks")
+
+    def set_selection_style(self, rgb, strength: float) -> None:
+        """Highlight of selected splats: colour * (1 - strength) + rgb * strength (strength 0: no highlight)."""
+        c = (C.c_float * 3)(*[float(x) for x in rgb])
+        _lib.check(_lib.lib().gsr_set_selection_style(self._ctx, c, float(strength)), "gsr_set_selection_style")
+
+    def splat_masks(self) -> tuple[np.ndarray, np.ndarray]:
+        """(hidden, selected): numpy bool arrays over the source splats (synchronises).  The kept cloud is table[~hidden]."""
+        n = self._max_splats
+        words = (n + 31) // 32
+        hid, sel = np.zeros(words, dtype=np.uint32), np.zeros(words, dtype=np.uint32)
+        u32p = C.POINTER(C.c_uint32)
+        _lib.check(_lib.lib().gsr_get_splat_masks(self._ctx, hid.ctypes.data_as(u32p), sel.ctypes.data_as(u32p), words), "gsr_get_splat_masks")
+        return unpack_mask(hid, n), unpack_mask(sel, n)
+
+    def set_splat_masks(self, hidden, selected) -> None:
+        """Restore masks read with splat_masks (undo): bool arrays over the source splats, never both True for one splat."""
+        n = self._max_splats
+        hid, sel = pack_mask(hidden, n), pack_mask(selected, n)
+        u32p = C.POINTER(C.c_uint32)
+        _lib.check(_lib.lib().gsr_set_splat_masks(self._ctx, hid.ctypes.data_as(u32p), sel.ctypes.data_as(u32p), hid.size), "gsr_set_splat_masks")
+
+    def selection_counts(self) -> tuple[int, int]:
+        """(selected, hidden) splat counts (synchronises)."""
+        s, h = C.c_uint64(0), C.c_uint64(0)
+        _lib.check(_lib.lib().gsr_splat_mask_counts(self._ctx, C.byref(s), C.byref(h)), "gsr_splat_mask_counts")
+        return int(s.value), int(h.value)
 
     def render_raw(self, vp32: np.ndarray, uniforms32: bytes, heatmap: float = 0.0, host_ptr: int | None = None,
                    asynchronous: bool = True, rgb_only: bool = False, out_format: int | None = None) -> None:
@@ -498,6 +569,21 @@ def splat_sources(ids: np.ndarray, ranges=None) -> np.ndarray:
     kk = k[hit].astype(np.int64)
     out[hit] = (first[kk] + (v[hit].astype(np.int64) - 32 * w0[kk])).astype(np.uint32)
     return out
+
+
+def pack_mask(mask, n: int) -> np.ndarray:
+    """A bool array over n splats -> the ceil(n / 32) uint32 words of include/gsr.h (splat s = bit s & 31 of word s >> 5)."""
+    m = np.asarray(mask, dtype=bool).reshape(-1)
+    assert m.size == n, (m.size, n)
+    words = (n + 31) // 32
+    bits = np.zeros(words * 32, dtype=bool)
+    bits[:n] = m
+    return np.packbits(bits, bitorder="little").view("<u4").astype(np.uint32)
+
+
+def unpack_mask(words: np.ndarray, n: int) -> np.ndarray:
+    """The inverse of pack_mask: uint32 words -> a bool array over n splats."""
+    return np.unpackbits(np.ascontiguousarray(words, dtype="<u4").view(np.uint8), bitorder="little")[:n].astype(bool)
 
 
 def godot_to_frame(transform, basis_override) -> np.ndarray:

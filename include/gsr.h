@@ -222,6 +222,7 @@ GSR_API int gsr_peer_import_framebuffers(gsr_ctx *ctx, const void *handles128);
  *        - anti-aliasing (gsr_set_antialiasing > 0);
  *        - view-depth order (gsr_set_depth_order GSR_DEPTH_ORDER_VIEW_DEPTH);
  *        - cutouts (gsr_set_cutouts with n > 0);
+ *        - splat masks in use (gsr_select_*, gsr_set_splat_masks; until gsr_clear_splat_masks);
  *        - orthographic frames (GSR_FLAG_ORTHOGRAPHIC; the flag alone is no feature, each orthographic frame is).
  *      A context is sharded while any of these holds:
  *        - a shard group is attached (gsr_group_attach with world > 1);
@@ -525,6 +526,75 @@ typedef struct gsr_cutout {
     int32_t shape, action, space;
 } gsr_cutout;
 GSR_API int gsr_set_cutouts(gsr_ctx *ctx, const gsr_cutout *cutouts, uint32_t n);
+
+/* ---- Splat selection: select, highlight and hide individual splats (no reference counterpart).  The cleaning loop of a splat editor
+ *      -- select floaters with a screen lasso, a volume or a click on what is visible, look at the highlighted selection, hide it, undo,
+ *      export what is left -- without touching the uploaded data.
+ *      State: two bitmasks over the SOURCE splats [0, max_splats), `hidden` and `selected`, one bit per splat, 32 splats per uint32 word
+ *      (splat s is bit s & 31 of word s >> 5); bits at or past max_splats are always 0.  With instances, a source splat's bits apply to
+ *      every instance that draws it (an edit of the asset, like a GSR_CUTOUT_SOURCE volume).  A hidden splat is never selected: every
+ *      operation ends with selected &= ~hidden.
+ *      The masks are IN USE from the first call that can set a bit (any gsr_select_*, gsr_set_splat_masks) until gsr_clear_splat_masks.
+ *      The first such call allocates the masks zeroed (it may synchronise once; GSR_ERR_OOM keeps the previous state); later calls never
+ *      synchronise and never allocate.  Uploads, gsr_resize, gsr_set_instances and appearance changes keep the masks.
+ *      Frame rule, while the masks are in use: the source splat of a drawn id v is s = v without instances and s = first_k + (v - 32 w_k)
+ *      with them (see gsr_set_instances).
+ *        - hidden: the splat is removed after the frustum cull and the cutouts, exactly like a cutout-removed splat: no record, no
+ *          pairs, no share of M, V or the last tile;
+ *        - selected, with highlight strength s_h > 0: after the SH clamp and the instance tint, each colour channel becomes
+ *          c' = (c * k) + h, an FMUL then an FADD (not fused), with k = 1 - s_h and h = rgb * s_h computed once in float32;
+ *        - everything else is bit for bit the frame without masks, including masks in use but empty, and s_h = 0.
+ *      Depth compositing, motion vectors and splat IDs follow from the records: IDs never report a hidden splat, and gsr_pick sees none.
+ *      Masks in use are a single-context feature (see "Single-context features"); gsr_clear_splat_masks is never refused.
+ *      Operations: each is enqueued on the stream the frames' projections run on (the render stream; with gsr_debug_pipeline(ctx, 1)
+ *      the front stream, so an operation does not wait for the previous frame's compositor, except gsr_select_ids, which reads an ID
+ *      plane a compositor wrote), does not synchronise the host, and is ordered after every frame enqueued before it and before every
+ *      frame enqueued after it.  `op` combines the operation's `inside` set with the selection:
+ *        GSR_SELECT_SET       selected = inside (splats outside the tested range count as outside)
+ *        GSR_SELECT_ADD       selected | inside
+ *        GSR_SELECT_SUBTRACT  selected & ~inside
+ *        GSR_SELECT_TOGGLE    selected ^ inside
+ *      gsr_select_all: inside = every splat (SET: select all; SUBTRACT: select none; TOGGLE: invert).
+ *      gsr_select_polygon: a screen lasso or rectangle of 3 <= n <= GSR_MAX_SELECT_VERTICES vertices xy (x0, y0, x1, y1, ...) in the
+ *        frame's pixel axes (column, row; y grows downwards) at the current gsr_resize size.  Tested position q: instance = -1 tests every
+ *        splat with q = sp = position * model_scale; instance = k tests only instance k's source range with
+ *        q[r] = ((A[r] sp0 + A[3+r] sp1) + A[6+r] sp2) + A[9+r], A = instance k's current to_frame.  (px, py) = pix(view_proj, q), the
+ *        rule of gsr_set_motion_vectors.  Inside requires clip3 > 0 and the even-odd test in float32 (one rounding per operation, no
+ *        contraction): for every edge a -> b (the last vertex connects to the first) with (a.y > py) != (b.y > py),
+ *        x = (((b.x - a.x) (py - a.y)) / (b.y - a.y)) + a.x, and px < x toggles inside.  A NaN position is outside.
+ *      gsr_select_volume: the cutout shape test of gsr_set_cutouts on the same tested range, on sp (GSR_CUTOUT_SOURCE) or q
+ *        (GSR_CUTOUT_FRAME); `action` is ignored.
+ *      gsr_select_ids: "select what you see".  Every pixel of [x0, x1) x [y0, y1) of a device ID plane in the layout of gsr_set_splat_ids
+ *        whose v != GSR_NO_ID marks the source splat of v under the current instance layout; a v past the layout's drawn ids is ignored.
+ *      gsr_select_polygon and gsr_select_ids return GSR_ERR_STATE before gsr_resize.
+ *      gsr_hide_selection: hidden |= selected, then selected = 0.  gsr_unhide_all: hidden = 0.
+ *      gsr_clear_splat_masks: both masks 0 and no longer in use: frames take exactly the kernels they took before.
+ *      gsr_get_splat_masks / gsr_splat_mask_counts synchronise and return the masks (zeros while not in use) / their population counts.
+ *      gsr_set_splat_masks (undo, restore) has read the host arrays when it returns: a copy from pageable memory, it may wait for the
+ *      work already enqueued on that stream.
+ *      gsr_set_selection_style: rgb finite in [0, GSR_TINT_MAX], strength in [0, 1]; default {1, 0.5, 0} at 0.5; read when a frame is
+ *        enqueued.
+ *      GSR_ERR_INVALID, previous state kept: an unknown op, an instance outside the current layout, n out of range, a non-finite vertex
+ *      or to_local, an unknown shape or space, a rectangle outside the image, a NULL array, words != ceil(max_splats / 32), bits past
+ *      max_splats, hidden and selected bits that overlap (gsr_set_splat_masks).  Export of the kept cloud: the rows of the source table
+ *      whose hidden bit is 0. ---- */
+#define GSR_MAX_SELECT_VERTICES 64
+#define GSR_SELECT_SET 0
+#define GSR_SELECT_ADD 1
+#define GSR_SELECT_SUBTRACT 2
+#define GSR_SELECT_TOGGLE 3
+GSR_API int gsr_select_all(gsr_ctx *ctx, int32_t op);
+GSR_API int gsr_select_polygon(gsr_ctx *ctx, const float view_proj[32], float model_scale, int32_t instance, const float *xy, uint32_t n,
+                               int32_t op);
+GSR_API int gsr_select_volume(gsr_ctx *ctx, const gsr_cutout *volume, float model_scale, int32_t instance, int32_t op);
+GSR_API int gsr_select_ids(gsr_ctx *ctx, const uint32_t *ids_device, int32_t x0, int32_t y0, int32_t x1, int32_t y1, int32_t op);
+GSR_API int gsr_hide_selection(gsr_ctx *ctx);
+GSR_API int gsr_unhide_all(gsr_ctx *ctx);
+GSR_API int gsr_clear_splat_masks(gsr_ctx *ctx);
+GSR_API int gsr_get_splat_masks(gsr_ctx *ctx, uint32_t *hidden, uint32_t *selected, uint64_t words);
+GSR_API int gsr_set_splat_masks(gsr_ctx *ctx, const uint32_t *hidden, const uint32_t *selected, uint64_t words);
+GSR_API int gsr_splat_mask_counts(gsr_ctx *ctx, uint64_t *selected, uint64_t *hidden);
+GSR_API int gsr_set_selection_style(gsr_ctx *ctx, const float rgb[3], float strength);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
