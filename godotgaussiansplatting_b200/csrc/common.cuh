@@ -316,6 +316,24 @@ int launch_hide_selection(uint32_t *hidden, uint32_t *selected, uint32_t words, 
 int launch_mask_counts(const uint32_t *selected, const uint32_t *hidden, uint32_t words, unsigned long long *counts, cudaStream_t stream);
 int preload_selection_kernels();
 
+// ---- selection transform edits (gsr_transform_selection; selection.cu) ----
+// The operation's constants: to_source [L | t] (12 floats, column-major 3x4), then the SH band matrices M~_1, M~_2, M~_3 (3x3, 5x5, 7x7,
+// row-major): 95 floats, the layout of GSR_BUF_EDIT_TRANSFORM.
+__host__ __device__ constexpr int edit_matrix_offset(int l) { return l == 1 ? 12 : l == 2 ? 21 : 46; }   // M~_l, l = 1..3
+constexpr int EDIT_TRANSFORM_FLOATS = 95;
+// Host, float64: the 95 floats of to_source.  GSR_ERR_INVALID when det(L) is 0 or not finite (entries are checked by the caller).
+int edit_transform_matrices(const float to_source[12], float out[EDIT_TRANSFORM_FLOATS]);
+struct TransformArgs {
+    float4 *dst;               // the store
+    const float4 *src;         // the store itself, or a snapshot in its layout
+    uint64_t plane_stride;
+    const uint32_t *selected;
+    uint32_t words;
+    float m[EDIT_TRANSFORM_FLOATS];
+};
+// Rewrites every selected splat of the store from `src` (store bands and format as given).
+int launch_transform_selection(const TransformArgs &a, int bands, bool sh_half, cudaStream_t stream);
+
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.
 __host__ __device__ __forceinline__ uint32_t depth_order_word(uint32_t bits) { return bits ^ ((bits >> 31) ? 0xFFFFFFFFu : 0x80000000u); }

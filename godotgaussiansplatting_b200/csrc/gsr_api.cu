@@ -56,6 +56,9 @@ struct gsr_ctx {
         float rgb[3] = {1.0f, 0.5f, 0.0f};
         float strength = 0.5f;
     } masks;
+    // store edits and snapshots (gsr_transform_selection, gsr_copy_splat_store, gsr_restore_splat_store)
+    float edit_last[EDIT_TRANSFORM_FLOATS] = {};   // GSR_BUF_EDIT_TRANSFORM: the constants of the last accepted transform
+    cudaEvent_t store_ready = nullptr;             // with front / back overlap: the render stream's work enqueued before the operation
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -317,6 +320,7 @@ void free_ctx(gsr_ctx *c) {
     cudaFree(c->inst.desc); cudaFree(c->inst.warps); cudaFree(c->inst.frame);
     cudaFree(c->masks.counts);   // the base of the mask allocation
     if (c->masks.ids_ready) cudaEventDestroy(c->masks.ids_ready);
+    if (c->store_ready) cudaEventDestroy(c->store_ready);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
     for (int i = 0; i < GSR_INSTANCE_RING; ++i) if (c->inst.ev[i]) cudaEventDestroy(c->inst.ev[i]);
     delete[] c->inst.range; delete[] c->inst.xf; delete[] c->inst.app;
@@ -1931,6 +1935,61 @@ GSR_API int gsr_set_selection_style(gsr_ctx *c, const float rgb[3], float streng
     return GSR_OK;
 }
 
+// ---- splat transform edits and store snapshots ------------------------------------------------------------------------------------
+// Enqueued on the projections' stream (mask_stream) like the mask operations, so they come before the projections of later frames.
+// Unlike them they also wait for the render stream's work: the previous frame's compositor reads plane 0 for the motion vectors of
+// instanced frames.
+static int store_stream(gsr_ctx *c, cudaStream_t *out) {
+    const cudaStream_t ms = mask_stream(c);
+    if (ms != c->stream) {
+        if (!c->store_ready) GSR_CUDA_TRY(cudaEventCreateWithFlags(&c->store_ready, cudaEventDisableTiming));
+        GSR_CUDA_TRY(cudaEventRecord(c->store_ready, c->stream));
+        GSR_CUDA_TRY(cudaStreamWaitEvent(ms, c->store_ready, 0));
+    }
+    *out = ms;
+    return GSR_OK;
+}
+
+static uint64_t store_bytes(const gsr_ctx *c) { return sizeof(float4) * (uint64_t)soa_planes(c->sh_bands, sh_half(c)) * c->plane_stride; }
+
+GSR_API int gsr_transform_selection(gsr_ctx *c, const float to_source[12], const void *src_store) {
+    if (!c || !to_source) { set_last_error("gsr_transform_selection: NULL argument"); return GSR_ERR_INVALID; }
+    for (int e = 0; e < 12; ++e) {
+        if (!(fabsf(to_source[e]) <= 3.402823466e38f)) { set_last_error("gsr_transform_selection: non-finite to_source[%d]", e); return GSR_ERR_INVALID; }
+    }
+    TransformArgs a;
+    if (edit_transform_matrices(to_source, a.m)) { set_last_error("gsr_transform_selection: det(L) is 0 or not finite"); return GSR_ERR_INVALID; }
+    if (!c->masks.on) { set_last_error("gsr_transform_selection: the splat masks are not in use"); return GSR_ERR_STATE; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    cudaStream_t s;
+    if ((rc = store_stream(c, &s))) return rc;
+    a.dst = c->soa;
+    a.src = src_store ? static_cast<const float4 *>(src_store) : c->soa;
+    a.plane_stride = c->plane_stride;
+    a.selected = c->masks.selected;
+    a.words = c->masks.words;
+    if ((rc = launch_transform_selection(a, c->sh_bands, sh_half(c), s))) return rc;
+    memcpy(c->edit_last, a.m, sizeof c->edit_last);
+    return GSR_OK;
+}
+
+GSR_API uint64_t gsr_splat_store_bytes(gsr_ctx *c) { return c ? store_bytes(c) : 0ull; }
+
+static int store_copy(gsr_ctx *c, void *dst, const void *src, const char *where) {
+    if (!c || !dst || !src) { set_last_error("%s: NULL argument", where); return GSR_ERR_INVALID; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    cudaStream_t s;
+    if ((rc = store_stream(c, &s))) return rc;
+    GSR_CUDA_TRY(cudaMemcpyAsync(dst, src, store_bytes(c), cudaMemcpyDefault, s));
+    return GSR_OK;
+}
+
+GSR_API int gsr_copy_splat_store(gsr_ctx *c, void *dst) { return store_copy(c, dst, c ? c->soa : nullptr, "gsr_copy_splat_store"); }
+
+GSR_API int gsr_restore_splat_store(gsr_ctx *c, const void *src) { return store_copy(c, c ? c->soa : nullptr, src, "gsr_restore_splat_store"); }
+
 GSR_API int gsr_pick(gsr_ctx *c, uint32_t tile_id, float heatmap_factor, float out_xyzn[4]) {
     if (!c || !out_xyzn) return GSR_ERR_INVALID;
     if (c->width == 0) { set_last_error("gsr_pick before gsr_resize"); return GSR_ERR_STATE; }
@@ -2083,6 +2142,12 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
             avail = sizeof(float) * INSTANCE_XFORM_FLOATS * c->inst.n;
             if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }
             memcpy(dst, c->inst.xf, bytes);
+            return GSR_OK;
+        }
+        case GSR_BUF_EDIT_TRANSFORM: {   // host copy: no device involved
+            avail = sizeof c->edit_last;
+            if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }
+            memcpy(dst, c->edit_last, bytes);
             return GSR_OK;
         }
         case GSR_BUF_INSTANCE_APPEARANCE: {   // host copy: no device involved

@@ -147,12 +147,247 @@ __global__ void __launch_bounds__(SEL_THREADS) mask_counts_kernel(const uint32_t
     }
 }
 
+// gsr_transform_selection: every selected splat s of the store is rewritten from its planes in `src` (include/gsr.h "Splat transform
+// edits").  Like the region kernels a warp owns one mask word: a warp whose word is 0 leaves after that one load, and the lanes of a
+// selected warp read consecutive 16-byte words of every plane.  Unselected splats are never written (a hidden splat is never selected).
+// In float32, one rounding per operation, no contraction: position L x + t, covariance (L S) L^T (the six stored entries), SH band l
+// c'_j = sum_i c_i M~_l[i][j] left to right per channel; creation time, opacity, plane-2 pad and DC copied bit for bit, slots past 3K +0.
+template <int BANDS, bool HALF>
+__global__ void __launch_bounds__(SEL_THREADS) transform_selection_kernel(const __grid_constant__ TransformArgs a) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t w = blockIdx.x * SEL_WARPS + (threadIdx.x >> 5);
+    if (w >= a.words) return;   // warp-uniform
+    const uint32_t word = a.selected[w];
+    if (((word >> lane) & 1u) == 0u) return;
+    const uint64_t s = 32ull * w + lane, st = a.plane_stride;
+    const float4 *src = a.src + s;
+    float4 *dst = a.dst + s;
+    const float *L = a.m;
+    const float4 p0 = src[0], p1 = src[st], p2 = src[2 * st];
+    const float x[3] = {p0.x, p0.y, p0.z};
+    float q[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+        q[r] = __fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(L[r], x[0]), __fmul_rn(L[3 + r], x[1])), __fmul_rn(L[6 + r], x[2])), L[9 + r]);
+    const float S[3][3] = {{p1.x, p1.y, p1.z}, {p1.y, p1.w, p2.x}, {p1.z, p2.x, p2.y}};
+    float G[3][3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+            G[r][c] = __fadd_rn(__fadd_rn(__fmul_rn(L[r], S[0][c]), __fmul_rn(L[3 + r], S[1][c])), __fmul_rn(L[6 + r], S[2][c]));
+    float E[3][3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+        for (int c = r; c < 3; ++c)
+            E[r][c] = __fadd_rn(__fadd_rn(__fmul_rn(G[r][0], L[c]), __fmul_rn(G[r][1], L[3 + c])), __fmul_rn(G[r][2], L[6 + c]));
+    dst[0] = make_float4(q[0], q[1], q[2], p0.w);
+    dst[st] = make_float4(E[0][0], E[0][1], E[0][2], E[1][1]);
+    dst[2 * st] = make_float4(E[1][2], E[2][2], p2.z, p2.w);
+
+    constexpr int NV = 3 * sh_coeffs(BANDS), P = sh_planes(BANDS, HALF);
+    float c[HALF ? 8 * P : 4 * P];
+    uint32_t dc_words[2] = {0u, 0u};   // binary16: the words holding values 0-3 (the DC halves are copied as stored)
+#pragma unroll
+    for (int k = 0; k < P; ++k) {
+        const float4 v = src[(uint64_t)(3 + k) * st];
+        if constexpr (HALF) {
+            const uint32_t u[4] = {__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
+            if (k == 0) { dc_words[0] = u[0]; dc_words[1] = u[1]; }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                c[8 * k + 2 * j] = half_bits_to_float(u[j] & 0xFFFFu);
+                c[8 * k + 2 * j + 1] = half_bits_to_float(u[j] >> 16);
+            }
+        } else {
+            c[4 * k + 0] = v.x; c[4 * k + 1] = v.y; c[4 * k + 2] = v.z; c[4 * k + 3] = v.w;
+        }
+    }
+#pragma unroll
+    for (int l = 1; l < BANDS; ++l) {
+        const int n = 2 * l + 1, k0 = l * l;
+        const float *M = a.m + edit_matrix_offset(l);
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) {
+            float in[7];
+#pragma unroll
+            for (int i = 0; i < n; ++i) in[i] = c[3 * (k0 + i) + ch];
+#pragma unroll
+            for (int j = 0; j < n; ++j) {
+                float acc = __fmul_rn(in[0], M[j]);
+#pragma unroll
+                for (int i = 1; i < n; ++i) acc = __fadd_rn(acc, __fmul_rn(in[i], M[i * n + j]));
+                c[3 * (k0 + j) + ch] = acc;
+            }
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < P; ++k) {
+        uint32_t u[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if constexpr (HALF) {
+                const int i = 8 * k + 2 * j;
+                const uint32_t lo = i < 3 ? (dc_words[i >> 1] & 0xFFFFu) : i < NV ? sh_half(c[i]) : 0u;
+                const uint32_t hi = i + 1 < 3 ? (dc_words[(i + 1) >> 1] >> 16) : i + 1 < NV ? sh_half(c[i + 1]) : 0u;
+                u[j] = lo | (hi << 16);
+            } else {
+                u[j] = 4 * k + j < NV ? __float_as_uint(c[4 * k + j]) : 0u;
+            }
+        }
+        dst[(uint64_t)(3 + k) * st] = make_float4(__uint_as_float(u[0]), __uint_as_float(u[1]), __uint_as_float(u[2]), __uint_as_float(u[3]));
+    }
+}
+
 }  // namespace
+
+// ---- the host's float64 matrices of gsr_transform_selection (also compiled into the CPU kernel emulator) ----
+namespace {
+// P_l(d): the polynomials that multiply coefficients l^2 .. l^2 + 2l in sh_color (projection.cu), signs included, with the float64
+// values of its constants
+void sh_band_poly(int l, const double d[3], double *p) {
+    const double x = d[0], y = d[1], z = d[2], xx = x * x, yy = y * y, zz = z * z;
+    if (l == 1) {
+        const double c1 = 0.4886025119029199;
+        p[0] = -c1 * y; p[1] = c1 * z; p[2] = -c1 * x;
+    } else if (l == 2) {
+        p[0] = 1.0925484305920792 * x * y; p[1] = -1.0925484305920792 * y * z; p[2] = 0.31539156525252005 * (2.0 * zz - xx - yy);
+        p[3] = -1.0925484305920792 * x * z; p[4] = 0.5462742152960396 * (xx - yy);
+    } else {
+        p[0] = -0.5900435899266435 * y * (3.0 * xx - yy); p[1] = 2.890611442640554 * x * y * z;
+        p[2] = -0.4570457994644658 * y * (4.0 * zz - xx - yy); p[3] = 0.3731763325901154 * z * (2.0 * zz - 3.0 * xx - 3.0 * yy);
+        p[4] = -0.4570457994644658 * x * (4.0 * zz - xx - yy); p[5] = 1.445305721320277 * z * (xx - yy);
+        p[6] = -0.5900435899266435 * x * (xx - 3.0 * yy);
+    }
+}
+
+double det3(const double X[3][3]) {
+    return X[0][0] * (X[1][1] * X[2][2] - X[1][2] * X[2][1]) - X[0][1] * (X[1][0] * X[2][2] - X[1][2] * X[2][0]) +
+           X[0][2] * (X[1][0] * X[2][1] - X[1][1] * X[2][0]);
+}
+
+// Solves A X = B in place (A n x n, B n x m, row-major), Gaussian elimination with partial pivoting
+void solve(double *A, double *B, int n, int m) {
+    for (int k = 0; k < n; ++k) {
+        int piv = k;
+        for (int r = k + 1; r < n; ++r) if (fabs(A[r * n + k]) > fabs(A[piv * n + k])) piv = r;
+        if (piv != k) {
+            for (int c = 0; c < n; ++c) { const double t = A[k * n + c]; A[k * n + c] = A[piv * n + c]; A[piv * n + c] = t; }
+            for (int c = 0; c < m; ++c) { const double t = B[k * m + c]; B[k * m + c] = B[piv * m + c]; B[piv * m + c] = t; }
+        }
+        for (int r = k + 1; r < n; ++r) {
+            const double f = A[r * n + k] / A[k * n + k];
+            for (int c = k; c < n; ++c) A[r * n + c] -= f * A[k * n + c];
+            for (int c = 0; c < m; ++c) B[r * m + c] -= f * B[k * m + c];
+        }
+    }
+    for (int k = n - 1; k >= 0; --k) {
+        for (int c = 0; c < m; ++c) {
+            double v = B[k * m + c];
+            for (int j = k + 1; j < n; ++j) v -= A[k * n + j] * B[j * m + c];
+            B[k * m + c] = v / A[k * n + k];
+        }
+    }
+}
+
+// Q = the orthogonal polar factor of L (U V^T of its SVD; improper when det L < 0) by Newton's iteration X <- (g X + (g X)^-T) / 2,
+// with the determinant scaling g = |det X|^(-1/3) while X is far from orthogonal.
+void polar_factor(const double L[3][3], double X[3][3]) {
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) X[r][c] = L[r][c];
+    for (int it = 0; it < 100; ++it) {
+        const double d = det3(X);
+        double cof[3][3];   // X^-T = cof(X) / det X
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) {
+                const int r1 = (r + 1) % 3, r2 = (r + 2) % 3, c1 = (c + 1) % 3, c2 = (c + 2) % 3;
+                cof[r][c] = X[r1][c1] * X[r2][c2] - X[r1][c2] * X[r2][c1];
+            }
+        double err = 0.0;
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) { const double e = X[r][c] - cof[r][c] / d; err += e * e; }
+        const double g = err > 1e-4 ? pow(fabs(d), -1.0 / 3.0) : 1.0;
+        double diff = 0.0;
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) {
+                const double y = 0.5 * (g * X[r][c] + cof[r][c] / (g * d));
+                diff += (y - X[r][c]) * (y - X[r][c]);
+                X[r][c] = y;
+            }
+        if (diff < 1e-30) break;
+    }
+}
+
+// M_l (row-major (2l+1)^2) with P_l(Q^T d) = M_l P_l(d) for every d: the least-squares solution over 64 directions of a Fibonacci
+// sphere (the relation is exact, so the fit is too), M_l A = B with A = sum P_l(d) P_l(d)^T and B = sum P_l(Q^T d) P_l(d)^T.
+void band_matrix(const double Q[3][3], int l, double *M) {
+    const int n = 2 * l + 1;
+    double A[49] = {}, B[49] = {};
+    for (int k = 0; k < 64; ++k) {
+        const double z = 1.0 - (2.0 * k + 1.0) / 64.0, rr = sqrt(1.0 - z * z), phi = 2.399963229728653 * k;
+        const double d[3] = {rr * cos(phi), rr * sin(phi), z};
+        const double qd[3] = {Q[0][0] * d[0] + Q[1][0] * d[1] + Q[2][0] * d[2], Q[0][1] * d[0] + Q[1][1] * d[1] + Q[2][1] * d[2],
+                              Q[0][2] * d[0] + Q[1][2] * d[1] + Q[2][2] * d[2]};   // Q^T d
+        double p[7], pq[7];
+        sh_band_poly(l, d, p);
+        sh_band_poly(l, qd, pq);
+        for (int i = 0; i < n; ++i)
+            for (int j = 0; j < n; ++j) { A[i * n + j] += p[i] * p[j]; B[i * n + j] += pq[i] * p[j]; }
+    }
+    double Bt[49];   // M A = B with A symmetric: A M^T = B^T
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < n; ++j) Bt[i * n + j] = B[j * n + i];
+    solve(A, Bt, n, n);
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < n; ++j) M[i * n + j] = Bt[j * n + i];
+}
+}  // namespace
+
+// The 95 floats: to_source, then M~_l = M_l(polar factor of L) with entries below 1e-9 in magnitude set to +0, rounded to float32.
+int edit_transform_matrices(const float to_source[12], float out[EDIT_TRANSFORM_FLOATS]) {
+    double L[3][3], Q[3][3];
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) L[r][c] = (double)to_source[3 * c + r];
+    const double det = det3(L);
+    if (!(det != 0.0 && fabs(det) <= 1.7976931348623157e308)) return GSR_ERR_INVALID;
+    polar_factor(L, Q);
+    for (int e = 0; e < 12; ++e) out[e] = to_source[e];
+    for (int l = 1; l <= 3; ++l) {
+        double M[49];
+        band_matrix(Q, l, M);
+        float *o = out + edit_matrix_offset(l);
+        for (int i = 0; i < (2 * l + 1) * (2 * l + 1); ++i) o[i] = fabs(M[i]) < 1e-9 ? 0.0f : (float)M[i];
+    }
+    return GSR_OK;
+}
 
 #ifndef GSR_CPU_EMU
 namespace {
 uint32_t word_blocks(uint32_t words) { return (words + SEL_THREADS - 1) / SEL_THREADS; }
+
+template <int BANDS, bool HALF>
+void launch_transform_variant(const TransformArgs &a, uint32_t blocks, cudaStream_t stream) {
+    transform_selection_kernel<BANDS, HALF><<<blocks, SEL_THREADS, 0, stream>>>(a);
+}
 }  // namespace
+
+int launch_transform_selection(const TransformArgs &a, int bands, bool sh_half, cudaStream_t stream) {
+    if (a.words == 0) return GSR_OK;
+    const uint32_t blocks = (a.words + SEL_WARPS - 1) / SEL_WARPS;
+    switch (bands * 2 + (sh_half ? 1 : 0)) {
+        case 2: launch_transform_variant<1, false>(a, blocks, stream); break;
+        case 3: launch_transform_variant<1, true>(a, blocks, stream); break;
+        case 4: launch_transform_variant<2, false>(a, blocks, stream); break;
+        case 5: launch_transform_variant<2, true>(a, blocks, stream); break;
+        case 6: launch_transform_variant<3, false>(a, blocks, stream); break;
+        case 7: launch_transform_variant<3, true>(a, blocks, stream); break;
+        case 8: launch_transform_variant<4, false>(a, blocks, stream); break;
+        default: launch_transform_variant<4, true>(a, blocks, stream); break;
+    }
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
 
 int launch_select_region(const SelectArgs &a, int kind, cudaStream_t stream) {
     if (a.words == 0) return GSR_OK;
@@ -207,6 +442,14 @@ int preload_selection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_combine_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, hide_selection_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, mask_counts_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<1, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<1, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<2, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<2, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<3, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<3, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<4, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<4, true>));
     return GSR_OK;
 }
 #endif  // GSR_CPU_EMU

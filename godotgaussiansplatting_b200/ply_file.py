@@ -62,6 +62,14 @@ class PlyFile:
             raise ValueError(f"PLY body truncated: {body.size} of {count} floats")
         self.vertices = body.astype(np.float32, copy=False)
 
+    def save(self, path: str) -> None:
+        """Write the table as a binary little-endian PLY of float properties (what parse reads back, and what 3DGS viewers load)."""
+        header = ["ply", "format binary_little_endian 1.0", f"element vertex {self.size}"]
+        header += [f"property float {name}" for name in self.properties] + ["end_header"]
+        with open(path, "wb") as f:
+            f.write(("\n".join(header) + "\n").encode("ascii"))
+            f.write(np.ascontiguousarray(self.table, dtype="<f4").tobytes())
+
     def get_vertex(self, index: int) -> dict:  # util/ply_file.gd:21-26
         n = len(self.properties)
         return {self.properties[i]: float(self.vertices[n * index + i]) for i in range(n)}

@@ -362,6 +362,55 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_splat_mask_counts(self._ctx, C.byref(s), C.byref(h)), "gsr_splat_mask_counts")
         return int(s.value), int(h.value)
 
+    # ---- splat transform edits (include/gsr.h "Splat transform edits") ----
+    def transform_selection(self, transform, space: int = _lib.GSR_CUTOUT_FRAME, instance: int = -1, snapshot_ptr: int | None = None) -> None:
+        """Move, rotate, scale or mirror the selected splats in the store.  transform: a frame-space (3, 4) [B | u] (godot_to_frame
+        converts a Godot Transform3D).  GSR_CUTOUT_SOURCE applies it to the stored positions as given; GSR_CUTOUT_FRAME applies it in
+        frame space as instance `instance` draws the splats (-1: no instance), with the current model_scale.  snapshot_ptr: a device
+        snapshot from copy_splat_store to read instead of the store (a drag re-applies its growing transform to the mouse-down state)."""
+        T = np.asarray(transform, dtype=np.float64)
+        if T.shape == (4, 4):
+            T = T[:3]
+        assert T.shape == (3, 4), T.shape
+        if int(space) == _lib.GSR_CUTOUT_SOURCE:
+            m = T.astype(np.float32)
+        else:
+            A, tk = np.eye(3), np.zeros(3)
+            if instance >= 0:
+                x = self.debug_copy(_lib.GSR_BUF_INSTANCES, 24 * len(self._instance_ranges), np.float32)
+                k = x[24 * instance:24 * instance + 12].astype(np.float64).reshape(4, 3).T
+                A, tk = k[:, :3], k[:, 3]
+            m = compose_frame_edit(T, A, tk, float(self.model_scale[0]))
+        ts = np.ascontiguousarray(m.T.reshape(12), dtype=np.float32)
+        _lib.check(_lib.lib().gsr_transform_selection(self._ctx, ts.ctypes.data_as(C.POINTER(C.c_float)),
+                                                      None if snapshot_ptr is None else C.c_void_p(snapshot_ptr)), "gsr_transform_selection")
+
+    def splat_store_bytes(self) -> int:
+        return int(_lib.lib().gsr_splat_store_bytes(self._ctx))
+
+    def copy_splat_store(self, ptr: int) -> None:
+        """Snapshot the whole store into device or page-locked host memory of splat_store_bytes() bytes (enqueued; no host sync)."""
+        _lib.check(_lib.lib().gsr_copy_splat_store(self._ctx, C.c_void_p(ptr)), "gsr_copy_splat_store")
+
+    def restore_splat_store(self, ptr: int) -> None:
+        """Write a snapshot of copy_splat_store back (undo of an edit, together with set_splat_masks)."""
+        _lib.check(_lib.lib().gsr_restore_splat_store(self._ctx, C.c_void_p(ptr)), "gsr_restore_splat_store")
+
+    def kept_table(self) -> np.ndarray:
+        """The edited cloud as a float32 3DGS vertex table (degree_properties of the store's degree, normals 0): the splats of
+        [0, num_splats) whose hidden bit is 0, read from the device store (synchronises).  PlyFile.from_array(table).save(path) writes
+        it."""
+        stride = self._plane_stride()
+        store = np.empty((self.splat_store_bytes() // (16 * stride), stride, 4), dtype=np.float32)
+        self.copy_splat_store(store.ctypes.data)   # pageable memory: the copy has landed when the call returns
+        n = int(self.stats().num_splats)
+        hidden, _ = self.splat_masks()
+        bands = self._sh_bands if self._sh_bands else 4
+        return store_to_table(store, n, bands, bool(self._flags & _lib.GSR_FLAG_SH_HALF), hidden[:n])
+
+    def _plane_stride(self) -> int:
+        return (self._max_splats + 255) // 256 * 256
+
     def render_raw(self, vp32: np.ndarray, uniforms32: bytes, heatmap: float = 0.0, host_ptr: int | None = None,
                    asynchronous: bool = True, rgb_only: bool = False, out_format: int | None = None) -> None:
         """rasterize() with pre-packed push constants / uniform block (bench hot loop).  out_format: GSR_OUT_* of the host frame
@@ -604,6 +653,95 @@ def godot_to_frame(transform, basis_override) -> np.ndarray:
     Fb[:3, :3] = np.diag([-1.0, -1.0, 1.0]) @ np.asarray(basis_override, dtype=np.float64).T
     M = np.eye(4) + Fb @ D @ np.linalg.inv(Fb)
     return M[:3].astype(np.float32)
+
+
+def compose_frame_edit(transform, A, t_k, model_scale: float) -> np.ndarray:
+    """The source-space [L | t] (3, 4) float32 of a frame-space edit [B | u] of the splats an instance with to_frame [A | t_k] draws:
+    it moves frame position A (x * model_scale) + t_k to B (that) + u, so L = A^-1 B A and t = A^-1 (B t_k + u - t_k) / model_scale.
+    Composed in float64 and narrowed once."""
+    T = np.asarray(transform, dtype=np.float64)
+    B, u = T[:, :3], T[:, 3]
+    A, t_k = np.asarray(A, dtype=np.float64), np.asarray(t_k, dtype=np.float64)
+    Ai = np.linalg.inv(A)
+    out = np.empty((3, 4))
+    out[:, :3] = Ai @ B @ A
+    out[:, 3] = Ai @ (B @ t_k + u - t_k) / model_scale
+    return out.astype(np.float32)
+
+
+# logits beyond +-104 give a stored opacity of exactly 0 or 1 in float32, so the export clamps there (a finite PLY value)
+_LOGIT_LIMIT = 104.0
+
+
+def store_to_table(store, n: int, bands: int, half: bool, hidden=None) -> np.ndarray:
+    """A store in the layout of GSR_BUF_SPLATS ((planes, plane_stride, 4) float32) -> the float32 3DGS vertex table of its first n
+    splats minus the hidden ones, in degree_properties(bands - 1) order with normals 0: the inverse of the ingest (ply_to_soa), in
+    float64.  Covariance: eigh(S) = V diag(l) V^T, a column of V flipped when det V < 0, rot = (w, x, y, z) of the rotation V,
+    scale_i = log(max(l_i, tiny)) / 2.  Opacity: the logit, clamped to +-104.  Positions and coefficients as stored (binary16 widened),
+    f_rest channel-major.  A Mip-Splatting filter is folded into the stored splat already, so no filter_3D property is written."""
+    from .ply_file import degree_properties
+    s = np.asarray(store, dtype=np.float32)
+    keep = np.ones(n, dtype=bool) if hidden is None else ~np.asarray(hidden, dtype=bool)[:n]
+    idx = np.flatnonzero(keep)
+    m = idx.size
+    p0, p1, p2 = s[0, idx].astype(np.float64), s[1, idx].astype(np.float64), s[2, idx].astype(np.float64)
+    K = bands * bands
+    P = (3 * K + 7) // 8 if half else (3 * K + 3) // 4
+    raw = np.ascontiguousarray(s[3:3 + P, idx].transpose(1, 0, 2)).reshape(m, 4 * P)
+    if half:
+        w = raw.view(np.uint32)
+        c = np.stack([w & 0xFFFF, w >> 16], axis=2).reshape(m, 8 * P).astype(np.uint16).view(np.float16).astype(np.float32)
+    else:
+        c = raw.copy()
+    c = c[:, :3 * K].reshape(m, K, 3)
+    S = np.empty((m, 3, 3))
+    S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1] = p1[:, 0], p1[:, 1], p1[:, 2], p1[:, 3]
+    S[:, 1, 2], S[:, 2, 2] = p2[:, 0], p2[:, 1]
+    S[:, 1, 0], S[:, 2, 0], S[:, 2, 1] = S[:, 0, 1], S[:, 0, 2], S[:, 1, 2]
+    lam, V = np.linalg.eigh(S)
+    V[np.linalg.det(V) < 0, :, 0] *= -1.0
+    with np.errstate(divide="ignore", invalid="ignore"):
+        scale = 0.5 * np.log(np.maximum(lam, np.finfo(np.float64).tiny))
+        o = p2[:, 2]
+        logit = np.clip(np.log(o) - np.log1p(-o), -_LOGIT_LIMIT, _LOGIT_LIMIT)
+    logit = np.where(np.isnan(logit), 0.0, logit)
+    names = degree_properties(bands - 1)
+    out = np.zeros((m, len(names)), dtype=np.float32)
+    col = {name: i for i, name in enumerate(names)}
+    out[:, 0:3] = s[0, idx, 0:3]
+    out[:, col["f_dc_0"]:col["f_dc_0"] + 3] = c[:, 0, :]
+    if K > 1:
+        out[:, col["f_rest_0"]:col["f_rest_0"] + 3 * (K - 1)] = c[:, 1:, :].transpose(0, 2, 1).reshape(m, 3 * (K - 1))
+    out[:, col["opacity"]] = logit
+    out[:, col["scale_0"]:col["scale_0"] + 3] = scale
+    out[:, col["rot_0"]:col["rot_0"] + 4] = rotation_quaternion(V)
+    return out
+
+
+def rotation_quaternion(R) -> np.ndarray:
+    """(m, 3, 3) proper rotations -> (m, 4) unit quaternions (w, x, y, z), float64 (Shepperd's method: the largest of w, x, y, z first)."""
+    R = np.asarray(R, dtype=np.float64)
+    tr = R[:, 0, 0] + R[:, 1, 1] + R[:, 2, 2]
+    cand = np.stack([tr, R[:, 0, 0], R[:, 1, 1], R[:, 2, 2]], axis=1)
+    k = np.argmax(cand, axis=1)
+    q = np.empty((R.shape[0], 4))
+    for i in range(4):
+        sel = k == i
+        r = R[sel]
+        if i == 0:
+            w = 0.5 * np.sqrt(1.0 + tr[sel])
+            f = 0.25 / w
+            q[sel] = np.stack([w, (r[:, 2, 1] - r[:, 1, 2]) * f, (r[:, 0, 2] - r[:, 2, 0]) * f, (r[:, 1, 0] - r[:, 0, 1]) * f], axis=1)
+        else:
+            a, b, cc = i - 1, i % 3, (i + 1) % 3
+            v = 0.5 * np.sqrt(1.0 + r[:, a, a] - r[:, b, b] - r[:, cc, cc])
+            f = 0.25 / v
+            xyz = np.empty((r.shape[0], 3))
+            xyz[:, a] = v
+            xyz[:, b] = (r[:, b, a] + r[:, a, b]) * f
+            xyz[:, cc] = (r[:, cc, a] + r[:, a, cc]) * f
+            q[sel] = np.concatenate([((r[:, cc, b] - r[:, b, cc]) * f)[:, None], xyz], axis=1)
+    return q
 
 
 def cutout_to_local(transform, basis_override) -> np.ndarray:

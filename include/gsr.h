@@ -97,8 +97,10 @@ enum {
                                            rounded up to 256 (gsr_config.sh_bands; 3 + P_h planes of binary16 SH with GSR_FLAG_SH_HALF) */
     GSR_BUF_DEPTH_WORDS_UNSORTED = 11,  /* gsr_set_depth_order: the last mode-1 frame's ord(d) per pair in emission order, M entries
                                            (kept with gsr_debug_keep_unsorted once mode 1 has been switched on) */
-    GSR_BUF_INSTANCE_APPEARANCE = 12    /* gsr_set_instance_appearance: one gsr_instance_appearance per instance as stored (the default
+    GSR_BUF_INSTANCE_APPEARANCE = 12,   /* gsr_set_instance_appearance: one gsr_instance_appearance per instance as stored (the default
                                            when none was set) */
+    GSR_BUF_EDIT_TRANSFORM = 13         /* gsr_transform_selection: the last accepted call's to_source (12 floats), then M~_1, M~_2, M~_3
+                                           row-major (9 + 25 + 49): 95 floats, zeros before the first call */
 };
 
 typedef struct gsr_ctx gsr_ctx;       /* one rasterizer = one GaussianSplattingRasterizer instance */
@@ -576,8 +578,9 @@ GSR_API int gsr_set_cutouts(gsr_ctx *ctx, const gsr_cutout *cutouts, uint32_t n)
  *        enqueued.
  *      GSR_ERR_INVALID, previous state kept: an unknown op, an instance outside the current layout, n out of range, a non-finite vertex
  *      or to_local, an unknown shape or space, a rectangle outside the image, a NULL array, words != ceil(max_splats / 32), bits past
- *      max_splats, hidden and selected bits that overlap (gsr_set_splat_masks).  Export of the kept cloud: the rows of the source table
- *      whose hidden bit is 0. ---- */
+ *      max_splats, hidden and selected bits that overlap (gsr_set_splat_masks).  Export of the kept cloud: the stored splats whose hidden
+ *      bit is 0, read from the device with gsr_copy_splat_store (after gsr_transform_selection the host's source table is stale;
+ *      see "Splat transform edits"). ---- */
 #define GSR_MAX_SELECT_VERTICES 64
 #define GSR_SELECT_SET 0
 #define GSR_SELECT_ADD 1
@@ -595,6 +598,41 @@ GSR_API int gsr_get_splat_masks(gsr_ctx *ctx, uint32_t *hidden, uint32_t *select
 GSR_API int gsr_set_splat_masks(gsr_ctx *ctx, const uint32_t *hidden, const uint32_t *selected, uint64_t words);
 GSR_API int gsr_splat_mask_counts(gsr_ctx *ctx, uint64_t *selected, uint64_t *hidden);
 GSR_API int gsr_set_selection_style(gsr_ctx *ctx, const float rgb[3], float strength);
+
+/* ---- Splat transform edits: move, rotate, scale or mirror the selected splats in the store (no reference counterpart).
+ *      gsr_transform_selection rewrites, for every source splat whose `selected` bit is set when the operation runs, its stored planes
+ *      from `src_store`: NULL = the store itself, or a caller-owned device snapshot in the layout of gsr_copy_splat_store (a gizmo drag
+ *      re-applies a growing transform to the snapshot taken at mouse-down, so no rounding accumulates).  Unselected (and so hidden)
+ *      splats are never written, also with a snapshot.  to_source = [L | t], column-major 3x4, acts on the stored position (plane 0
+ *      xyz, before model_scale).  Per selected splat, in float32 with one rounding per operation and no contraction:
+ *        - position: x'[r] = ((L[r] x + L[3+r] y) + L[6+r] z) + L[9+r] (the instance formula: at model_scale 1 a whole-cloud edit
+ *          gives exactly the positions an instance with to_frame = [L | t] writes into its records);
+ *        - covariance: with S the symmetric matrix of the six stored words, G[r][c] = ((L[r] S[0][c] + L[3+r] S[1][c]) + L[6+r] S[2][c])
+ *          and S'[r][c] = ((G[r][0] L[c] + G[r][1] L[3+c]) + G[r][2] L[6+c]) for the six stored entries (r <= c);
+ *        - SH bands 1 .. B-1 of the store: Q = the orthogonal polar factor of L (U V^T of its SVD), in float64 on the host: the
+ *          rotation of a rigid or similarity L (improper for a reflection), and for other L the same approximation gsr_set_instances
+ *          makes for non-uniform scales.  P_l(d) = the 2l+1 polynomials that multiply coefficients l^2 .. l^2 + 2l in the projection's
+ *          SH evaluation, M_l the float64 matrix with P_l(Q^T d) = M_l P_l(d) for every d, and M~_l = M_l with entries below 1e-9 in
+ *          magnitude set to +0, rounded to float32 (the identity gives exactly I).  Per channel c'_j = (..((c_0 M~[0][j] + c_1 M~[1][j])
+ *          + c_2 M~[2][j]) ..), left to right over i.  With GSR_FLAG_SH_HALF c is the stored half widened (exact) and c' is stored as
+ *          h(c') (round to nearest even, +-65504 saturation, as at upload);
+ *        - copied bit for bit: plane-0 w (creation time), opacity, the plane-2 pad and the DC coefficients; the floats or half slots
+ *          past 3K stay +0.
+ *      A frame after an edit is the default frame of the edited cloud; an edit is not motion (like an upload): with a static camera and
+ *      unchanged instance transforms the frame after it has motion (0, 0).  GSR_ERR_INVALID, store unchanged: a NULL to_source, a
+ *      non-finite entry, det(L) (float64) 0 or not finite.  GSR_ERR_STATE while the splat masks are not in use (so never on a sharded
+ *      context).
+ *      gsr_splat_store_bytes: the byte size of GSR_BUF_SPLATS, (3 + P) planes x plane_stride x 16.  gsr_copy_splat_store copies the
+ *      whole store to dst in that layout, gsr_restore_splat_store writes it back from src; both use cudaMemcpyDefault, so dst / src may
+ *      be device or page-locked host memory (pageable memory makes the copy synchronous), and both are allowed on any context.
+ *      Ordering of all three: after everything enqueued before on the context's streams (the render stream, and the front stream under
+ *      gsr_debug_pipeline(ctx, 1), including the previous frame's compositor), before the projection of every frame enqueued after
+ *      it; none synchronises the host.  Undo of an edit is exact: restore the snapshot taken before it, and the masks with
+ *      gsr_set_splat_masks. ---- */
+GSR_API int gsr_transform_selection(gsr_ctx *ctx, const float to_source[12], const void *src_store);
+GSR_API uint64_t gsr_splat_store_bytes(gsr_ctx *ctx);
+GSR_API int gsr_copy_splat_store(gsr_ctx *ctx, void *dst);
+GSR_API int gsr_restore_splat_store(gsr_ctx *ctx, const void *src);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
