@@ -17,7 +17,7 @@ GSR_FLAG_ORTHOGRAPHIC = 0x20
 GSR_FLAG_SH_HALF = 0x40   # SH coefficients stored as IEEE binary16 (include/gsr.h)
 (GSR_BUF_RECORDS, GSR_BUF_KEYS, GSR_BUF_VALUES, GSR_BUF_BOUNDS, GSR_BUF_KEYS_UNSORTED, GSR_BUF_VALUES_UNSORTED,
  GSR_BUF_FRAMEBUFFER, GSR_BUF_COMPOSITOR_TRACE, GSR_BUF_COMPOSITOR_TRACE_COUNT, GSR_BUF_INSTANCES, GSR_BUF_SPLATS, GSR_BUF_DEPTH_WORDS_UNSORTED,
- GSR_BUF_INSTANCE_APPEARANCE, GSR_BUF_EDIT_TRANSFORM) = range(14)
+ GSR_BUF_INSTANCE_APPEARANCE, GSR_BUF_EDIT_TRANSFORM, GSR_BUF_EDIT_COLOR) = range(15)
 GSR_DEPTH_ORDER_KEY16, GSR_DEPTH_ORDER_VIEW_DEPTH = 0, 1
 GSR_MAX_CUTOUTS = 16
 GSR_CUTOUT_BOX, GSR_CUTOUT_ELLIPSOID = 0, 1
@@ -38,7 +38,7 @@ EXPORTS = [
     "gsr_set_depth_compositing", "gsr_set_motion_vectors", "gsr_reset_motion", "gsr_set_splat_ids", "gsr_set_instances", "gsr_set_instance_appearance", "gsr_set_sh_degree", "gsr_set_antialiasing", "gsr_set_depth_order", "gsr_set_cutouts", "gsr_upload_ply_filtered", "gsr_pick",
     "gsr_select_all", "gsr_select_polygon", "gsr_select_volume", "gsr_select_ids", "gsr_hide_selection", "gsr_unhide_all", "gsr_clear_splat_masks",
     "gsr_get_splat_masks", "gsr_set_splat_masks", "gsr_splat_mask_counts", "gsr_set_selection_style",
-    "gsr_transform_selection", "gsr_splat_store_bytes", "gsr_copy_splat_store", "gsr_restore_splat_store",
+    "gsr_transform_selection", "gsr_splat_store_bytes", "gsr_copy_splat_store", "gsr_restore_splat_store", "gsr_recolor_selection",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -68,6 +68,10 @@ class GsrInstance(C.Structure):
 
 class GsrInstanceAppearance(C.Structure):
     _fields_ = [("tint", C.c_float * 3), ("opacity", C.c_float), ("draw_count", C.c_uint64)]
+
+
+class GsrColorEdit(C.Structure):
+    _fields_ = [("matrix", C.c_float * 12), ("band_scale", C.c_float * 3), ("opacity_scale", C.c_float), ("opacity_offset", C.c_float)]
 
 
 class GsrCutout(C.Structure):
@@ -160,6 +164,7 @@ def lib():
         L.gsr_splat_mask_counts.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
         L.gsr_set_selection_style.argtypes = [vp, fp, C.c_float]
         L.gsr_transform_selection.argtypes = [vp, fp, vp]
+        L.gsr_recolor_selection.argtypes = [vp, C.POINTER(GsrColorEdit), vp]
         L.gsr_splat_store_bytes.argtypes = [vp]
         L.gsr_splat_store_bytes.restype = u64
         L.gsr_copy_splat_store.argtypes = [vp, vp]

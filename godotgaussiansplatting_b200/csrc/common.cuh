@@ -24,6 +24,8 @@ __host__ __device__ constexpr int sh_planes(int bands, bool half = false) { retu
 __host__ __device__ constexpr int soa_planes(int bands, bool half = false) { return 3 + sh_planes(bands, half); }
 static_assert(soa_planes(SH_BANDS_MAX) == NUM_PLANES, "a degree-3 store is the 60-float Splat");
 static_assert(soa_planes(SH_BANDS_MAX, true) * 16 == 144, "a degree-3 binary16 store is 144 B per splat");
+// The DC factor of the projection's SH colour, colour = 0.5 + SH_C0 c_0 + ... (also the colour edits' host constants)
+constexpr float SH_C0 = 0.28209479177387814f;
 
 // binary16 SH store: h(c) = c rounded to binary16 (round to nearest even, subnormals and signed zeros kept); finite or infinite values
 // beyond +-65504 saturate to +-65504, NaN stays a NaN.  The decode of a half is exact.
@@ -333,6 +335,24 @@ struct TransformArgs {
 };
 // Rewrites every selected splat of the store from `src` (store bands and format as given).
 int launch_transform_selection(const TransformArgs &a, int bands, bool sh_half, cudaStream_t stream);
+
+// ---- selection colour edits (gsr_recolor_selection; selection.cu) ----
+// The operation's constants: A (3x3 row-major), d (3), N~_1, N~_2, N~_3 (3x3 row-major each), s, t: 41 floats, the layout of
+// GSR_BUF_EDIT_COLOR.
+constexpr int EDIT_COLOR_D = 9, EDIT_COLOR_S = 39, EDIT_COLOR_FLOATS = 41;
+__host__ __device__ constexpr int edit_color_band_offset(int l) { return 12 + 9 * (l - 1); }   // N~_l, l = 1..3
+// Host, float64: the 41 floats of a validated edit (the caller checks the fields).
+void edit_color_constants(const gsr_color_edit *e, float out[EDIT_COLOR_FLOATS]);
+struct RecolorArgs {
+    float4 *dst;               // the store
+    const float4 *src;         // the store itself, or a snapshot in its layout
+    uint64_t plane_stride;
+    const uint32_t *selected;
+    uint32_t words;
+    float k[EDIT_COLOR_FLOATS];
+};
+// Rewrites the SH coefficients and opacity of every selected splat of the store from `src` (store bands and format as given).
+int launch_recolor_selection(const RecolorArgs &a, int bands, bool sh_half, cudaStream_t stream);
 
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.

@@ -56,8 +56,9 @@ struct gsr_ctx {
         float rgb[3] = {1.0f, 0.5f, 0.0f};
         float strength = 0.5f;
     } masks;
-    // store edits and snapshots (gsr_transform_selection, gsr_copy_splat_store, gsr_restore_splat_store)
+    // store edits and snapshots (gsr_transform_selection, gsr_recolor_selection, gsr_copy_splat_store, gsr_restore_splat_store)
     float edit_last[EDIT_TRANSFORM_FLOATS] = {};   // GSR_BUF_EDIT_TRANSFORM: the constants of the last accepted transform
+    float color_last[EDIT_COLOR_FLOATS] = {};      // GSR_BUF_EDIT_COLOR: the constants of the last accepted colour edit
     cudaEvent_t store_ready = nullptr;             // with front / back overlap: the render stream's work enqueued before the operation
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
@@ -1935,7 +1936,7 @@ GSR_API int gsr_set_selection_style(gsr_ctx *c, const float rgb[3], float streng
     return GSR_OK;
 }
 
-// ---- splat transform edits and store snapshots ------------------------------------------------------------------------------------
+// ---- splat transform and colour edits, store snapshots ---------------------------------------------------------------------------
 // Enqueued on the projections' stream (mask_stream) like the mask operations, so they come before the projections of later frames.
 // Unlike them they also wait for the render stream's work: the previous frame's compositor reads plane 0 for the motion vectors of
 // instanced frames.
@@ -1971,6 +1972,33 @@ GSR_API int gsr_transform_selection(gsr_ctx *c, const float to_source[12], const
     a.words = c->masks.words;
     if ((rc = launch_transform_selection(a, c->sh_bands, sh_half(c), s))) return rc;
     memcpy(c->edit_last, a.m, sizeof c->edit_last);
+    return GSR_OK;
+}
+
+GSR_API int gsr_recolor_selection(gsr_ctx *c, const gsr_color_edit *e, const void *src_store) {
+    if (!c || !e) { set_last_error("gsr_recolor_selection: NULL argument"); return GSR_ERR_INVALID; }
+    for (int i = 0; i < 12; ++i) {
+        if (!(fabsf(e->matrix[i]) <= GSR_TINT_MAX)) { set_last_error("gsr_recolor_selection: matrix[%d] = %g not finite or beyond GSR_TINT_MAX", i, (double)e->matrix[i]); return GSR_ERR_INVALID; }
+    }
+    for (int l = 0; l < 3; ++l) {
+        if (!(e->band_scale[l] >= 0.0f && e->band_scale[l] <= GSR_TINT_MAX)) { set_last_error("gsr_recolor_selection: band_scale[%d] = %g outside [0, GSR_TINT_MAX]", l, (double)e->band_scale[l]); return GSR_ERR_INVALID; }
+    }
+    if (!(e->opacity_scale >= 0.0f && e->opacity_scale <= GSR_TINT_MAX)) { set_last_error("gsr_recolor_selection: opacity_scale = %g outside [0, GSR_TINT_MAX]", (double)e->opacity_scale); return GSR_ERR_INVALID; }
+    if (!(e->opacity_offset >= -1.0f && e->opacity_offset <= 1.0f)) { set_last_error("gsr_recolor_selection: opacity_offset = %g outside [-1, 1]", (double)e->opacity_offset); return GSR_ERR_INVALID; }
+    if (!c->masks.on) { set_last_error("gsr_recolor_selection: the splat masks are not in use"); return GSR_ERR_STATE; }
+    RecolorArgs a;
+    edit_color_constants(e, a.k);
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    cudaStream_t s;
+    if ((rc = store_stream(c, &s))) return rc;
+    a.dst = c->soa;
+    a.src = src_store ? static_cast<const float4 *>(src_store) : c->soa;
+    a.plane_stride = c->plane_stride;
+    a.selected = c->masks.selected;
+    a.words = c->masks.words;
+    if ((rc = launch_recolor_selection(a, c->sh_bands, sh_half(c), s))) return rc;
+    memcpy(c->color_last, a.k, sizeof c->color_last);
     return GSR_OK;
 }
 
@@ -2148,6 +2176,12 @@ GSR_API int gsr_debug_copy(gsr_ctx *c, int which, void *dst, size_t bytes) {
             avail = sizeof c->edit_last;
             if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }
             memcpy(dst, c->edit_last, bytes);
+            return GSR_OK;
+        }
+        case GSR_BUF_EDIT_COLOR: {   // host copy: no device involved
+            avail = sizeof c->color_last;
+            if (bytes > avail) { set_last_error("gsr_debug_copy(%d): %zu bytes requested, %zu available", which, bytes, avail); return GSR_ERR_INVALID; }
+            memcpy(dst, c->color_last, bytes);
             return GSR_OK;
         }
         case GSR_BUF_INSTANCE_APPEARANCE: {   // host copy: no device involved

@@ -21,7 +21,6 @@ namespace gsr {
 
 namespace {
 
-constexpr float SH_C0 = 0.28209479177387814f;
 constexpr float SH_C1 = 0.4886025119029199f;
 constexpr float SH_C2_0 = 1.0925484305920792f;
 constexpr float SH_C2_1 = 1.0925484305920792f;

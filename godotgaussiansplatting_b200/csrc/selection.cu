@@ -147,6 +147,53 @@ __global__ void __launch_bounds__(SEL_THREADS) mask_counts_kernel(const uint32_t
     }
 }
 
+// The SH planes of one splat in the edit kernels: `src` / `dst` point at plane 0 of the splat, P = sh_planes(BANDS, HALF) planes follow
+// plane 2.  Unpack: every stored value into c[] (a binary16 half widened, which is exact), and the raw words holding binary16 values 0-3.
+template <int BANDS, bool HALF>
+__device__ __forceinline__ void sh_unpack(const float4 *src, uint64_t st, float (&c)[HALF ? 8 * sh_planes(BANDS, HALF) : 4 * sh_planes(BANDS, HALF)],
+                                          uint32_t (&dc_words)[2]) {
+    constexpr int P = sh_planes(BANDS, HALF);
+#pragma unroll
+    for (int k = 0; k < P; ++k) {
+        const float4 v = src[(uint64_t)(3 + k) * st];
+        if constexpr (HALF) {
+            const uint32_t u[4] = {__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
+            if (k == 0) { dc_words[0] = u[0]; dc_words[1] = u[1]; }
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                c[8 * k + 2 * j] = half_bits_to_float(u[j] & 0xFFFFu);
+                c[8 * k + 2 * j + 1] = half_bits_to_float(u[j] >> 16);
+            }
+        } else {
+            c[4 * k + 0] = v.x; c[4 * k + 1] = v.y; c[4 * k + 2] = v.z; c[4 * k + 3] = v.w;
+        }
+    }
+}
+
+// Pack: c[] back into the planes, binary16 values as h(c) (sh_half: the upload's rounding), the slots past 3K +0.  KEEP_DC: a binary16
+// store's DC halves are written from dc_words as they were stored (a float store's DC values are c[0..2] either way).
+template <int BANDS, bool HALF, bool KEEP_DC>
+__device__ __forceinline__ void sh_pack(float4 *dst, uint64_t st, const float (&c)[HALF ? 8 * sh_planes(BANDS, HALF) : 4 * sh_planes(BANDS, HALF)],
+                                        const uint32_t (&dc_words)[2]) {
+    constexpr int NV = 3 * sh_coeffs(BANDS), P = sh_planes(BANDS, HALF), DC = KEEP_DC ? 3 : 0;
+#pragma unroll
+    for (int k = 0; k < P; ++k) {
+        uint32_t u[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if constexpr (HALF) {
+                const int i = 8 * k + 2 * j;
+                const uint32_t lo = i < DC ? (dc_words[i >> 1] & 0xFFFFu) : i < NV ? sh_half(c[i]) : 0u;
+                const uint32_t hi = i + 1 < DC ? (dc_words[(i + 1) >> 1] >> 16) : i + 1 < NV ? sh_half(c[i + 1]) : 0u;
+                u[j] = lo | (hi << 16);
+            } else {
+                u[j] = 4 * k + j < NV ? __float_as_uint(c[4 * k + j]) : 0u;
+            }
+        }
+        dst[(uint64_t)(3 + k) * st] = make_float4(__uint_as_float(u[0]), __uint_as_float(u[1]), __uint_as_float(u[2]), __uint_as_float(u[3]));
+    }
+}
+
 // gsr_transform_selection: every selected splat s of the store is rewritten from its planes in `src` (include/gsr.h "Splat transform
 // edits").  Like the region kernels a warp owns one mask word: a warp whose word is 0 leaves after that one load, and the lanes of a
 // selected warp read consecutive 16-byte words of every plane.  Unselected splats are never written (a hidden splat is never selected).
@@ -186,24 +233,10 @@ __global__ void __launch_bounds__(SEL_THREADS) transform_selection_kernel(const 
     dst[st] = make_float4(E[0][0], E[0][1], E[0][2], E[1][1]);
     dst[2 * st] = make_float4(E[1][2], E[2][2], p2.z, p2.w);
 
-    constexpr int NV = 3 * sh_coeffs(BANDS), P = sh_planes(BANDS, HALF);
+    constexpr int P = sh_planes(BANDS, HALF);
     float c[HALF ? 8 * P : 4 * P];
     uint32_t dc_words[2] = {0u, 0u};   // binary16: the words holding values 0-3 (the DC halves are copied as stored)
-#pragma unroll
-    for (int k = 0; k < P; ++k) {
-        const float4 v = src[(uint64_t)(3 + k) * st];
-        if constexpr (HALF) {
-            const uint32_t u[4] = {__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
-            if (k == 0) { dc_words[0] = u[0]; dc_words[1] = u[1]; }
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                c[8 * k + 2 * j] = half_bits_to_float(u[j] & 0xFFFFu);
-                c[8 * k + 2 * j + 1] = half_bits_to_float(u[j] >> 16);
-            }
-        } else {
-            c[4 * k + 0] = v.x; c[4 * k + 1] = v.y; c[4 * k + 2] = v.z; c[4 * k + 3] = v.w;
-        }
-    }
+    sh_unpack<BANDS, HALF>(src, st, c, dc_words);
 #pragma unroll
     for (int l = 1; l < BANDS; ++l) {
         const int n = 2 * l + 1, k0 = l * l;
@@ -222,22 +255,48 @@ __global__ void __launch_bounds__(SEL_THREADS) transform_selection_kernel(const 
             }
         }
     }
-#pragma unroll
-    for (int k = 0; k < P; ++k) {
-        uint32_t u[4];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            if constexpr (HALF) {
-                const int i = 8 * k + 2 * j;
-                const uint32_t lo = i < 3 ? (dc_words[i >> 1] & 0xFFFFu) : i < NV ? sh_half(c[i]) : 0u;
-                const uint32_t hi = i + 1 < 3 ? (dc_words[(i + 1) >> 1] >> 16) : i + 1 < NV ? sh_half(c[i + 1]) : 0u;
-                u[j] = lo | (hi << 16);
-            } else {
-                u[j] = 4 * k + j < NV ? __float_as_uint(c[4 * k + j]) : 0u;
-            }
-        }
-        dst[(uint64_t)(3 + k) * st] = make_float4(__uint_as_float(u[0]), __uint_as_float(u[1]), __uint_as_float(u[2]), __uint_as_float(u[3]));
+    sh_pack<BANDS, HALF, true>(dst, st, c, dc_words);
+}
+
+// gsr_recolor_selection: every selected splat s of the store is rewritten from its planes in `src` (include/gsr.h "Splat colour
+// edits"), with the skeleton of transform_selection_kernel.  In float32, one rounding per operation, no contraction, per coefficient k
+// (an RGB triple c): DC c'_i = ((A[i][0] c_r + A[i][1] c_g) + A[i][2] c_b) + d_i, band l >= 1 the same without d and with N~_l for A;
+// opacity u = (o s) + t, o' = 1 above 1, u above 0, else +0 (NaN included).  Planes 0-1, plane-2 x, y, w copied bit for bit (in place
+// planes 0-1 are neither read nor written), slots past 3K +0.
+template <int BANDS, bool HALF>
+__global__ void __launch_bounds__(SEL_THREADS) recolor_selection_kernel(const __grid_constant__ RecolorArgs a) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t w = blockIdx.x * SEL_WARPS + (threadIdx.x >> 5);
+    if (w >= a.words) return;   // warp-uniform
+    const uint32_t word = a.selected[w];
+    if (((word >> lane) & 1u) == 0u) return;
+    const uint64_t s = 32ull * w + lane, st = a.plane_stride;
+    const float4 *src = a.src + s;
+    float4 *dst = a.dst + s;
+    if (a.src != a.dst) {   // uniform: from a snapshot
+        dst[0] = src[0];
+        dst[st] = src[st];
     }
+    float4 p2 = src[2 * st];
+    const float u = __fadd_rn(__fmul_rn(p2.z, a.k[EDIT_COLOR_S]), a.k[EDIT_COLOR_S + 1]);
+    p2.z = u > 1.0f ? 1.0f : (u > 0.0f ? u : 0.0f);
+    dst[2 * st] = p2;
+
+    constexpr int K = sh_coeffs(BANDS), P = sh_planes(BANDS, HALF);
+    float c[HALF ? 8 * P : 4 * P];
+    uint32_t dc_words[2] = {0u, 0u};   // not used: the DC halves are edited
+    sh_unpack<BANDS, HALF>(src, st, c, dc_words);
+#pragma unroll
+    for (int k = 0; k < K; ++k) {
+        const float *M = a.k + (k == 0 ? 0 : edit_color_band_offset(k < 4 ? 1 : k < 9 ? 2 : 3));
+        const float r = c[3 * k], g = c[3 * k + 1], b = c[3 * k + 2];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+            const float v = __fadd_rn(__fadd_rn(__fmul_rn(M[3 * i], r), __fmul_rn(M[3 * i + 1], g)), __fmul_rn(M[3 * i + 2], b));
+            c[3 * k + i] = k == 0 ? __fadd_rn(v, a.k[EDIT_COLOR_D + i]) : v;
+        }
+    }
+    sh_pack<BANDS, HALF, false>(dst, st, c, dc_words);
 }
 
 }  // namespace
@@ -362,6 +421,23 @@ int edit_transform_matrices(const float to_source[12], float out[EDIT_TRANSFORM_
     return GSR_OK;
 }
 
+// The 41 floats of gsr_recolor_selection, each computed in float64 from the float inputs and rounded to float32 once: A row-major,
+// d_i = ((((A[i][0] / 2 + A[i][1] / 2) + A[i][2] / 2) + b_i) - 1/2) / C0 with C0 the projection's SH_C0, N~_l = band_scale[l-1] A (the
+// double product of two floats is exact), s, t.  colour' = A colour + b on 0.5 + C0 c_0 + sum_k P_k(d) c_k is c_0' = A c_0 + d and
+// c_k' = A c_k: every such map is an exact map of the coefficients.
+void edit_color_constants(const gsr_color_edit *e, float out[EDIT_COLOR_FLOATS]) {
+    const double c0 = (double)SH_C0;
+    for (int i = 0; i < 3; ++i) {
+        const double A0 = e->matrix[i], A1 = e->matrix[3 + i], A2 = e->matrix[6 + i];
+        out[3 * i] = (float)A0; out[3 * i + 1] = (float)A1; out[3 * i + 2] = (float)A2;
+        out[EDIT_COLOR_D + i] = (float)(((((A0 * 0.5 + A1 * 0.5) + A2 * 0.5) + (double)e->matrix[9 + i]) - 0.5) / c0);
+        for (int l = 1; l <= 3; ++l)
+            for (int j = 0; j < 3; ++j) out[edit_color_band_offset(l) + 3 * i + j] = (float)((double)e->band_scale[l - 1] * (double)e->matrix[3 * j + i]);
+    }
+    out[EDIT_COLOR_S] = e->opacity_scale;
+    out[EDIT_COLOR_S + 1] = e->opacity_offset;
+}
+
 #ifndef GSR_CPU_EMU
 namespace {
 uint32_t word_blocks(uint32_t words) { return (words + SEL_THREADS - 1) / SEL_THREADS; }
@@ -384,6 +460,30 @@ int launch_transform_selection(const TransformArgs &a, int bands, bool sh_half, 
         case 7: launch_transform_variant<3, true>(a, blocks, stream); break;
         case 8: launch_transform_variant<4, false>(a, blocks, stream); break;
         default: launch_transform_variant<4, true>(a, blocks, stream); break;
+    }
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+namespace {
+template <int BANDS, bool HALF>
+void launch_recolor_variant(const RecolorArgs &a, uint32_t blocks, cudaStream_t stream) {
+    recolor_selection_kernel<BANDS, HALF><<<blocks, SEL_THREADS, 0, stream>>>(a);
+}
+}  // namespace
+
+int launch_recolor_selection(const RecolorArgs &a, int bands, bool sh_half, cudaStream_t stream) {
+    if (a.words == 0) return GSR_OK;
+    const uint32_t blocks = (a.words + SEL_WARPS - 1) / SEL_WARPS;
+    switch (bands * 2 + (sh_half ? 1 : 0)) {
+        case 2: launch_recolor_variant<1, false>(a, blocks, stream); break;
+        case 3: launch_recolor_variant<1, true>(a, blocks, stream); break;
+        case 4: launch_recolor_variant<2, false>(a, blocks, stream); break;
+        case 5: launch_recolor_variant<2, true>(a, blocks, stream); break;
+        case 6: launch_recolor_variant<3, false>(a, blocks, stream); break;
+        case 7: launch_recolor_variant<3, true>(a, blocks, stream); break;
+        case 8: launch_recolor_variant<4, false>(a, blocks, stream); break;
+        default: launch_recolor_variant<4, true>(a, blocks, stream); break;
     }
     GSR_CUDA_TRY(cudaGetLastError());
     return GSR_OK;
@@ -450,6 +550,14 @@ int preload_selection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<3, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<4, false>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, transform_selection_kernel<4, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<1, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<1, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<2, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<2, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<3, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<3, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<4, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<4, true>));
     return GSR_OK;
 }
 #endif  // GSR_CPU_EMU

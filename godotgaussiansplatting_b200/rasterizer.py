@@ -385,6 +385,13 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_transform_selection(self._ctx, ts.ctypes.data_as(C.POINTER(C.c_float)),
                                                       None if snapshot_ptr is None else C.c_void_p(snapshot_ptr)), "gsr_transform_selection")
 
+    def recolor_selection(self, edit: _lib.GsrColorEdit, snapshot_ptr: int | None = None) -> None:
+        """Recolour, fade or flatten the selected splats in the store (include/gsr.h "Splat colour edits"); color_edit() builds `edit`.
+        snapshot_ptr: a device snapshot from copy_splat_store to read instead of the store (a slider drag re-applies its growing edit
+        to the mouse-down state)."""
+        _lib.check(_lib.lib().gsr_recolor_selection(self._ctx, C.byref(edit), None if snapshot_ptr is None else C.c_void_p(snapshot_ptr)),
+                   "gsr_recolor_selection")
+
     def splat_store_bytes(self) -> int:
         return int(_lib.lib().gsr_splat_store_bytes(self._ctx))
 
@@ -667,6 +674,43 @@ def compose_frame_edit(transform, A, t_k, model_scale: float) -> np.ndarray:
     out[:, :3] = Ai @ B @ A
     out[:, 3] = Ai @ (B @ t_k + u - t_k) / model_scale
     return out.astype(np.float32)
+
+
+REC709_LUMA = (0.2126, 0.7152, 0.0722)
+
+
+def color_edit(gain=(1.0, 1.0, 1.0), brightness=0.0, contrast=1.0, saturation=1.0, hue=0.0, view_dependence=1.0, opacity=1.0,
+               opacity_offset=0.0) -> _lib.GsrColorEdit:
+    """The gsr_color_edit of a colour grade, composed in float64 in this order and narrowed once:
+      1. channel gain: colour * gain;
+      2. saturation: a lerp from the Rec. 709 luma grey (0.2126, 0.7152, 0.0722) . colour to the colour (0: grey, above 1: more
+         saturated);
+      3. hue: a rotation by `hue` degrees about the grey axis (1, 1, 1);
+      4. contrast about 0.5: (colour - 0.5) * contrast + 0.5;
+      5. brightness: + brightness.
+    view_dependence scales the view-dependent colour (SH bands 1-3; 0 flattens it); opacity and opacity_offset map the stored opacity
+    to clamp(o * opacity + opacity_offset, 0, 1).  The defaults give exactly the identity edit."""
+    M, b = np.eye(3), np.zeros(3)
+
+    def then(A, t):
+        nonlocal M, b
+        M, b = A @ M, A @ b + t
+
+    then(np.diag(np.asarray(gain, dtype=np.float64)), np.zeros(3))
+    s = float(saturation)
+    then(s * np.eye(3) + (1.0 - s) * np.outer(np.ones(3), REC709_LUMA), np.zeros(3))
+    a = np.deg2rad(float(hue))
+    k = np.ones(3) / np.sqrt(3.0)
+    K = np.array([[0.0, -k[2], k[1]], [k[2], 0.0, -k[0]], [-k[1], k[0], 0.0]])
+    then(np.cos(a) * np.eye(3) + np.sin(a) * K + (1.0 - np.cos(a)) * np.outer(k, k), np.zeros(3))
+    c = float(contrast)
+    then(c * np.eye(3), np.full(3, 0.5 * (1.0 - c)))
+    then(np.eye(3), np.full(3, float(brightness)))
+    e = _lib.GsrColorEdit()
+    e.matrix[:] = [float(np.float32(v)) for v in np.concatenate([M.T.reshape(9), b])]
+    e.band_scale[:] = [float(view_dependence)] * 3
+    e.opacity_scale, e.opacity_offset = float(opacity), float(opacity_offset)
+    return e
 
 
 # logits beyond +-104 give a stored opacity of exactly 0 or 1 in float32, so the export clamps there (a finite PLY value)

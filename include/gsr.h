@@ -99,8 +99,10 @@ enum {
                                            (kept with gsr_debug_keep_unsorted once mode 1 has been switched on) */
     GSR_BUF_INSTANCE_APPEARANCE = 12,   /* gsr_set_instance_appearance: one gsr_instance_appearance per instance as stored (the default
                                            when none was set) */
-    GSR_BUF_EDIT_TRANSFORM = 13         /* gsr_transform_selection: the last accepted call's to_source (12 floats), then M~_1, M~_2, M~_3
+    GSR_BUF_EDIT_TRANSFORM = 13,        /* gsr_transform_selection: the last accepted call's to_source (12 floats), then M~_1, M~_2, M~_3
                                            row-major (9 + 25 + 49): 95 floats, zeros before the first call */
+    GSR_BUF_EDIT_COLOR = 14             /* gsr_recolor_selection: the last accepted call's A (9 floats, row-major), d (3), N~_1, N~_2, N~_3
+                                           (27, row-major), s and t: 41 floats, zeros before the first call */
 };
 
 typedef struct gsr_ctx gsr_ctx;       /* one rasterizer = one GaussianSplattingRasterizer instance */
@@ -579,8 +581,8 @@ GSR_API int gsr_set_cutouts(gsr_ctx *ctx, const gsr_cutout *cutouts, uint32_t n)
  *      GSR_ERR_INVALID, previous state kept: an unknown op, an instance outside the current layout, n out of range, a non-finite vertex
  *      or to_local, an unknown shape or space, a rectangle outside the image, a NULL array, words != ceil(max_splats / 32), bits past
  *      max_splats, hidden and selected bits that overlap (gsr_set_splat_masks).  Export of the kept cloud: the stored splats whose hidden
- *      bit is 0, read from the device with gsr_copy_splat_store (after gsr_transform_selection the host's source table is stale;
- *      see "Splat transform edits"). ---- */
+ *      bit is 0, read from the device with gsr_copy_splat_store (after gsr_transform_selection or gsr_recolor_selection the host's
+ *      source table is stale; see "Splat transform edits" and "Splat colour edits"). ---- */
 #define GSR_MAX_SELECT_VERTICES 64
 #define GSR_SELECT_SET 0
 #define GSR_SELECT_ADD 1
@@ -633,6 +635,43 @@ GSR_API int gsr_transform_selection(gsr_ctx *ctx, const float to_source[12], con
 GSR_API uint64_t gsr_splat_store_bytes(gsr_ctx *ctx);
 GSR_API int gsr_copy_splat_store(gsr_ctx *ctx, void *dst);
 GSR_API int gsr_restore_splat_store(gsr_ctx *ctx, const void *src);
+
+/* ---- Splat colour edits: recolour, fade or flatten the selected splats in the store (no reference counterpart).
+ *      gsr_recolor_selection rewrites, for every source splat whose `selected` bit is set when the operation runs, its SH coefficients
+ *      and opacity from `src_store`: NULL = the store itself, or a caller-owned device snapshot in the layout of gsr_copy_splat_store
+ *      (a colour-slider drag re-applies a growing edit to the snapshot taken at mouse-down, so no rounding accumulates).  Unselected
+ *      (and so hidden) splats are never written, also with a snapshot.  The edit covers all B stored bands, whatever gsr_set_sh_degree
+ *      renders.
+ *      Meaning: for every view direction, the selected splat's colour before the projection's clamp at 0 (0.5 + C0 c_0 + the
+ *      view-dependent terms) becomes A colour + b, up to float32 rounding, with the view-dependent share of band l scaled by
+ *      band_scale[l-1].  A channel that was clamped at 0 before the edit is edited from its unclamped value.
+ *      Constants, each computed in float64 from the float fields and rounded to float32 once: A[i][j] = matrix[3j + i];
+ *      d_i = ((((A[i][0] 0.5 + A[i][1] 0.5) + A[i][2] 0.5) + b_i) - 0.5) / C0 with C0 the projection's float SH_C0;
+ *      N~_l[i][j] = band_scale[l-1] A[i][j] (l = 1, 2, 3); s = opacity_scale, t = opacity_offset.
+ *      Per selected splat, in float32 with one rounding per operation and no contraction, for each stored coefficient k < K = B^2 with
+ *      c = (c_r, c_g, c_b) = values 3k .. 3k+2 (with GSR_FLAG_SH_HALF the stored halves widened, exact):
+ *        - k = 0: c'_i = (((A[i][0] c_r + A[i][1] c_g) + A[i][2] c_b) + d_i);
+ *        - k in band l >= 1: c'_i = ((N~_l[i][0] c_r + N~_l[i][1] c_g) + N~_l[i][2] c_b);
+ *        - with GSR_FLAG_SH_HALF c' is stored as h(c') (round to nearest even, +-65504 saturation, NaN stays NaN, as at upload);
+ *        - opacity (plane-2 z): u = (o s) + t, o' = u > 1 ? 1 : (u > 0 ? u : +0), so NaN, +-0 and negative values give +0;
+ *        - copied bit for bit: planes 0 and 1 (position, creation time, covariance), plane-2 x, y and w; the floats or half slots past
+ *          3K stay +0.
+ *      The identity edit ({I | 0}, {1, 1, 1}, 1, 0) leaves every stored word of finite coefficients unchanged, except that a -0
+ *      coefficient may become +0, so its frame is bit for bit the unedited frame (an infinite coefficient turns the other channels of
+ *      its triple NaN: 0 * inf).  A frame after an edit is the default frame of the edited cloud; an edit is not
+ *      motion.  Ordering as gsr_transform_selection: on the projections' stream after an event on the render stream, after everything
+ *      enqueued before and before the projection of every frame enqueued after it; it never synchronises the host.  Undo of an edit is
+ *      exact: restore the snapshot taken before it, then the masks with gsr_set_splat_masks.
+ *      GSR_ERR_INVALID, store unchanged: a NULL edit, a non-finite field, |A[i][j]| or |b_i| > GSR_TINT_MAX, a band_scale or
+ *      opacity_scale outside [0, GSR_TINT_MAX], opacity_offset outside [-1, 1].  The arguments are checked first; then GSR_ERR_STATE
+ *      while the splat masks are not in use (so never on a sharded context). ---- */
+typedef struct gsr_color_edit {
+    float matrix[12];       /* [A | b], column-major 3x4 like gsr_instance.to_frame: colour' = A colour + b, on the colour the
+                               projection evaluates before its clamp at 0 */
+    float band_scale[3];    /* further multiplies A for SH bands 1, 2, 3 (the view-dependent colour): 1 keeps it, 0 removes it */
+    float opacity_scale, opacity_offset;   /* stored opacity o' = clamp(o * scale + offset, 0, 1), rule above */
+} gsr_color_edit;           /* 68 bytes; identity = {I | 0}, {1, 1, 1}, 1, 0 */
+GSR_API int gsr_recolor_selection(gsr_ctx *ctx, const gsr_color_edit *edit, const void *src_store);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
