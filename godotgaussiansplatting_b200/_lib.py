@@ -39,6 +39,7 @@ EXPORTS = [
     "gsr_select_all", "gsr_select_polygon", "gsr_select_volume", "gsr_select_ids", "gsr_hide_selection", "gsr_unhide_all", "gsr_clear_splat_masks",
     "gsr_get_splat_masks", "gsr_set_splat_masks", "gsr_splat_mask_counts", "gsr_set_selection_style",
     "gsr_transform_selection", "gsr_splat_store_bytes", "gsr_copy_splat_store", "gsr_restore_splat_store", "gsr_recolor_selection",
+    "gsr_delete_hidden", "gsr_duplicate_selection", "gsr_set_splat_count",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -165,6 +166,9 @@ def lib():
         L.gsr_set_selection_style.argtypes = [vp, fp, C.c_float]
         L.gsr_transform_selection.argtypes = [vp, fp, vp]
         L.gsr_recolor_selection.argtypes = [vp, C.POINTER(GsrColorEdit), vp]
+        L.gsr_delete_hidden.argtypes = [vp, C.POINTER(u64)]
+        L.gsr_duplicate_selection.argtypes = [vp, C.POINTER(u64)]
+        L.gsr_set_splat_count.argtypes = [vp, u64]
         L.gsr_splat_store_bytes.argtypes = [vp]
         L.gsr_splat_store_bytes.restype = u64
         L.gsr_copy_splat_store.argtypes = [vp, vp]

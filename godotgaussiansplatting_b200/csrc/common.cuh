@@ -354,6 +354,34 @@ struct RecolorArgs {
 // Rewrites the SH coefficients and opacity of every selected splat of the store from `src` (store bands and format as given).
 int launch_recolor_selection(const RecolorArgs &a, int bands, bool sh_half, cudaStream_t stream);
 
+// ---- splat delete and duplicate (gsr_delete_hidden, gsr_duplicate_selection; selection.cu) ----
+// One pass of compact_store_kernel moves the planes of the splats of [0, n) whose bit is set (DELETE: hidden clear; DUPLICATE: selected
+// set) to prefix (DELETE, in place) or n + prefix (DUPLICATE), in order.  A CTA owns COMPACT_TILE_WORDS mask words (one splat per thread)
+// and takes its tile from an atomic ticket; its look-back status word (a 64-bit flag | count) and the ticket live in `lookback`.
+enum CompactMode { COMPACT_DELETE = 0, COMPACT_DUPLICATE = 1 };
+constexpr int COMPACT_THREADS = 256;
+constexpr uint32_t COMPACT_TILE_WORDS = COMPACT_THREADS / 32;
+// The look-back scratch of `words` mask words: one status word per tile, then the ticket.
+__host__ __device__ constexpr uint64_t compact_lookback_words(uint32_t words) { return (words + COMPACT_TILE_WORDS - 1) / COMPACT_TILE_WORDS + 1; }
+struct CompactArgs {
+    float4 *soa;
+    uint64_t plane_stride;
+    uint64_t n;                        // the cloud's size: the kernel reads mask words [0, ceil(n / 32)) and moves splats below n
+    const uint32_t *hidden, *selected;
+    uint32_t *sel_out;                 // DELETE: the moved splats' selected bits at their destinations, OR-ed into a zeroed scratch mask
+    unsigned long long *lookback;      // compact_lookback_words(ceil(n / 32)) words, zeroed before the launch
+    unsigned long long *total;         // the tile owning the last word writes the number of moved (DUPLICATE) or kept (DELETE) splats
+};
+// The launch covers every tile of [0, n); nothing is launched for n == 0.
+int launch_compact_store(const CompactArgs &a, int mode, int bands, bool sh_half, cudaStream_t stream);
+// After a delete that kept k of n splats: selected = scratch (then zeroed) and hidden = 0 over all `words`, slots [k, n) vacant.
+int launch_delete_finish(float4 *soa, uint64_t plane_stride, int planes, uint64_t k, uint64_t n, uint32_t *hidden, uint32_t *selected,
+                         uint32_t *scratch, uint32_t words, cudaStream_t stream);
+// After a duplicate of S splats behind n: selected = exactly [n, n + S), and hidden cleared there (the copies are not hidden).
+int launch_duplicate_finish(uint64_t n, uint64_t S, uint32_t *hidden, uint32_t *selected, uint32_t words, cudaStream_t stream);
+// counts[0] = popcount of the selected bits below n
+int launch_count_selected(const uint32_t *selected, uint64_t n, unsigned long long *counts, cudaStream_t stream);
+
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.
 __host__ __device__ __forceinline__ uint32_t depth_order_word(uint32_t bits) { return bits ^ ((bits >> 31) ? 0xFFFFFFFFu : 0x80000000u); }

@@ -45,13 +45,14 @@ struct gsr_ctx {
     float aa_variance = 0.0f;    // anti-aliasing filter of the next frames (gsr_set_antialiasing); 0 = off
     int32_t depth_order = GSR_DEPTH_ORDER_KEY16;   // sort order of the next frames (gsr_set_depth_order)
     CutoutArgs cutouts = {};     // cutout set of the next frames (gsr_set_cutouts), KEEP volumes first; none = off
-    // splat masks (gsr_select_*): one device allocation of [hidden | selected | scratch] words, then two 64-bit counters; allocated by
-    // the first call that can set a bit and kept until gsr_destroy.  on == false: not in use (the frames take their usual kernels).
+    // splat masks (gsr_select_*): one device allocation of [hidden | selected | scratch] words, then two 64-bit counters (and the
+    // look-back words of delete / duplicate); allocated by the first call that can set a bit and kept until gsr_destroy.  on == false: not in use (the frames take their usual kernels).
     struct Masks {
         bool on = false;
         uint32_t words = 0;               // ceil(max_splats / 32)
         uint32_t *hidden = nullptr, *selected = nullptr, *scratch = nullptr;
         unsigned long long *counts = nullptr;
+        unsigned long long *lookback = nullptr;   // gsr_delete_hidden / gsr_duplicate_selection: tile status words and ticket
         cudaEvent_t ids_ready = nullptr;  // gsr_select_ids with front / back overlap: the render stream's work that wrote the ID plane
         float rgb[3] = {1.0f, 0.5f, 0.0f};
         float strength = 0.5f;
@@ -1731,7 +1732,8 @@ static int masks_use(gsr_ctx *c, const char *where) {
     gsr_ctx::Masks &m = c->masks;
     if (!m.hidden) {
         const uint32_t words = (uint32_t)((c->max_splats + 31ull) / 32ull);
-        const size_t bytes = 2 * sizeof(unsigned long long) + sizeof(uint32_t) * 3ull * words;
+        const size_t mask_bytes = (2 * sizeof(unsigned long long) + sizeof(uint32_t) * 3ull * words + 7ull) & ~7ull;
+        const size_t bytes = mask_bytes + sizeof(unsigned long long) * compact_lookback_words(words);
         void *buf = nullptr;
         cudaEvent_t ev = nullptr;
         cudaError_t e = cudaMalloc(&buf, bytes);
@@ -1747,6 +1749,7 @@ static int masks_use(gsr_ctx *c, const char *where) {
         m.hidden = reinterpret_cast<uint32_t *>(m.counts + 2);
         m.selected = m.hidden + words;
         m.scratch = m.selected + words;
+        m.lookback = reinterpret_cast<unsigned long long *>(static_cast<char *>(buf) + mask_bytes);
         m.words = words;
         m.ids_ready = ev;
     }
@@ -1999,6 +2002,69 @@ GSR_API int gsr_recolor_selection(gsr_ctx *c, const gsr_color_edit *e, const voi
     a.words = c->masks.words;
     if ((rc = launch_recolor_selection(a, c->sh_bands, sh_half(c), s))) return rc;
     memcpy(c->color_last, a.k, sizeof c->color_last);
+    return GSR_OK;
+}
+
+// ---- splat delete and duplicate: structural edits of the store, enqueued like the edits above; each synchronises the host once ----
+GSR_API int gsr_delete_hidden(gsr_ctx *c, uint64_t *kept_out) {
+    if (!c || !kept_out) { set_last_error("gsr_delete_hidden: NULL argument"); return GSR_ERR_INVALID; }
+    if (!c->masks.on) { set_last_error("gsr_delete_hidden: the splat masks are not in use"); return GSR_ERR_STATE; }
+    if (c->inst.n > 0) { set_last_error("gsr_delete_hidden: instances are set (their ranges would point at other splats)"); return GSR_ERR_STATE; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    cudaStream_t s;
+    if ((rc = store_stream(c, &s))) return rc;
+    const uint64_t n = c->num_splats;
+    CompactArgs a;
+    a.soa = c->soa; a.plane_stride = c->plane_stride; a.n = n;
+    a.hidden = c->masks.hidden; a.selected = c->masks.selected; a.sel_out = c->masks.scratch;
+    a.lookback = c->masks.lookback; a.total = c->masks.counts;
+    GSR_CUDA_TRY(cudaMemsetAsync(c->masks.counts, 0, sizeof(unsigned long long), s));
+    if ((rc = launch_compact_store(a, COMPACT_DELETE, c->sh_bands, sh_half(c), s))) return rc;
+    unsigned long long k = 0ull;
+    GSR_CUDA_TRY(cudaMemcpyAsync(&k, c->masks.counts, sizeof k, cudaMemcpyDeviceToHost, s));
+    GSR_CUDA_TRY(cudaStreamSynchronize(s));
+    if ((rc = launch_delete_finish(c->soa, c->plane_stride, soa_planes(c->sh_bands, sh_half(c)), k, n, c->masks.hidden, c->masks.selected,
+                                   c->masks.scratch, c->masks.words, s))) return rc;
+    c->num_splats = k;
+    *kept_out = k;
+    return GSR_OK;
+}
+
+GSR_API int gsr_duplicate_selection(gsr_ctx *c, uint64_t *copies_out) {
+    if (!c || !copies_out) { set_last_error("gsr_duplicate_selection: NULL argument"); return GSR_ERR_INVALID; }
+    if (!c->masks.on) { set_last_error("gsr_duplicate_selection: the splat masks are not in use"); return GSR_ERR_STATE; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    cudaStream_t s;
+    if ((rc = store_stream(c, &s))) return rc;
+    const uint64_t n = c->num_splats;
+    if ((rc = launch_count_selected(c->masks.selected, n, c->masks.counts, s))) return rc;
+    unsigned long long S = 0ull;
+    GSR_CUDA_TRY(cudaMemcpyAsync(&S, c->masks.counts, sizeof S, cudaMemcpyDeviceToHost, s));
+    GSR_CUDA_TRY(cudaStreamSynchronize(s));
+    if (S > c->max_splats - n) {
+        set_last_error("gsr_duplicate_selection: %llu selected splats, room for %llu behind the cloud's %llu", S,
+                       (unsigned long long)(c->max_splats - n), (unsigned long long)n);
+        return GSR_ERR_INVALID;
+    }
+    if (S) {
+        CompactArgs a;
+        a.soa = c->soa; a.plane_stride = c->plane_stride; a.n = n;
+        a.hidden = c->masks.hidden; a.selected = c->masks.selected; a.sel_out = nullptr;
+        a.lookback = c->masks.lookback; a.total = c->masks.counts;
+        if ((rc = launch_compact_store(a, COMPACT_DUPLICATE, c->sh_bands, sh_half(c), s))) return rc;
+    }
+    if ((rc = launch_duplicate_finish(n, S, c->masks.hidden, c->masks.selected, c->masks.words, s))) return rc;
+    c->num_splats = n + S;
+    *copies_out = S;
+    return GSR_OK;
+}
+
+GSR_API int gsr_set_splat_count(gsr_ctx *c, uint64_t n) {
+    if (!c) return GSR_ERR_INVALID;
+    if (n > c->max_splats) { set_last_error("gsr_set_splat_count: %llu > max_splats %llu", (unsigned long long)n, (unsigned long long)c->max_splats); return GSR_ERR_INVALID; }
+    c->num_splats = n;
     return GSR_OK;
 }
 

@@ -4,7 +4,8 @@
 // one warp: lane l tests splat 32 w + l, a ballot forms the word's `inside` bits and lane 0 combines them with the word it owns, so no
 // update is atomic, even for an instance range that starts inside a word.  The grid covers every word of [0, max_splats): SET clears the
 // splats outside the tested range.  The ID-plane operation scatters into a scratch mask with atomicOr (pixels share splats) and a
-// second kernel combines it.  Every kernel ends a word with selected &= ~hidden.
+// second kernel combines it.  Every kernel ends a word with selected &= ~hidden.  Delete and duplicate (compact_store_kernel) move whole
+// splats between indices with one chained scan over the mask words.
 // The arithmetic follows the library's deterministic math (-fmad=false): one rounding per operator, in the order of include/gsr.h.
 #include "common.cuh"
 
@@ -299,6 +300,189 @@ __global__ void __launch_bounds__(SEL_THREADS) recolor_selection_kernel(const __
     sh_pack<BANDS, HALF, false>(dst, st, c, dc_words);
 }
 
+// ---- gsr_delete_hidden / gsr_duplicate_selection: a chained scan with decoupled look-back over the mask words of [0, n) ----
+// A tile's status word is a flag | count: EARLY (its count, published right after its ballots), AGG (its count, published after every
+// load of its moved splats has returned) or PREFIX (the inclusive count of tiles 0 .. t, published after AGG and a look-back over AGG /
+// PREFIX words).  So a PREFIX of tile t also says that every tile up to t has read its sources.
+constexpr unsigned long long CS_EARLY = 1ull << 61, CS_AGG = 1ull << 62, CS_PREFIX = 1ull << 63, CS_VALUE = CS_EARLY - 1ull;
+
+struct CompactShared {
+    uint32_t tile;
+    uint32_t warp_count[COMPACT_TILE_WORDS];
+    uint32_t sel[COMPACT_TILE_WORDS];   // DELETE: the selected bits of the kept splats, by CTA rank
+    unsigned long long excl;
+};
+// The CPU kernel emulator runs several CTAs of one launch at once and gives each its own copy of the CTA's shared state.
+#ifndef COMPACT_CTA_SHARED
+#define COMPACT_CTA_SHARED(T, name) __shared__ T name
+#endif
+
+// Warp 0: the exclusive count of tiles [0, tile), walking back 32 status words at a time and spinning on a word until its flag is in
+// `ready`; the walk ends at the nearest PREFIX.
+__device__ __forceinline__ unsigned long long lookback_exclusive(volatile unsigned long long *status, uint32_t tile, unsigned long long ready) {
+    const uint32_t lane = threadIdx.x & 31u;
+    unsigned long long excl = 0ull;
+    for (int64_t hi = (int64_t)tile - 1; hi >= 0; hi -= 32) {
+        const int64_t t = hi - (int64_t)lane;
+        unsigned long long v = CS_PREFIX;   // before tile 0: a prefix of 0
+        if (t >= 0) {
+            while (((v = status[t]) & ready) == 0ull) __nanosleep(32);
+        }
+        const uint32_t pre = __ballot_sync(0xffffffffu, (v & CS_PREFIX) != 0ull);
+        const uint32_t last = pre ? (uint32_t)(__ffs(pre) - 1) : 31u;   // the highest tile with a PREFIX ends the walk
+        unsigned long long c = lane <= last ? (v & CS_VALUE) : 0ull;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+        excl += c;
+        if (pre) break;
+    }
+    __threadfence();   // acquire: what the tiles did before publishing the words read above comes before what this CTA does next
+    return excl;
+}
+
+// One pass: the splats of [0, n) whose bit is set (DELETE: hidden clear, the kept splats; DUPLICATE: selected set) move, in order and
+// bit for bit (all 3 + P planes), to prefix (DELETE, in place) or n + prefix (DUPLICATE), prefix = the number of set bits below them.
+// A CTA owns COMPACT_TILE_WORDS consecutive mask words, one splat per thread, and takes its tile from an atomic ticket, so every
+// predecessor it waits on holds an earlier ticket and is resident or done.  A splat whose destination is its own index is neither read
+// nor written (a DELETE below the first hidden splat touches no plane).
+// In-place DELETE: destinations never exceed sources, but a CTA's destinations can overlap the sources of earlier CTAs.  The exact
+// destinations come from a first look-back over EARLY words (reads are always safe); the CTA then loads its moved splats into registers,
+// and publishes AGG only after every one of those loads has returned (loads, __syncthreads, fence, flag store).  Its second look-back
+// waits for AGG / PREFIX words down to the nearest PREFIX, so when it publishes its own PREFIX and starts to store (flag acquire, then
+// stores), every tile at or below it has read its sources: a destination is only ever written after the splat that lived there was
+// read.  Inside a CTA every load comes before any store.  DUPLICATE writes only at or above n, where no source lives, so it publishes
+// its PREFIX right after the first look-back.
+template <int BANDS, bool HALF, int MODE>
+__global__ void __launch_bounds__(COMPACT_THREADS) compact_store_kernel(const __grid_constant__ CompactArgs a) {
+    constexpr int PL = soa_planes(BANDS, HALF);
+    COMPACT_CTA_SHARED(CompactShared, sh);
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t nw = (uint32_t)((a.n + 31ull) >> 5), tiles = (nw + COMPACT_TILE_WORDS - 1) / COMPACT_TILE_WORDS;
+    volatile unsigned long long *status = a.lookback;
+    if (tid == 0) sh.tile = (uint32_t)atomicAdd(a.lookback + tiles, 1ull);
+    if (tid < COMPACT_TILE_WORDS) sh.sel[tid] = 0u;
+    __syncthreads();
+    const uint32_t tile = sh.tile, w = tile * COMPACT_TILE_WORDS + warp;
+    const uint64_t s = 32ull * w + lane, st = a.plane_stride;
+    uint32_t bits = 0u, sel = 0u;
+    if (w < nw) {
+        const uint32_t valid = 32ull * (w + 1) <= a.n ? 0xffffffffu : (1u << (uint32_t)(a.n & 31ull)) - 1u;
+        if constexpr (MODE == COMPACT_DELETE) {
+            bits = ~a.hidden[w] & valid;
+            sel = a.selected[w] & bits;
+        } else {
+            bits = a.selected[w] & valid;
+        }
+    }
+    if (lane == 0) sh.warp_count[warp] = (uint32_t)__popc(bits);
+    __syncthreads();
+    uint32_t rank = (uint32_t)__popc(bits & ((1u << lane) - 1u)), agg = 0u;
+#pragma unroll
+    for (uint32_t i = 0; i < COMPACT_TILE_WORDS; ++i) {
+        const uint32_t c = sh.warp_count[i];
+        rank += i < warp ? c : 0u;
+        agg += c;
+    }
+    const bool mine = (bits >> lane) & 1u;
+    if constexpr (MODE == COMPACT_DELETE) {
+        if (mine && ((sel >> lane) & 1u)) atomicOr(&sh.sel[rank >> 5], 1u << (rank & 31u));
+    }
+    if (tid == 0) status[tile] = CS_EARLY | agg;
+    if (warp == 0) {
+        const unsigned long long e = tile ? lookback_exclusive(status, tile, CS_EARLY | CS_AGG | CS_PREFIX) : 0ull;
+        if (lane == 0) {
+            sh.excl = e;
+            if constexpr (MODE == COMPACT_DUPLICATE) {
+                status[tile] = CS_PREFIX | (e + agg);
+                if (tile == tiles - 1) *a.total = e + agg;
+            }
+        }
+    }
+    __syncthreads();
+    const unsigned long long excl = sh.excl;
+    const uint64_t dst = (MODE == COMPACT_DUPLICATE ? a.n : 0ull) + excl + rank;
+    const bool move = mine && dst != s;
+    float4 v[PL];
+    if (move) {
+#pragma unroll
+        for (int p = 0; p < PL; ++p) v[p] = a.soa[(uint64_t)p * st + s];
+    }
+    if constexpr (MODE == COMPACT_DELETE) {
+        __syncthreads();   // every load of this tile's moved splats has returned
+        if (tid == 0) {
+            __threadfence();
+            status[tile] = (tile == 0 ? CS_PREFIX : CS_AGG) | agg;
+        }
+        if (warp == 0 && tile) {
+            const unsigned long long e = lookback_exclusive(status, tile, CS_AGG | CS_PREFIX);   // == excl
+            if (lane == 0) {
+                __threadfence();
+                status[tile] = CS_PREFIX | (e + agg);
+            }
+        }
+        if (tid == 0 && tile == tiles - 1) *a.total = excl + agg;
+        __syncthreads();
+        // the selected bits of the destinations [excl, excl + agg): word j of the CTA's rank bits lands at bit offset excl & 31
+        if (tid <= COMPACT_TILE_WORDS && agg) {
+            const uint32_t off = (uint32_t)(excl & 31ull);
+            const uint32_t val = (tid < COMPACT_TILE_WORDS ? sh.sel[tid] << off : 0u) | (tid > 0 && off ? sh.sel[tid - 1] >> (32u - off) : 0u);
+            const uint64_t ow = (excl >> 5) + tid;
+            if (val) {
+                if (32ull * ow >= excl && 32ull * ow + 32ull <= excl + agg) a.sel_out[ow] = val;   // no other CTA writes this word
+                else atomicOr(a.sel_out + ow, val);
+            }
+        }
+    }
+    if (move) {
+#pragma unroll
+        for (int p = 0; p < PL; ++p) a.soa[(uint64_t)p * st + dst] = v[p];
+    }
+}
+
+// After a delete that kept k of n splats: selected = the moved bits (scratch, zeroed again), hidden = 0 over every word, and the slots
+// [k, n) vacant: plane-0 x, y, z the quiet NaN 0x7FC00000, every other word +0.
+__global__ void __launch_bounds__(SEL_THREADS) delete_finish_kernel(float4 *soa, uint64_t st, int planes, uint64_t k, uint64_t n, uint32_t *hidden,
+                                                                    uint32_t *selected, uint32_t *scratch, uint32_t words) {
+    const uint64_t i = (uint64_t)blockIdx.x * SEL_THREADS + threadIdx.x;
+    if (i < words) {
+        selected[i] = scratch[i];
+        scratch[i] = 0u;
+        hidden[i] = 0u;
+    }
+    if (i < n - k) {
+        const float qnan = __uint_as_float(0x7FC00000u);
+        soa[k + i] = make_float4(qnan, qnan, qnan, 0.0f);
+#pragma unroll 1
+        for (int p = 1; p < planes; ++p) soa[(uint64_t)p * st + k + i] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    }
+}
+
+// After a duplicate of S splats behind n: selected = exactly [n, n + S), hidden cleared there
+__global__ void __launch_bounds__(SEL_THREADS) duplicate_finish_kernel(uint64_t n, uint64_t S, uint32_t *hidden, uint32_t *selected, uint32_t words) {
+    const uint32_t w = blockIdx.x * SEL_THREADS + threadIdx.x;
+    if (w >= words) return;
+    const uint64_t lo = 32ull * w, a = n > lo ? n : lo, b = n + S < lo + 32ull ? n + S : lo + 32ull;
+    uint32_t m = 0u;
+    if (a < b) {
+        const uint32_t i0 = (uint32_t)(a - lo), c = (uint32_t)(b - a);
+        m = (c == 32u ? 0xffffffffu : (1u << c) - 1u) << i0;
+    }
+    selected[w] = m;
+    hidden[w] &= ~m;
+}
+
+// counts[0] += the selected bits below n (the bounded count of gsr_duplicate_selection; mask_counts_kernel counts every word)
+__global__ void __launch_bounds__(SEL_THREADS) count_selected_kernel(const uint32_t *selected, uint64_t n, unsigned long long *counts) {
+    const uint32_t nw = (uint32_t)((n + 31ull) >> 5);
+    uint32_t ns = 0u;
+    for (uint32_t w = blockIdx.x * SEL_THREADS + threadIdx.x; w < nw; w += gridDim.x * SEL_THREADS) {
+        const uint32_t valid = 32ull * (w + 1) <= n ? 0xffffffffu : (1u << (uint32_t)(n & 31ull)) - 1u;
+        ns += __popc(selected[w] & valid);
+    }
+    ns = __reduce_add_sync(0xffffffffu, ns);
+    if ((threadIdx.x & 31u) == 0u && ns) atomicAdd(counts, (unsigned long long)ns);
+}
+
 }  // namespace
 
 // ---- the host's float64 matrices of gsr_transform_selection (also compiled into the CPU kernel emulator) ----
@@ -489,6 +673,60 @@ int launch_recolor_selection(const RecolorArgs &a, int bands, bool sh_half, cuda
     return GSR_OK;
 }
 
+namespace {
+template <int BANDS, bool HALF>
+void launch_compact_variant(const CompactArgs &a, int mode, uint32_t blocks, cudaStream_t stream) {
+    if (mode == COMPACT_DELETE) compact_store_kernel<BANDS, HALF, COMPACT_DELETE><<<blocks, COMPACT_THREADS, 0, stream>>>(a);
+    else compact_store_kernel<BANDS, HALF, COMPACT_DUPLICATE><<<blocks, COMPACT_THREADS, 0, stream>>>(a);
+}
+}  // namespace
+
+int launch_compact_store(const CompactArgs &a, int mode, int bands, bool sh_half, cudaStream_t stream) {
+    if (a.n == 0) return GSR_OK;
+    const uint32_t words = (uint32_t)((a.n + 31ull) >> 5);
+    const uint32_t blocks = (uint32_t)compact_lookback_words(words) - 1u;
+    GSR_CUDA_TRY(cudaMemsetAsync(a.lookback, 0, sizeof(unsigned long long) * compact_lookback_words(words), stream));
+    switch (bands * 2 + (sh_half ? 1 : 0)) {
+        case 2: launch_compact_variant<1, false>(a, mode, blocks, stream); break;
+        case 3: launch_compact_variant<1, true>(a, mode, blocks, stream); break;
+        case 4: launch_compact_variant<2, false>(a, mode, blocks, stream); break;
+        case 5: launch_compact_variant<2, true>(a, mode, blocks, stream); break;
+        case 6: launch_compact_variant<3, false>(a, mode, blocks, stream); break;
+        case 7: launch_compact_variant<3, true>(a, mode, blocks, stream); break;
+        case 8: launch_compact_variant<4, false>(a, mode, blocks, stream); break;
+        default: launch_compact_variant<4, true>(a, mode, blocks, stream); break;
+    }
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+int launch_delete_finish(float4 *soa, uint64_t plane_stride, int planes, uint64_t k, uint64_t n, uint32_t *hidden, uint32_t *selected,
+                         uint32_t *scratch, uint32_t words, cudaStream_t stream) {
+    const uint64_t items = words > n - k ? (uint64_t)words : n - k;
+    if (!items) return GSR_OK;
+    delete_finish_kernel<<<(uint32_t)((items + SEL_THREADS - 1) / SEL_THREADS), SEL_THREADS, 0, stream>>>(soa, plane_stride, planes, k, n, hidden,
+                                                                                                         selected, scratch, words);
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+int launch_duplicate_finish(uint64_t n, uint64_t S, uint32_t *hidden, uint32_t *selected, uint32_t words, cudaStream_t stream) {
+    if (!words) return GSR_OK;
+    duplicate_finish_kernel<<<word_blocks(words), SEL_THREADS, 0, stream>>>(n, S, hidden, selected, words);
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+int launch_count_selected(const uint32_t *selected, uint64_t n, unsigned long long *counts, cudaStream_t stream) {
+    GSR_CUDA_TRY(cudaMemsetAsync(counts, 0, sizeof(unsigned long long), stream));
+    const uint32_t words = (uint32_t)((n + 31ull) >> 5);
+    if (!words) return GSR_OK;
+    const uint32_t blocks = word_blocks(words) < 1024u ? word_blocks(words) : 1024u;
+    count_selected_kernel<<<blocks, SEL_THREADS, 0, stream>>>(selected, n, counts);
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
 int launch_select_region(const SelectArgs &a, int kind, cudaStream_t stream) {
     if (a.words == 0) return GSR_OK;
     const uint32_t blocks = (a.words + SEL_WARPS - 1) / SEL_WARPS;
@@ -558,6 +796,25 @@ int preload_selection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<3, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<4, false>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, recolor_selection_kernel<4, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<1, false, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<1, true, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<2, false, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<2, true, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<3, false, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<3, true, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<4, false, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<4, true, COMPACT_DELETE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<1, false, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<1, true, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<2, false, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<2, true, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<3, false, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<3, true, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<4, false, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, compact_store_kernel<4, true, COMPACT_DUPLICATE>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, delete_finish_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, duplicate_finish_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, count_selected_kernel));
     return GSR_OK;
 }
 #endif  // GSR_CPU_EMU

@@ -392,6 +392,24 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_recolor_selection(self._ctx, C.byref(edit), None if snapshot_ptr is None else C.c_void_p(snapshot_ptr)),
                    "gsr_recolor_selection")
 
+    # ---- splat delete and duplicate (include/gsr.h "Splat delete and duplicate"); each synchronises once ----
+    def delete_hidden(self) -> int:
+        """Compact the hidden splats out of [0, num_splats): the kept splats move down in order and the count k of them becomes
+        num_splats.  Returns k.  The splat at s moves to delete_remap(hidden)[s] (hidden as splat_masks() read it before the call)."""
+        k = C.c_uint64(0)
+        _lib.check(_lib.lib().gsr_delete_hidden(self._ctx, C.byref(k)), "gsr_delete_hidden")
+        return int(k.value)
+
+    def duplicate_selection(self) -> int:
+        """Append copies of the selected splats of [0, num_splats) behind it and select exactly the copies.  Returns their count."""
+        s = C.c_uint64(0)
+        _lib.check(_lib.lib().gsr_duplicate_selection(self._ctx, C.byref(s)), "gsr_duplicate_selection")
+        return int(s.value)
+
+    def set_splat_count(self, n: int) -> None:
+        """Set num_splats (undo of delete_hidden / duplicate_selection, after restore_splat_store and set_splat_masks)."""
+        _lib.check(_lib.lib().gsr_set_splat_count(self._ctx, int(n)), "gsr_set_splat_count")
+
     def splat_store_bytes(self) -> int:
         return int(_lib.lib().gsr_splat_store_bytes(self._ctx))
 
@@ -640,6 +658,14 @@ def pack_mask(mask, n: int) -> np.ndarray:
 def unpack_mask(words: np.ndarray, n: int) -> np.ndarray:
     """The inverse of pack_mask: uint32 words -> a bool array over n splats."""
     return np.unpackbits(np.ascontiguousarray(words, dtype="<u4").view(np.uint8), bitorder="little")[:n].astype(bool)
+
+
+def delete_remap(hidden, n: int) -> np.ndarray:
+    """The new index of every splat of [0, n) after delete_hidden, from the hidden mask read before it: the number of kept splats
+    below it (int64), or -1 for a deleted splat."""
+    h = np.asarray(hidden, dtype=bool).reshape(-1)[:n]
+    rank = np.cumsum(~h, dtype=np.int64) - 1
+    return np.where(h, np.int64(-1), rank)
 
 
 def godot_to_frame(transform, basis_override) -> np.ndarray:

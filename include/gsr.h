@@ -120,7 +120,8 @@ typedef struct gsr_config {
 } gsr_config;
 
 typedef struct gsr_stats {
-    uint64_t num_splats;  /* highest uploaded splat index + 1 */
+    uint64_t num_splats;  /* the cloud's size n: uploads raise it to first + count when that is larger; gsr_delete_hidden,
+                             gsr_duplicate_selection and gsr_set_splat_count set it (see "Splat delete and duplicate") */
     uint64_t duplicates;  /* M = histogram[0] of the reference (main.gd:98) -- true count, may exceed capacity */
     uint64_t visible;     /* V: splats that passed the cull and touch >= 1 tile */
     uint64_t capacity;    /* sort capacity in pairs */
@@ -570,6 +571,7 @@ GSR_API int gsr_set_cutouts(gsr_ctx *ctx, const gsr_cutout *cutouts, uint32_t n)
  *        (GSR_CUTOUT_FRAME); `action` is ignored.
  *      gsr_select_ids: "select what you see".  Every pixel of [x0, x1) x [y0, y1) of a device ID plane in the layout of gsr_set_splat_ids
  *        whose v != GSR_NO_ID marks the source splat of v under the current instance layout; a v past the layout's drawn ids is ignored.
+ *        An ID plane written before a gsr_delete_hidden or gsr_duplicate_selection names the splats by their indices before it.
  *      gsr_select_polygon and gsr_select_ids return GSR_ERR_STATE before gsr_resize.
  *      gsr_hide_selection: hidden |= selected, then selected = 0.  gsr_unhide_all: hidden = 0.
  *      gsr_clear_splat_masks: both masks 0 and no longer in use: frames take exactly the kernels they took before.
@@ -672,6 +674,36 @@ typedef struct gsr_color_edit {
     float opacity_scale, opacity_offset;   /* stored opacity o' = clamp(o * scale + offset, 0, 1), rule above */
 } gsr_color_edit;           /* 68 bytes; identity = {I | 0}, {1, 1, 1}, 1, 0 */
 GSR_API int gsr_recolor_selection(gsr_ctx *ctx, const gsr_color_edit *edit, const void *src_store);
+
+/* ---- Splat delete and duplicate: change how many splats the cloud has (no reference counterpart).
+ *      The cloud is the splats of [0, n), n = gsr_stats.num_splats.  A slot that stops holding a splat is left vacant: plane-0 x, y and
+ *      z the quiet NaN 0x7FC00000, every other float word of every plane +0 (with GSR_FLAG_SH_HALF every half slot +0), its hidden and
+ *      selected bits 0.  Every projection variant culls a vacant slot like a frustum-culled splat (no record, no pairs, no share of M, V
+ *      or the last tile) by its rule that a splat whose projected centre or radius is not finite is culled; a NaN position is also
+ *      outside every polygon and volume selection.
+ *      gsr_delete_hidden: the kept splats are those of [0, n) whose hidden bit is 0.  They move to [0, k) in their order, every word of
+ *      every plane bit for bit, each with its selected bit; then [k, n) is vacant, every hidden bit is cleared, every selected bit at or
+ *      above k is cleared, n = k and *kept_out = k.  Slots at or above the old n are not touched.  The new index of the splat at s is
+ *      the number of kept splats below s, so the host can remap from masks read before the call (no device index map is returned).
+ *      A frame after a delete is bit for bit the frame before it with the deleted splats hidden (RGBA, depth, motion, M, V, last tile,
+ *      keys, tile ranges and the selection highlight): only sort values, record indices and IDs change, by the rank rule above.
+ *      GSR_ERR_INVALID: a NULL kept_out.  GSR_ERR_STATE while the splat masks are not in use, or while instances are set (their ranges
+ *      would silently point at other splats).  Nothing changes on an error.
+ *      gsr_duplicate_selection: the S selected splats of [0, n) are copied in order, bit for bit, to [n, n + S); then n = n + S and
+ *      *copies_out = S.  The selection is then exactly the copies (the originals are deselected and selected bits at or above the old n
+ *      dropped); hidden bits are unchanged except that the copies are not hidden.  Paste-and-move is gsr_duplicate_selection followed by
+ *      gsr_transform_selection.  With instances set the copies lie outside every instance range (so are not drawn) until the host
+ *      changes the ranges.  GSR_ERR_INVALID, nothing written and the state kept: a NULL copies_out, or n + S > max_splats (the message
+ *      gives S and the room left).  The arguments are checked first; then GSR_ERR_STATE while the splat masks are not in use.
+ *      gsr_set_splat_count: sets n and writes nothing else, for undo.  GSR_ERR_INVALID: n > max_splats.  Undo of a delete or duplicate
+ *      is exact: gsr_restore_splat_store of the snapshot taken before it, then gsr_set_splat_masks, then gsr_set_splat_count.
+ *      Ordering as gsr_transform_selection: on the projections' stream after an event on the render stream, after every frame enqueued
+ *      before it and before every frame enqueued after it.  Unlike the other edits each synchronises the host once (a delete must learn
+ *      k, a duplicate must know S before it writes anything): they are click-time operations, not per-frame ones.  Neither is motion
+ *      (like an upload).  Masks in use are single-context, so neither applies to a sharded context. ---- */
+GSR_API int gsr_delete_hidden(gsr_ctx *ctx, uint64_t *kept_out);
+GSR_API int gsr_duplicate_selection(gsr_ctx *ctx, uint64_t *copies_out);
+GSR_API int gsr_set_splat_count(gsr_ctx *ctx, uint64_t n);
 
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
