@@ -29,6 +29,10 @@ GSR_DRAW_ALL = 0xFFFFFFFFFFFFFFFF   # gsr_instance_appearance.draw_count: every 
 GSR_NO_ID = 0xFFFFFFFF              # gsr_set_splat_ids: no splat / no instance
 GSR_MAX_SELECT_VERTICES = 64
 GSR_SELECT_SET, GSR_SELECT_ADD, GSR_SELECT_SUBTRACT, GSR_SELECT_TOGGLE = range(4)
+GSR_PROP_OPACITY, GSR_PROP_SIZE, GSR_PROP_VOLUME, GSR_PROP_ISOTROPY, GSR_PROP_COLOR_DISTANCE = range(5)
+GSR_MAX_SPLAT_FILTERS = 8
+GSR_MAX_HISTOGRAM_BINS = 1024
+GSR_HISTOGRAM_KEPT, GSR_HISTOGRAM_SELECTED = 0, 1
 
 # every symbol include/gsr.h declares (tests/test_abi.py checks the header against this list and the .so)
 EXPORTS = [
@@ -39,7 +43,7 @@ EXPORTS = [
     "gsr_select_all", "gsr_select_polygon", "gsr_select_volume", "gsr_select_ids", "gsr_hide_selection", "gsr_unhide_all", "gsr_clear_splat_masks",
     "gsr_get_splat_masks", "gsr_set_splat_masks", "gsr_splat_mask_counts", "gsr_set_selection_style",
     "gsr_transform_selection", "gsr_splat_store_bytes", "gsr_copy_splat_store", "gsr_restore_splat_store", "gsr_recolor_selection",
-    "gsr_delete_hidden", "gsr_duplicate_selection", "gsr_set_splat_count",
+    "gsr_delete_hidden", "gsr_duplicate_selection", "gsr_set_splat_count", "gsr_select_where", "gsr_splat_histogram",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -73,6 +77,10 @@ class GsrInstanceAppearance(C.Structure):
 
 class GsrColorEdit(C.Structure):
     _fields_ = [("matrix", C.c_float * 12), ("band_scale", C.c_float * 3), ("opacity_scale", C.c_float), ("opacity_offset", C.c_float)]
+
+
+class GsrSplatFilter(C.Structure):
+    _fields_ = [("property", C.c_int32), ("lo", C.c_float), ("hi", C.c_float), ("rgb", C.c_float * 3)]
 
 
 class GsrCutout(C.Structure):
@@ -169,6 +177,8 @@ def lib():
         L.gsr_delete_hidden.argtypes = [vp, C.POINTER(u64)]
         L.gsr_duplicate_selection.argtypes = [vp, C.POINTER(u64)]
         L.gsr_set_splat_count.argtypes = [vp, u64]
+        L.gsr_select_where.argtypes = [vp, C.POINTER(GsrSplatFilter), u32, C.c_int32, C.c_int32]
+        L.gsr_splat_histogram.argtypes = [vp, C.POINTER(GsrSplatFilter), C.c_int32, C.c_int32, fp, u32, C.POINTER(u64), fp]
         L.gsr_splat_store_bytes.argtypes = [vp]
         L.gsr_splat_store_bytes.restype = u64
         L.gsr_copy_splat_store.argtypes = [vp, vp]

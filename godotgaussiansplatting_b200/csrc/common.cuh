@@ -382,6 +382,48 @@ int launch_duplicate_finish(uint64_t n, uint64_t S, uint32_t *hidden, uint32_t *
 // counts[0] = popcount of the selected bits below n
 int launch_count_selected(const uint32_t *selected, uint64_t n, unsigned long long *counts, cudaStream_t stream);
 
+// ---- splat property selection (gsr_select_where, gsr_splat_histogram; selection.cu) ----
+// The planes a property reads beyond plane 0 (a size, volume or isotropy reads planes 1 and 2).  The kernels are templated on the union
+// of a filter set's bits, so each reads only the planes its set needs.
+enum PropPlanes : int { PROP_P1 = 1, PROP_P2 = 2, PROP_P3 = 4 };
+__host__ __device__ constexpr int prop_planes(int32_t p) {
+    return p == GSR_PROP_OPACITY ? PROP_P2 : p == GSR_PROP_COLOR_DISTANCE ? PROP_P3 : PROP_P1 | PROP_P2;
+}
+// inside(s) for the splats s of [first, first + count) (the caller bounds it by the cloud's n), combined into the selected mask by `op`
+// over every word, then selected &= ~hidden.
+struct WhereArgs {
+    uint32_t *selected;
+    const uint32_t *hidden;
+    uint32_t words, op;
+    uint64_t first, count;
+    const float4 *soa;
+    uint64_t plane_stride;
+    uint32_t n;                                   // filters
+    gsr_splat_filter f[GSR_MAX_SPLAT_FILTERS];
+};
+// planes: the union of prop_planes over the set; sh_half: the store's SH format (read only when the set reads plane 3)
+int launch_select_where(const WhereArgs &a, int planes, bool sh_half, cudaStream_t stream);
+// The histogram's device buffer: the counters, then the min / max keys, then the edges.  The keys are kept as ints so that one
+// atomicMax serves both: keys[0] = max of hist_signed_key(~ord(v)) (the least ord(v)), keys[1] = max of hist_signed_key(ord(v)) (the
+// greatest), ord the map of gsr_set_depth_order; INT32_MIN, the key of a NaN, means no value.
+__host__ __device__ __forceinline__ int32_t hist_signed_key(uint32_t k) { return (int32_t)(k ^ 0x80000000u); }
+constexpr uint32_t HIST_COUNTS = GSR_MAX_HISTOGRAM_BINS + 3;
+constexpr size_t HIST_KEYS_OFFSET = sizeof(unsigned long long) * HIST_COUNTS, HIST_EDGES_OFFSET = HIST_KEYS_OFFSET + 2 * sizeof(uint32_t);
+constexpr size_t HIST_BUFFER_BYTES = HIST_EDGES_OFFSET + sizeof(float) * (GSR_MAX_HISTOGRAM_BINS + 1);
+struct HistArgs {
+    const float4 *soa;
+    uint64_t plane_stride;
+    uint64_t first, count;                        // the tested range, bounded by n
+    const uint32_t *hidden, *selected;            // hidden == nullptr: the masks are not in use (nothing hidden, nothing selected)
+    uint32_t selected_only;                       // GSR_HISTOGRAM_SELECTED
+    uint32_t bins, top;                           // top: the largest power of two <= max(bins - 1, 1) (the binary search's first step)
+    gsr_splat_filter prop;
+    unsigned long long *counts;                   // bins + 3, zeroed
+    int32_t *keys;                                // INT32_MIN, INT32_MIN on entry: the least and greatest ord(v), as above
+    const float *edges;                           // bins + 1
+};
+int launch_splat_histogram(const HistArgs &a, int planes, bool sh_half, int sm_count, cudaStream_t stream);
+
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.
 __host__ __device__ __forceinline__ uint32_t depth_order_word(uint32_t bits) { return bits ^ ((bits >> 31) ? 0xFFFFFFFFu : 0x80000000u); }

@@ -61,6 +61,8 @@ struct gsr_ctx {
     float edit_last[EDIT_TRANSFORM_FLOATS] = {};   // GSR_BUF_EDIT_TRANSFORM: the constants of the last accepted transform
     float color_last[EDIT_COLOR_FLOATS] = {};      // GSR_BUF_EDIT_COLOR: the constants of the last accepted colour edit
     cudaEvent_t store_ready = nullptr;             // with front / back overlap: the render stream's work enqueued before the operation
+    void *hist = nullptr;                          // gsr_splat_histogram: HIST_BUFFER_BYTES (counters, min / max keys, edges), first call
+    unsigned char *hist_host = nullptr;            // its page-locked image (upload and read-back)
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -323,6 +325,8 @@ void free_ctx(gsr_ctx *c) {
     cudaFree(c->masks.counts);   // the base of the mask allocation
     if (c->masks.ids_ready) cudaEventDestroy(c->masks.ids_ready);
     if (c->store_ready) cudaEventDestroy(c->store_ready);
+    cudaFree(c->hist);
+    if (c->hist_host) cudaFreeHost(c->hist_host);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
     for (int i = 0; i < GSR_INSTANCE_RING; ++i) if (c->inst.ev[i]) cudaEventDestroy(c->inst.ev[i]);
     delete[] c->inst.range; delete[] c->inst.xf; delete[] c->inst.app;
@@ -2065,6 +2069,116 @@ GSR_API int gsr_set_splat_count(gsr_ctx *c, uint64_t n) {
     if (!c) return GSR_ERR_INVALID;
     if (n > c->max_splats) { set_last_error("gsr_set_splat_count: %llu > max_splats %llu", (unsigned long long)n, (unsigned long long)c->max_splats); return GSR_ERR_INVALID; }
     c->num_splats = n;
+    return GSR_OK;
+}
+
+// ---- splat property selection: gsr_select_where is enqueued like the selections, gsr_splat_histogram like the store edits ----------
+static int check_property(const gsr_splat_filter &f, const char *where, uint32_t i) {
+    if (f.property < GSR_PROP_OPACITY || f.property > GSR_PROP_COLOR_DISTANCE) { set_last_error("%s: filter %u: unknown property %d", where, i, f.property); return GSR_ERR_INVALID; }
+    if (f.property != GSR_PROP_COLOR_DISTANCE) return GSR_OK;   // rgb is ignored
+    for (int k = 0; k < 3; ++k) {
+        if (!(fabsf(f.rgb[k]) <= 3.402823466e38f)) { set_last_error("%s: filter %u: non-finite rgb[%d]", where, i, k); return GSR_ERR_INVALID; }
+    }
+    return GSR_OK;
+}
+
+// The tested range of select_range (instance -1: the store, k: instance k's source range) intersected with the cloud [0, n)
+static int property_range(const gsr_ctx *c, const char *where, int32_t instance, uint64_t &first, uint64_t &count) {
+    SelectArgs a;
+    int rc = select_range(c, where, instance, a);
+    if (rc) return rc;
+    const uint64_t n = c->num_splats;
+    first = a.first;
+    count = a.first >= n ? 0ull : (a.count < n - a.first ? a.count : n - a.first);
+    return GSR_OK;
+}
+
+GSR_API int gsr_select_where(gsr_ctx *c, const gsr_splat_filter *filters, uint32_t n, int32_t instance, int32_t op) {
+    if (!c || !filters) { set_last_error("gsr_select_where: NULL argument"); return GSR_ERR_INVALID; }
+    if (n < 1 || n > GSR_MAX_SPLAT_FILTERS) { set_last_error("gsr_select_where: %u filters, need 1..%d", n, GSR_MAX_SPLAT_FILTERS); return GSR_ERR_INVALID; }
+    int planes = 0, rc;
+    for (uint32_t i = 0; i < n; ++i) {
+        if ((rc = check_property(filters[i], "gsr_select_where", i))) return rc;
+        if (filters[i].lo != filters[i].lo || filters[i].hi != filters[i].hi) { set_last_error("gsr_select_where: filter %u: NaN bound", i); return GSR_ERR_INVALID; }
+        planes |= prop_planes(filters[i].property);
+    }
+    if (!select_op_valid(op)) { set_last_error("gsr_select_where: unknown op %d", op); return GSR_ERR_INVALID; }
+    WhereArgs a;
+    memset(&a, 0, sizeof a);
+    if ((rc = property_range(c, "gsr_select_where", instance, a.first, a.count))) return rc;
+    if ((rc = masks_use(c, "gsr_select_where"))) return rc;
+    a.selected = c->masks.selected; a.hidden = c->masks.hidden; a.words = c->masks.words; a.op = (uint32_t)op;
+    a.soa = c->soa; a.plane_stride = c->plane_stride;
+    a.n = n;
+    memcpy(a.f, filters, sizeof(gsr_splat_filter) * n);
+    return launch_select_where(a, planes, sh_half(c), mask_stream(c));
+}
+
+// ord (gsr_set_depth_order) back to the float
+static float ord_float(uint32_t key) { const uint32_t b = (key >> 31) ? key ^ 0x80000000u : ~key; float f; memcpy(&f, &b, 4); return f; }
+
+GSR_API int gsr_splat_histogram(gsr_ctx *c, const gsr_splat_filter *property, int32_t instance, int32_t scope, const float *edges,
+                                uint32_t bins, uint64_t *counts, float minmax[2]) {
+    if (!c || !property || !edges || !counts) { set_last_error("gsr_splat_histogram: NULL argument"); return GSR_ERR_INVALID; }
+    if (bins < 1 || bins > GSR_MAX_HISTOGRAM_BINS) { set_last_error("gsr_splat_histogram: %u bins, need 1..%d", bins, GSR_MAX_HISTOGRAM_BINS); return GSR_ERR_INVALID; }
+    for (uint32_t i = 0; i <= bins; ++i) {
+        if (!(fabsf(edges[i]) <= 3.402823466e38f)) { set_last_error("gsr_splat_histogram: edge %u is not finite", i); return GSR_ERR_INVALID; }
+        if (i && !(edges[i] > edges[i - 1])) { set_last_error("gsr_splat_histogram: edge %u does not increase", i); return GSR_ERR_INVALID; }
+    }
+    int rc = check_property(*property, "gsr_splat_histogram", 0);
+    if (rc) return rc;
+    if (scope != GSR_HISTOGRAM_KEPT && scope != GSR_HISTOGRAM_SELECTED) { set_last_error("gsr_splat_histogram: unknown scope %d", scope); return GSR_ERR_INVALID; }
+    HistArgs a;
+    memset(&a, 0, sizeof a);
+    if ((rc = property_range(c, "gsr_splat_histogram", instance, a.first, a.count))) return rc;
+    const bool none = scope == GSR_HISTOGRAM_SELECTED && !c->masks.on;   // nothing is selected
+    unsigned long long *got = nullptr;
+    int32_t keys[2] = {INT32_MIN, INT32_MIN};
+    if (a.count && !none) {
+        if ((rc = use_device(c->device))) return rc;
+        if (!c->hist) {   // the device buffer and its page-locked image, so both copies are asynchronous
+            void *d = nullptr, *h = nullptr;
+            cudaError_t e = cudaMalloc(&d, HIST_BUFFER_BYTES);
+            if (e == cudaSuccess) e = cudaMallocHost(&h, HIST_BUFFER_BYTES);
+            if (e != cudaSuccess) {
+                cudaFree(d);
+                set_last_error("gsr_splat_histogram: %zu B -> %s", HIST_BUFFER_BYTES, cudaGetErrorString(e));
+                return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+            }
+            c->hist = d;
+            c->hist_host = static_cast<unsigned char *>(h);
+        }
+        cudaStream_t s;
+        if ((rc = store_stream(c, &s))) return rc;
+        // the image: zeroed counters, the initial keys, the edges
+        unsigned char *img = c->hist_host;
+        memset(img, 0, HIST_EDGES_OFFSET);
+        memcpy(img + HIST_KEYS_OFFSET, keys, sizeof keys);
+        memcpy(img + HIST_EDGES_OFFSET, edges, sizeof(float) * (bins + 1));
+        char *buf = static_cast<char *>(c->hist);
+        GSR_CUDA_TRY(cudaMemcpyAsync(buf, img, HIST_EDGES_OFFSET + sizeof(float) * (bins + 1), cudaMemcpyHostToDevice, s));
+        a.soa = c->soa; a.plane_stride = c->plane_stride;
+        a.hidden = c->masks.on ? c->masks.hidden : nullptr; a.selected = c->masks.on ? c->masks.selected : nullptr;
+        a.selected_only = scope == GSR_HISTOGRAM_SELECTED;
+        a.bins = bins;
+        a.top = 1u;
+        while (2u * a.top <= bins - 1u) a.top *= 2u;
+        a.prop = *property;
+        a.counts = reinterpret_cast<unsigned long long *>(buf);
+        a.keys = reinterpret_cast<int32_t *>(buf + HIST_KEYS_OFFSET);
+        a.edges = reinterpret_cast<const float *>(buf + HIST_EDGES_OFFSET);
+        if ((rc = launch_splat_histogram(a, prop_planes(property->property), sh_half(c), c->sm_count, s))) return rc;
+        GSR_CUDA_TRY(cudaMemcpyAsync(img, buf, HIST_EDGES_OFFSET, cudaMemcpyDeviceToHost, s));
+        GSR_CUDA_TRY(cudaStreamSynchronize(s));
+        got = reinterpret_cast<unsigned long long *>(img);
+        memcpy(keys, img + HIST_KEYS_OFFSET, sizeof keys);
+    }
+    for (uint32_t i = 0; i < bins + 3; ++i) counts[i] = got ? got[i] : 0ull;
+    if (minmax) {
+        const bool any = keys[1] != INT32_MIN;
+        minmax[0] = any ? ord_float(~((uint32_t)keys[0] ^ 0x80000000u)) : INFINITY;
+        minmax[1] = any ? ord_float((uint32_t)keys[1] ^ 0x80000000u) : -INFINITY;
+    }
     return GSR_OK;
 }
 

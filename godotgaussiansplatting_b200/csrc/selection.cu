@@ -5,7 +5,8 @@
 // update is atomic, even for an instance range that starts inside a word.  The grid covers every word of [0, max_splats): SET clears the
 // splats outside the tested range.  The ID-plane operation scatters into a scratch mask with atomicOr (pixels share splats) and a
 // second kernel combines it.  Every kernel ends a word with selected &= ~hidden.  Delete and duplicate (compact_store_kernel) move whole
-// splats between indices with one chained scan over the mask words.
+// splats between indices with one chained scan over the mask words.  Property selection (select_where_kernel) has the region
+// operations' shape and tests the stored words; the property histogram (splat_histogram_kernel) is a grid-stride pass with the same reads.
 // The arithmetic follows the library's deterministic math (-fmad=false): one rounding per operator, in the order of include/gsr.h.
 #include "common.cuh"
 
@@ -483,6 +484,149 @@ __global__ void __launch_bounds__(SEL_THREADS) count_selected_kernel(const uint3
     if ((threadIdx.x & 31u) == 0u && ns) atomicAdd(counts, (unsigned long long)ns);
 }
 
+// ---- gsr_select_where / gsr_splat_histogram: per-splat properties of the stored words (include/gsr.h "Splat property selection") ----
+// A tested splat counts only if none of its plane-0 x, y, z is NaN (a vacant slot never counts).
+__device__ __forceinline__ bool splat_vacant(const float4 &p0) { return p0.x != p0.x || p0.y != p0.y || p0.z != p0.z; }
+
+// The planes of one splat beyond plane 0, each loaded the first time a property needs it, so a splat that failed an earlier filter
+// reads nothing more.  PL: the prop_planes bits of the filter set (a plane outside PL is never read); HALF: the SH format of plane 3.
+// Every value in float32, one rounding per operation, in the order of include/gsr.h.
+template <bool HALF, int PL>
+struct SplatProps {
+    const float4 *src;   // plane 0 of the splat
+    uint64_t st;
+    float4 p1 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), p2 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    float dc[3] = {0.0f, 0.0f, 0.0f};
+    int have = 0;
+    __device__ __forceinline__ SplatProps(const float4 *s, uint64_t stride) : src(s), st(stride) {}
+
+    __device__ __forceinline__ float value(const gsr_splat_filter &f) {
+        const int need = prop_planes(f.property) & ~have;
+        if constexpr ((PL & PROP_P1) != 0) if (need & PROP_P1) p1 = __ldg(src + st);
+        if constexpr ((PL & PROP_P2) != 0) if (need & PROP_P2) p2 = __ldg(src + 2 * st);
+        if constexpr ((PL & PROP_P3) != 0) {
+            if (need & PROP_P3) {
+                const float4 v = __ldg(src + 3 * st);
+                if constexpr (HALF) {   // values 0, 1 in word x, value 2 in the low half of word y
+                    dc[0] = half_bits_to_float(__float_as_uint(v.x) & 0xFFFFu);
+                    dc[1] = half_bits_to_float(__float_as_uint(v.x) >> 16);
+                    dc[2] = half_bits_to_float(__float_as_uint(v.y) & 0xFFFFu);
+                } else {
+                    dc[0] = v.x; dc[1] = v.y; dc[2] = v.z;
+                }
+            }
+        }
+        have |= need;
+        const int32_t p = f.property;
+        if (p == GSR_PROP_OPACITY) return p2.z;
+        if (p == GSR_PROP_COLOR_DISTANCE) {
+            float d2 = 0.0f;
+#pragma unroll
+            for (int i = 0; i < 3; ++i) {
+                const float d = __fsub_rn(__fadd_rn(0.5f, __fmul_rn(dc[i], SH_C0)), f.rgb[i]);
+                d2 = i == 0 ? __fmul_rn(d, d) : __fadd_rn(d2, __fmul_rn(d, d));
+            }
+            return d2;
+        }
+        const float S00 = p1.x, S01 = p1.y, S02 = p1.z, S11 = p1.w, S12 = p2.x, S22 = p2.y;
+        const float t = __fadd_rn(__fadd_rn(S00, S11), S22);
+        if (p == GSR_PROP_SIZE) return t;
+        const float det = __fadd_rn(__fsub_rn(__fmul_rn(S00, __fsub_rn(__fmul_rn(S11, S22), __fmul_rn(S12, S12))),
+                                              __fmul_rn(S01, __fsub_rn(__fmul_rn(S01, S22), __fmul_rn(S12, S02)))),
+                                    __fmul_rn(S02, __fsub_rn(__fmul_rn(S01, S12), __fmul_rn(S11, S02))));
+        if (p == GSR_PROP_VOLUME) return det;
+        return __fdiv_rn(__fmul_rn(27.0f, det), __fmul_rn(__fmul_rn(t, t), t));   // GSR_PROP_ISOTROPY
+    }
+};
+
+// gsr_select_where: the shape of select_region_kernel -- a warp per mask word, a lane per splat, a ballot, lane 0 combines.  Lanes
+// outside the tested range read nothing; a lane leaves the filter loop at its first failed filter.
+template <bool HALF, int PL>
+__global__ void __launch_bounds__(SEL_THREADS) select_where_kernel(const __grid_constant__ WhereArgs a) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t w = blockIdx.x * SEL_WARPS + (threadIdx.x >> 5);
+    if (w >= a.words) return;   // warp-uniform
+    const uint64_t s = 32ull * w + lane;
+    bool in = s >= a.first && s - a.first < a.count;
+    if (in) {
+        const float4 *src = a.soa + s;
+        in = !splat_vacant(__ldg(src));
+        SplatProps<HALF, PL> sp(src, a.plane_stride);
+#pragma unroll 1
+        for (uint32_t i = 0; in && i < a.n; ++i) {
+            const float v = sp.value(a.f[i]);
+            in = a.f[i].lo <= v && v <= a.f[i].hi;
+        }
+    }
+    const uint32_t inside = __ballot_sync(0xffffffffu, in);
+    if (lane == 0) a.selected[w] = combine_op(a.op, a.selected[w], inside) & ~a.hidden[w];
+}
+
+// gsr_splat_histogram: a grid-stride pass over the tested range.  Each CTA keeps the edges and a private bins + 3 histogram in shared
+// memory, finds a value's bin by a branch-free binary search (the largest i < bins with e_i <= v; the comparisons place below, above
+// and NaN), and adds its non-zero counters to the 64-bit global ones once at the end.  The least and greatest ord(v) of the non-NaN
+// values are reduced per warp (a shuffle butterfly), then go to the global keys with one atomicMax each per warp: max of
+// signed_key(~lo) for the least, max of signed_key(hi) for the greatest (signed_key orders an unsigned key as an int).  Launched only while something can count (not for
+// GSR_HISTOGRAM_SELECTED while the masks are not in use).
+constexpr int PROP_HIST_THREADS = 512;
+struct PropHistShared {
+    uint32_t count[HIST_COUNTS];
+    float edge[GSR_MAX_HISTOGRAM_BINS + 1];
+};
+// The CPU kernel emulator runs several CTAs of one launch at once and gives each its own copy of the CTA's shared state.
+#ifndef HIST_CTA_SHARED
+#define HIST_CTA_SHARED(T, name) __shared__ T name
+#endif
+
+template <bool HALF, int PL>
+__global__ void __launch_bounds__(PROP_HIST_THREADS) splat_histogram_kernel(const __grid_constant__ HistArgs a) {
+    HIST_CTA_SHARED(PropHistShared, sh);
+    const uint32_t tid = threadIdx.x, B = a.bins;
+    for (uint32_t i = tid; i < B + 3; i += PROP_HIST_THREADS) sh.count[i] = 0u;
+    for (uint32_t i = tid; i <= B; i += PROP_HIST_THREADS) sh.edge[i] = __ldg(a.edges + i);
+    __syncthreads();
+    const float e0 = sh.edge[0], eb = sh.edge[B];
+    uint32_t lo = 0xFFFFFFFFu, hi = 0u;
+    for (uint64_t i = (uint64_t)blockIdx.x * PROP_HIST_THREADS + tid; i < a.count; i += (uint64_t)gridDim.x * PROP_HIST_THREADS) {
+        const uint64_t s = a.first + i;
+        if (a.hidden) {
+            const uint32_t bit = 1u << (uint32_t)(s & 31u);
+            if ((__ldg(a.hidden + (s >> 5)) & bit) || (a.selected_only && !(__ldg(a.selected + (s >> 5)) & bit))) continue;
+        }
+        const float4 *src = a.soa + s;
+        if (splat_vacant(__ldg(src))) continue;
+        SplatProps<HALF, PL> sp(src, a.plane_stride);
+        const float v = sp.value(a.prop);
+        uint32_t k = 0u;
+        for (uint32_t step = a.top; step; step >>= 1) {
+            const uint32_t j = k + step;
+            k = (j < B && sh.edge[j] <= v) ? j : k;
+        }
+        const bool nan = v != v;
+        atomicAdd(&sh.count[nan ? B + 2 : v < e0 ? B : v > eb ? B + 1 : k], 1u);
+        if (!nan) {
+            const uint32_t key = depth_order_word(__float_as_uint(v));
+            lo = key < lo ? key : lo;
+            hi = key > hi ? key : hi;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const uint32_t l = __shfl_xor_sync(0xffffffffu, lo, o), h = __shfl_xor_sync(0xffffffffu, hi, o);
+        lo = l < lo ? l : lo;
+        hi = h > hi ? h : hi;
+    }
+    if ((tid & 31u) == 0u && lo <= hi) {   // lo > hi: no value in this warp
+        atomicMax(a.keys, hist_signed_key(~lo));
+        atomicMax(a.keys + 1, hist_signed_key(hi));
+    }
+    __syncthreads();
+    for (uint32_t i = tid; i < B + 3; i += PROP_HIST_THREADS) {
+        const uint32_t c = sh.count[i];
+        if (c) atomicAdd(a.counts + i, (unsigned long long)c);
+    }
+}
+
 }  // namespace
 
 // ---- the host's float64 matrices of gsr_transform_selection (also compiled into the CPU kernel emulator) ----
@@ -727,6 +871,46 @@ int launch_count_selected(const uint32_t *selected, uint64_t n, unsigned long lo
     return GSR_OK;
 }
 
+namespace {
+template <bool HALF, int PL>
+void launch_property_variant(const WhereArgs &a, uint32_t blocks, cudaStream_t stream) {
+    select_where_kernel<HALF, PL><<<blocks, SEL_THREADS, 0, stream>>>(a);
+}
+template <bool HALF, int PL>
+void launch_property_variant(const HistArgs &a, uint32_t blocks, cudaStream_t stream) {
+    splat_histogram_kernel<HALF, PL><<<blocks, PROP_HIST_THREADS, 0, stream>>>(a);
+}
+
+// The variants: the plane sets a filter set can need (plane 1 always comes with plane 2), and the SH format only where plane 3 is read.
+template <class Args>
+int launch_property(const Args &a, int planes, bool sh_half, uint32_t blocks, cudaStream_t stream) {
+    switch (planes | (sh_half && (planes & PROP_P3) ? 8 : 0)) {
+        case PROP_P2: launch_property_variant<false, PROP_P2>(a, blocks, stream); break;
+        case PROP_P1 | PROP_P2: launch_property_variant<false, PROP_P1 | PROP_P2>(a, blocks, stream); break;
+        case PROP_P3: launch_property_variant<false, PROP_P3>(a, blocks, stream); break;
+        case PROP_P2 | PROP_P3: launch_property_variant<false, PROP_P2 | PROP_P3>(a, blocks, stream); break;
+        case PROP_P1 | PROP_P2 | PROP_P3: launch_property_variant<false, PROP_P1 | PROP_P2 | PROP_P3>(a, blocks, stream); break;
+        case 8 | PROP_P3: launch_property_variant<true, PROP_P3>(a, blocks, stream); break;
+        case 8 | PROP_P2 | PROP_P3: launch_property_variant<true, PROP_P2 | PROP_P3>(a, blocks, stream); break;
+        case 8 | PROP_P1 | PROP_P2 | PROP_P3: launch_property_variant<true, PROP_P1 | PROP_P2 | PROP_P3>(a, blocks, stream); break;
+        default: set_last_error("splat property kernels: no variant for plane set %d", planes); return GSR_ERR_INVALID;
+    }
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+}  // namespace
+
+int launch_select_where(const WhereArgs &a, int planes, bool sh_half, cudaStream_t stream) {
+    if (a.words == 0) return GSR_OK;
+    return launch_property(a, planes, sh_half, (a.words + SEL_WARPS - 1) / SEL_WARPS, stream);
+}
+
+int launch_splat_histogram(const HistArgs &a, int planes, bool sh_half, int sm_count, cudaStream_t stream) {
+    if (a.count == 0) return GSR_OK;
+    const uint64_t need = (a.count + PROP_HIST_THREADS - 1) / PROP_HIST_THREADS, most = 4ull * (uint64_t)(sm_count > 0 ? sm_count : 1);   // 4 CTAs of 512 per SM
+    return launch_property(a, planes, sh_half, (uint32_t)(need < most ? need : most), stream);
+}
+
 int launch_select_region(const SelectArgs &a, int kind, cudaStream_t stream) {
     if (a.words == 0) return GSR_OK;
     const uint32_t blocks = (a.words + SEL_WARPS - 1) / SEL_WARPS;
@@ -815,6 +999,22 @@ int preload_selection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, delete_finish_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, duplicate_finish_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, count_selected_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P2>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P1 | PROP_P2>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P1 | PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<true, PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<true, PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<true, PROP_P1 | PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_P2>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_P1 | PROP_P2>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_P1 | PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_P1 | PROP_P2 | PROP_P3>));
     return GSR_OK;
 }
 #endif  // GSR_CPU_EMU

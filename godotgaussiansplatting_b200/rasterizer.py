@@ -362,6 +362,35 @@ class GaussianSplattingRasterizer:
         _lib.check(_lib.lib().gsr_splat_mask_counts(self._ctx, C.byref(s), C.byref(h)), "gsr_splat_mask_counts")
         return int(s.value), int(h.value)
 
+    # ---- splat property selection (include/gsr.h "Splat property selection") ----
+    def select_where(self, filters, op: int = _lib.GSR_SELECT_SET, instance: int = -1) -> None:
+        """Select the splats of the cloud (instance = -1) or of instance k's range, within [0, num_splats), that pass ALL filters:
+        each a splat_filter() or a (property, lo, hi[, rgb]) tuple, passing iff lo <= value <= hi (a NaN value never passes), 1 to
+        GSR_MAX_SPLAT_FILTERS of them.  Properties (GSR_PROP_*) come from the stored words: opacity, size (the sum of the squared
+        scales), volume (their product), isotropy (1 for a sphere, towards 0 for needles and discs) and the squared distance of the DC
+        colour from rgb.  A vacant slot is never selected.  op: GSR_SELECT_SET / _ADD / _SUBTRACT / _TOGGLE; hidden splats stay
+        unselected."""
+        fs = [f if isinstance(f, _lib.GsrSplatFilter) else splat_filter(*f) for f in filters]
+        arr = (_lib.GsrSplatFilter * max(1, len(fs)))(*fs)
+        _lib.check(_lib.lib().gsr_select_where(self._ctx, arr, len(fs), int(instance), int(op)), "gsr_select_where")
+
+    def splat_histogram(self, property: int, edges, scope: int = _lib.GSR_HISTOGRAM_KEPT, instance: int = -1, rgb=None):
+        """Histogram of a property (GSR_PROP_*; rgb for GSR_PROP_COLOR_DISTANCE) over the splats that are not hidden
+        (GSR_HISTOGRAM_KEPT) or that are selected (GSR_HISTOGRAM_SELECTED), of the cloud or of instance k's range.  edges: bins + 1
+        finite, strictly increasing values.  Returns (counts, below, above, nan, (min, max)): counts[i] of edges[i] <= v < edges[i + 1]
+        (the last bin also takes v == edges[-1]), the counts below edges[0], above edges[-1] and of NaN values, and the least and
+        greatest non-NaN value ((inf, -inf) when there is none).  Synchronises once."""
+        e = np.ascontiguousarray(edges, dtype=np.float32).reshape(-1)
+        bins = max(e.size - 1, 0)
+        counts = np.zeros(bins + 3, dtype=np.uint64)
+        mm = np.zeros(2, dtype=np.float32)
+        f = splat_filter(property, rgb=rgb)
+        fp = C.POINTER(C.c_float)
+        _lib.check(_lib.lib().gsr_splat_histogram(self._ctx, C.byref(f), int(instance), int(scope), e.ctypes.data_as(fp), bins,
+                                                  counts.ctypes.data_as(C.POINTER(C.c_uint64)), mm.ctypes.data_as(fp)),
+                   "gsr_splat_histogram")
+        return counts[:bins], int(counts[bins]), int(counts[bins + 1]), int(counts[bins + 2]), (float(mm[0]), float(mm[1]))
+
     # ---- splat transform edits (include/gsr.h "Splat transform edits") ----
     def transform_selection(self, transform, space: int = _lib.GSR_CUTOUT_FRAME, instance: int = -1, snapshot_ptr: int | None = None) -> None:
         """Move, rotate, scale or mirror the selected splats in the store.  transform: a frame-space (3, 4) [B | u] (godot_to_frame
@@ -658,6 +687,15 @@ def pack_mask(mask, n: int) -> np.ndarray:
 def unpack_mask(words: np.ndarray, n: int) -> np.ndarray:
     """The inverse of pack_mask: uint32 words -> a bool array over n splats."""
     return np.unpackbits(np.ascontiguousarray(words, dtype="<u4").view(np.uint8), bitorder="little")[:n].astype(bool)
+
+
+def splat_filter(property: int, lo: float = -np.inf, hi: float = np.inf, rgb=None) -> _lib.GsrSplatFilter:
+    """One gsr_splat_filter: the property (GSR_PROP_*) passes iff lo <= value <= hi; rgb is the reference colour of
+    GSR_PROP_COLOR_DISTANCE (default black; ignored by the other properties)."""
+    f = _lib.GsrSplatFilter()
+    f.property, f.lo, f.hi = int(property), float(lo), float(hi)
+    f.rgb[:] = [float(x) for x in (rgb if rgb is not None else (0.0, 0.0, 0.0))]
+    return f
 
 
 def delete_remap(hidden, n: int) -> np.ndarray:

@@ -705,6 +705,59 @@ GSR_API int gsr_delete_hidden(gsr_ctx *ctx, uint64_t *kept_out);
 GSR_API int gsr_duplicate_selection(gsr_ctx *ctx, uint64_t *copies_out);
 GSR_API int gsr_set_splat_count(gsr_ctx *ctx, uint64_t n);
 
+/* ---- Splat property selection: select splats by what they are -- opacity, size, shape, colour -- and histogram those properties
+ *      (no reference counterpart).  The cleanup of a capture: floaters and haze are nearly transparent, "spikes" are needle-shaped,
+ *      a trainer's sky or fog is huge, a colour cast is a colour.  A UI places a threshold on a histogram and selects by it.
+ *      Properties: a float32 value per stored splat from its stored words (source units, before model_scale and any instance
+ *      transform), in float32 with one rounding per operation, no contraction, in the order written.  S00 S01 S02 S11 = plane 1 x y z w,
+ *      S12 S22 = plane 2 x y, o = plane-2 z, f_r f_g f_b = SH values 0..2 (plane 3 x y z; with GSR_FLAG_SH_HALF half slots 0..2 of
+ *      plane 3 widened, which is exact):
+ *        GSR_PROP_OPACITY         o
+ *        GSR_PROP_SIZE            t = (S00 + S11) + S22, the sum of the squared principal scales
+ *        GSR_PROP_VOLUME          det = ((S00 ((S11 S22) - (S12 S12))) - (S01 ((S01 S22) - (S12 S02)))) + (S02 ((S01 S12) - (S11 S02))),
+ *                                 the product of the squared scales
+ *        GSR_PROP_ISOTROPY        (27 det) / ((t t) t): 1 for a sphere, towards 0 for needles and discs
+ *        GSR_PROP_COLOR_DISTANCE  c_i = 0.5 + (f_i SH_C0) (the projection's DC colour before its clamp, view-dependent terms excluded),
+ *                                 d_i = c_i - rgb_i, value ((d_r d_r) + (d_g d_g)) + (d_b d_b)
+ *      No eigen-decomposition and no transcendental function: the values are exact functions of the stored words.  A value can be
+ *      negative (det under cancellation), infinite or NaN; it is still the value.  A NaN value is outside every range.
+ *      Tested range: instance = -1 the splats of [0, n), n = gsr_stats.num_splats; instance = k instance k's source range intersected
+ *      with [0, n).  A tested splat counts only if none of its plane-0 x, y, z is NaN (so a vacant slot never counts).
+ *      gsr_select_where: inside = the tested splat passes ALL n filters, 1 <= n <= GSR_MAX_SPLAT_FILTERS; filter f passes iff
+ *        f.lo <= v && v <= f.hi (IEEE: lo > hi is empty, +-inf bounds are allowed).  `op` combines inside with the selection as every
+ *        gsr_select_* (GSR_SELECT_SET clears the splats outside the tested range), then selected &= ~hidden.  The call puts the masks
+ *        in use (so it is refused with GSR_ERR_STATE on a sharded context), is enqueued like the other selections and never
+ *        synchronises the host.  GSR_ERR_INVALID, state kept: a NULL array, n out of range, an unknown property, a NaN lo or hi, a
+ *        non-finite rgb of a GSR_PROP_COLOR_DISTANCE filter (rgb is ignored otherwise), an unknown op, an instance outside the layout.
+ *      gsr_splat_histogram: counts the property `property->property` (with `property->rgb`; lo and hi are ignored) over the tested
+ *        splats that are not hidden and, with GSR_HISTOGRAM_SELECTED, selected.  edges = bins + 1 finite, strictly increasing floats,
+ *        1 <= bins <= GSR_MAX_HISTOGRAM_BINS (linear, log-spaced or quantile edges: the rule is comparisons only).  counts has bins + 3
+ *        entries: counts[i] = #(e_i <= v < e_{i+1}), the last bin also takes v == e_bins (numpy's convention); counts[bins] = #(v < e_0),
+ *        counts[bins + 1] = #(v > e_bins), counts[bins + 2] = #NaN.  minmax (may be NULL) receives the least and the greatest non-NaN
+ *        v of the counted splats in the order of gsr_set_depth_order's ord (-0 before +0), or (+inf, -inf) when there is none.  While
+ *        the masks are not in use nothing is hidden and nothing is selected.  The call reads only: it does not put the masks in use and
+ *        is allowed on any context, sharded ones included.  It is enqueued like the store edits (on the projections' stream after an
+ *        event on the render stream, so after every upload, selection and edit enqueued before it) and synchronises the host once.
+ *        GSR_ERR_INVALID, nothing written: a NULL property, edges or counts, bins out of range, non-finite or non-increasing edges, an
+ *        unknown property, scope or instance, a non-finite rgb of a GSR_PROP_COLOR_DISTANCE property. ---- */
+#define GSR_PROP_OPACITY 0
+#define GSR_PROP_SIZE 1
+#define GSR_PROP_VOLUME 2
+#define GSR_PROP_ISOTROPY 3
+#define GSR_PROP_COLOR_DISTANCE 4
+#define GSR_MAX_SPLAT_FILTERS 8
+typedef struct gsr_splat_filter {
+    int32_t property;   /* GSR_PROP_* */
+    float lo, hi;       /* passes iff lo <= v && v <= hi (a NaN v never passes); +-inf allowed, NaN not */
+    float rgb[3];       /* GSR_PROP_COLOR_DISTANCE: the reference colour; ignored otherwise */
+} gsr_splat_filter;     /* 24 bytes */
+GSR_API int gsr_select_where(gsr_ctx *ctx, const gsr_splat_filter *filters, uint32_t n, int32_t instance, int32_t op);
+#define GSR_MAX_HISTOGRAM_BINS 1024
+#define GSR_HISTOGRAM_KEPT 0       /* every tested splat that is not hidden */
+#define GSR_HISTOGRAM_SELECTED 1   /* only the selected ones */
+GSR_API int gsr_splat_histogram(gsr_ctx *ctx, const gsr_splat_filter *property, int32_t instance, int32_t scope, const float *edges,
+                                uint32_t bins, uint64_t *counts, float minmax[2]);
+
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
  *      num_tile_splats -- persistent across calls exactly like the reference's storage buffer.
