@@ -282,6 +282,15 @@ struct CutParams {
     __host__ __device__ CutParams(const CutoutArgs &s) : set(s) {}
 };
 __device__ __forceinline__ bool mask_bit(const uint32_t *m, uint64_t s) { return ((m[s >> 5] >> (uint32_t)(s & 31u)) & 1u) != 0u; }
+// One selection operation on a mask word: GSR_SELECT_* of the selected bits and the operation's inside bits (selection.cu, neighbors.cu)
+__device__ __forceinline__ uint32_t combine_op(uint32_t op, uint32_t selected, uint32_t inside) {
+    switch (op) {
+        case GSR_SELECT_SET: return inside;
+        case GSR_SELECT_ADD: return selected | inside;
+        case GSR_SELECT_SUBTRACT: return selected & ~inside;
+        default: return selected ^ inside;   // GSR_SELECT_TOGGLE
+    }
+}
 
 // ---- selection operations (selection.cu) ----
 constexpr int SELECT_MAX_VERTICES = GSR_MAX_SELECT_VERTICES;
@@ -423,6 +432,46 @@ struct HistArgs {
     const float *edges;                           // bins + 1
 };
 int launch_splat_histogram(const HistArgs &a, int planes, bool sh_half, int sm_count, cudaStream_t stream);
+
+// ---- splat neighbourhood selection (gsr_select_neighborhood; neighbors.cu) ----
+// The grid: a participant's cell is floor(x / h) per axis in float64, clamped to [-2^62, 2^62]; a cell's 32-bit key is a hash of its
+// three coordinates, and the key's top p bits are its bucket (2^p buckets).  The pairs (key, slot) of the participants are sorted by key,
+// so a bucket is one range of the sorted entries, and within it the cells of different keys are apart.  start[b] is the first entry of
+// bucket b (start[2^p] = the participant count), with NB_IMPURE set when the bucket holds entries of more than one cell.
+constexpr uint32_t NB_IMPURE = 0x80000000u;
+constexpr uint32_t NB_NONE = 0xFFFFFFFFu;   // parent of a slot that does not participate
+constexpr uint32_t NB_SEED = 0x80000000u;   // size word of a root: the cluster holds a selected participant
+struct NeighborCounters {                   // one device block, read back page-locked
+    uint32_t n, pad;                        // participants (the sort's device count)
+    unsigned long long candidates, inside, clusters, largest;
+};
+struct NeighborArgs {
+    const float4 *plane0;
+    const uint32_t *hidden;
+    uint32_t *selected;
+    uint32_t words, op;
+    uint64_t first, count;                  // the tested range, bounded by the cloud's n
+    double h;                               // (double)radius (1 + 2^-20)
+    float r2;                               // radius radius
+    uint32_t mode, threshold;               // GSR_NEIGHBOR_*, count
+    uint32_t shift;                         // 32 - p: bucket = key >> shift
+    uint32_t *keys, *vals;                  // max_splats each: the participants' (key, slot), sorted by key
+    uint32_t *parent, *size;                // max_splats each, by slot: the union-find (the sort's ping-pong halves once it is done)
+    float4 *pos;                            // max_splats: sorted entry e = (x, y, z, slot bits) of slot vals[e]
+    uint32_t *start;                        // 2^p + 1
+    uint32_t *inside;                       // `words` scratch mask words, zero on entry and left zero: SPARSE / GROW
+    NeighborCounters *ctr;                  // zero on entry
+};
+// The grid's parameters: h, and p for a tested range of `count` slots (the least p >= 1 with 2^p >= 2 count)
+double neighbor_cell_size(float radius);
+uint32_t neighbor_bucket_bits(uint64_t count);
+// Stage launchers, in call order; the entry grids cover the tested range (the participant count is read on the device).  Between keys
+// and grid the caller sorts (keys, vals) with sort_pairs_device, parent and size as the ping-pong halves.
+int launch_neighbor_keys(const NeighborArgs &a, cudaStream_t stream);
+int launch_neighbor_grid(const NeighborArgs &a, uint64_t max_splats, cudaStream_t stream);   // also clears parent and size
+int launch_neighbor_budget(const NeighborArgs &a, cudaStream_t stream);
+int launch_neighbor_select(const NeighborArgs &a, cudaStream_t stream);   // the mode's queries, then the mask words
+int preload_neighbor_kernels();
 
 // gsr_set_depth_order: the order-preserving map of a float's bits to an unsigned word (negative: all bits flipped; positive: the sign
 // bit set).  Every finite value orders as its float does, -0 just before +0.

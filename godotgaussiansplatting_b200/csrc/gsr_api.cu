@@ -63,6 +63,14 @@ struct gsr_ctx {
     cudaEvent_t store_ready = nullptr;             // with front / back overlap: the render stream's work enqueued before the operation
     void *hist = nullptr;                          // gsr_splat_histogram: HIST_BUFFER_BYTES (counters, min / max keys, edges), first call
     unsigned char *hist_host = nullptr;            // its page-locked image (upload and read-back)
+    // gsr_select_neighborhood: the grid's scratch (GSR_NEIGHBOR_SCRATCH_BYTES_PER_SLOT per slot, the bucket starts, a sort workspace of
+    // max_splats pairs and the counters with their page-locked image), allocated by the first call and kept until gsr_destroy
+    struct Neighbors {
+        SortWorkspace ws;
+        uint32_t *keys = nullptr, *vals = nullptr, *parent = nullptr, *size = nullptr, *start = nullptr;
+        float4 *pos = nullptr;
+        NeighborCounters *ctr = nullptr, *ctr_host = nullptr;
+    } nb;
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -303,6 +311,41 @@ int alloc_depth_order(gsr_ctx *c) {
     return GSR_OK;
 }
 
+void free_neighbors(gsr_ctx::Neighbors &nb) {
+    sort_workspace_destroy(nb.ws);
+    cudaFree(nb.keys); cudaFree(nb.vals); cudaFree(nb.parent); cudaFree(nb.size); cudaFree(nb.start); cudaFree(nb.pos); cudaFree(nb.ctr);
+    if (nb.ctr_host) cudaFreeHost(nb.ctr_host);
+    nb = gsr_ctx::Neighbors();
+}
+
+// gsr_select_neighborhood's scratch for max_splats slots; on failure nothing is left allocated
+int alloc_neighbors(gsr_ctx *c, const char *where) {
+    gsr_ctx::Neighbors &nb = c->nb;
+    if (nb.ctr) return GSR_OK;
+    const uint64_t m = c->max_splats, buckets = 1ull << neighbor_bucket_bits(m);
+    int rc = sort_workspace_create(nb.ws, m, /*need_alt_buffers=*/false);
+    cudaError_t e = cudaSuccess;
+    if (!rc) {
+        e = cudaMalloc((void **)&nb.keys, sizeof(uint32_t) * m);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&nb.vals, sizeof(uint32_t) * m);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&nb.parent, sizeof(uint32_t) * m);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&nb.size, sizeof(uint32_t) * m);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&nb.pos, sizeof(float4) * m);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&nb.start, sizeof(uint32_t) * (buckets + 1));
+        if (e == cudaSuccess) e = cudaMalloc((void **)&nb.ctr, sizeof(NeighborCounters));
+        if (e == cudaSuccess) e = cudaMallocHost((void **)&nb.ctr_host, sizeof(NeighborCounters));
+    }
+    if (rc || e != cudaSuccess) {
+        free_neighbors(nb);
+        if (e != cudaSuccess) {
+            set_last_error("%s: grid scratch for %llu slots -> %s", where, (unsigned long long)m, cudaGetErrorString(e));
+            rc = e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+        }
+        return rc;
+    }
+    return GSR_OK;
+}
+
 void free_ctx(gsr_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
@@ -326,6 +369,7 @@ void free_ctx(gsr_ctx *c) {
     if (c->masks.ids_ready) cudaEventDestroy(c->masks.ids_ready);
     if (c->store_ready) cudaEventDestroy(c->store_ready);
     cudaFree(c->hist);
+    free_neighbors(c->nb);
     if (c->hist_host) cudaFreeHost(c->hist_host);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
     for (int i = 0; i < GSR_INSTANCE_RING; ++i) if (c->inst.ev[i]) cudaEventDestroy(c->inst.ev[i]);
@@ -466,7 +510,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     // happen on the frame path (and would deadlock a group whose ranks share one process: a wait kernel spins meanwhile)
     if ((rc = preload_group_kernels()) || (rc = preload_projection_kernels()) || (rc = preload_sort_kernels()) || (rc = preload_ranges_kernels()) ||
         (rc = preload_ingest_kernels()) || (rc = preload_present_kernels()) || (rc = preload_composite_kernels()) || (rc = preload_selection_kernels()) ||
-        (sh_half(c) && (rc = preload_projection_half_kernels()))) { free_ctx(c); return rc; }
+        (rc = preload_neighbor_kernels()) || (sh_half(c) && (rc = preload_projection_half_kernels()))) { free_ctx(c); return rc; }
     cudaError_t e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_last_error("init sync -> %s", cudaGetErrorString(e)); free_ctx(c); return GSR_ERR_CUDA; }
     *out = c;
@@ -2178,6 +2222,61 @@ GSR_API int gsr_splat_histogram(gsr_ctx *c, const gsr_splat_filter *property, in
         const bool any = keys[1] != INT32_MIN;
         minmax[0] = any ? ord_float(~((uint32_t)keys[0] ^ 0x80000000u)) : INFINITY;
         minmax[1] = any ? ord_float((uint32_t)keys[1] ^ 0x80000000u) : -INFINITY;
+    }
+    return GSR_OK;
+}
+
+// ---- splat neighbourhood selection: enqueued like gsr_splat_histogram; synchronises the host for the budget and for the stats --------
+GSR_API int gsr_select_neighborhood(gsr_ctx *c, const gsr_neighborhood *q, int32_t op, gsr_neighborhood_stats *stats) {
+    static const char *where = "gsr_select_neighborhood";
+    if (!c || !q) { set_last_error("%s: NULL argument", where); return GSR_ERR_INVALID; }
+    if (q->mode < GSR_NEIGHBOR_SPARSE || q->mode > GSR_NEIGHBOR_SMALL_CLUSTERS) { set_last_error("%s: unknown mode %d", where, q->mode); return GSR_ERR_INVALID; }
+    if (!(q->radius >= GSR_NEIGHBOR_MIN_RADIUS && q->radius <= GSR_NEIGHBOR_MAX_RADIUS)) {
+        set_last_error("%s: radius %g is not finite or outside [2^-60, 2^60]", where, (double)q->radius);
+        return GSR_ERR_INVALID;
+    }
+    if (q->count == 0 && (q->mode == GSR_NEIGHBOR_SPARSE || q->mode == GSR_NEIGHBOR_SMALL_CLUSTERS)) {
+        set_last_error("%s: count 0 (need >= 1)", where);
+        return GSR_ERR_INVALID;
+    }
+    if (!select_op_valid(op)) { set_last_error("%s: unknown op %d", where, op); return GSR_ERR_INVALID; }
+    NeighborArgs a;
+    memset(&a, 0, sizeof a);
+    int rc = property_range(c, where, q->instance, a.first, a.count);
+    if (rc || (rc = masks_use(c, where)) || (rc = alloc_neighbors(c, where))) return rc;
+    gsr_ctx::Neighbors &nb = c->nb;
+    a.plane0 = c->soa; a.hidden = c->masks.hidden; a.selected = c->masks.selected; a.words = c->masks.words; a.op = (uint32_t)op;
+    a.h = neighbor_cell_size(q->radius);
+    a.r2 = q->radius * q->radius;
+    a.mode = (uint32_t)q->mode; a.threshold = q->count;
+    a.shift = 32u - neighbor_bucket_bits(a.count);
+    a.keys = nb.keys; a.vals = nb.vals; a.parent = nb.parent; a.size = nb.size; a.pos = nb.pos; a.start = nb.start;
+    a.inside = c->masks.scratch;
+    a.ctr = nb.ctr;
+    cudaStream_t s;
+    if ((rc = store_stream(c, &s))) return rc;
+    GSR_CUDA_TRY(cudaMemsetAsync(nb.ctr, 0, sizeof(NeighborCounters), s));
+    if (a.count) {
+        if ((rc = launch_neighbor_keys(a, s))) return rc;
+        // the participants' pairs sorted by key; parent and size are the sort's ping-pong halves until launch_neighbor_grid clears them
+        if ((rc = sort_pairs_device(nb.ws, nb.keys, nb.vals, &nb.ctr->n, nb.parent, nb.size, s, nullptr))) return rc;
+        if ((rc = launch_neighbor_grid(a, c->max_splats, s)) || (rc = launch_neighbor_budget(a, s))) return rc;
+        GSR_CUDA_TRY(cudaMemcpyAsync(nb.ctr_host, nb.ctr, sizeof(NeighborCounters), cudaMemcpyDeviceToHost, s));
+        GSR_CUDA_TRY(cudaStreamSynchronize(s));
+        if (nb.ctr_host->candidates > GSR_MAX_NEIGHBOR_CANDIDATES) {
+            set_last_error("%s: %llu candidates at radius %g, more than GSR_MAX_NEIGHBOR_CANDIDATES (%llu)", where, nb.ctr_host->candidates,
+                           (double)q->radius, (unsigned long long)GSR_MAX_NEIGHBOR_CANDIDATES);
+            return GSR_ERR_INVALID;
+        }
+    }
+    if ((rc = launch_neighbor_select(a, s))) return rc;
+    if (stats) {
+        GSR_CUDA_TRY(cudaMemcpyAsync(nb.ctr_host, nb.ctr, sizeof(NeighborCounters), cudaMemcpyDeviceToHost, s));
+        GSR_CUDA_TRY(cudaStreamSynchronize(s));
+        const NeighborCounters &k = *nb.ctr_host;
+        const bool clusters = q->mode == GSR_NEIGHBOR_CONNECTED || q->mode == GSR_NEIGHBOR_SMALL_CLUSTERS;
+        stats->participants = k.n; stats->inside = k.inside; stats->candidates = k.candidates;
+        stats->clusters = clusters ? k.clusters : 0ull; stats->largest_cluster = clusters ? k.largest : 0ull;
     }
     return GSR_OK;
 }

@@ -17,15 +17,6 @@ namespace {
 constexpr int SEL_THREADS = 256;
 constexpr int SEL_WARPS = SEL_THREADS / 32;
 
-__device__ __forceinline__ uint32_t combine_op(uint32_t op, uint32_t selected, uint32_t inside) {
-    switch (op) {
-        case GSR_SELECT_SET: return inside;
-        case GSR_SELECT_ADD: return selected | inside;
-        case GSR_SELECT_SUBTRACT: return selected & ~inside;
-        default: return selected ^ inside;   // GSR_SELECT_TOGGLE
-    }
-}
-
 // pix(M, q) of include/gsr.h (the projection's image_pos without the load-in term); w = clip[3]
 __device__ __forceinline__ void select_pix(const float *M, float q0, float q1, float q2, float fw, float fh, float &x, float &y, float &w) {
     const float *V = M, *P = M + 16;

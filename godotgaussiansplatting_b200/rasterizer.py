@@ -374,6 +374,17 @@ class GaussianSplattingRasterizer:
         arr = (_lib.GsrSplatFilter * max(1, len(fs)))(*fs)
         _lib.check(_lib.lib().gsr_select_where(self._ctx, arr, len(fs), int(instance), int(op)), "gsr_select_where")
 
+    def select_neighborhood(self, mode: int, radius: float, count: int = 1, op: int = _lib.GSR_SELECT_SET, instance: int = -1) -> dict:
+        """Select splats by their neighbourhood (include/gsr.h "Splat neighbourhood selection"): participants are the splats of the cloud
+        (instance = -1) or of instance k's range that are not hidden and have a finite position; two are neighbours within `radius`
+        (source units).  mode: GSR_NEIGHBOR_SPARSE (fewer than `count` neighbours), _GROW (selected or next to a selected splat),
+        _CONNECTED (the clusters holding a selected splat), _SMALL_CLUSTERS (clusters of fewer than `count` splats); op as every
+        select_*.  Returns the stats: participants, inside, candidates, clusters, largest_cluster.  Synchronises at most twice."""
+        q = _lib.GsrNeighborhood(int(mode), float(radius), int(count), int(instance))
+        st = _lib.GsrNeighborhoodStats()
+        _lib.check(_lib.lib().gsr_select_neighborhood(self._ctx, C.byref(q), int(op), C.byref(st)), "gsr_select_neighborhood")
+        return {k: int(getattr(st, k)) for k, _ in _lib.GsrNeighborhoodStats._fields_}
+
     def splat_histogram(self, property: int, edges, scope: int = _lib.GSR_HISTOGRAM_KEPT, instance: int = -1, rgb=None):
         """Histogram of a property (GSR_PROP_*; rgb for GSR_PROP_COLOR_DISTANCE) over the splats that are not hidden
         (GSR_HISTOGRAM_KEPT) or that are selected (GSR_HISTOGRAM_SELECTED), of the cloud or of instance k's range.  edges: bins + 1

@@ -758,6 +758,59 @@ GSR_API int gsr_select_where(gsr_ctx *ctx, const gsr_splat_filter *filters, uint
 GSR_API int gsr_splat_histogram(gsr_ctx *ctx, const gsr_splat_filter *property, int32_t instance, int32_t scope, const float *edges,
                                 uint32_t bins, uint64_t *counts, float minmax[2]);
 
+/* ---- Splat neighbourhood selection: select splats by the splats around them -- isolated floaters, one step of "select more", the
+ *      object under a clicked splat, every small clump (no reference counterpart).  Queries run on a spatial grid on the GPU.
+ *      Participants: the splats of the tested range (the rule of gsr_select_where: instance = -1 [0, n), instance = k instance k's
+ *        source range intersected with [0, n)) whose hidden bit is 0 and whose plane-0 x, y and z are all finite.  Vacant slots, NaN
+ *        and infinite positions and hidden splats never participate and are never inside.
+ *      Neighbours: for participants i != j, dx = x_j - x_i (dy, dz the same way) and d2 = ((dx dx) + (dy dy)) + (dz dz), all float32,
+ *        one rounding per operation, no contraction; j is a neighbour of i iff d2 <= r2, r2 = radius radius in float32.  The relation is
+ *        symmetric (fl(a - b) = -fl(b - a)); coincident splats (a duplicate and its copy) are neighbours.  A cluster is a connected
+ *        component of the graph of participants with these edges (single linkage at `radius`).  radius is in source units (the stored
+ *        position, before model_scale and any instance transform).
+ *      Modes (`selected` = the selection when the call runs, restricted to participants):
+ *        GSR_NEIGHBOR_SPARSE          inside = participants with fewer than `count` neighbours (count >= 1; 1 = no neighbour at all)
+ *        GSR_NEIGHBOR_GROW            inside = participants that are selected or have a selected neighbour (one step, not a fixed point)
+ *        GSR_NEIGHBOR_CONNECTED       inside = the participants of every cluster that holds a selected participant
+ *        GSR_NEIGHBOR_SMALL_CLUSTERS  inside = the participants of clusters of fewer than `count` participants ("keep the main object":
+ *                                     count = largest_cluster of an earlier call)
+ *      `op` combines inside with the selection as every gsr_select_* (GSR_SELECT_SET clears everything outside the tested range), then
+ *      selected &= ~hidden.  The call puts the masks in use (so it is refused with GSR_ERR_STATE on a sharded context).
+ *      Grid and work measure (part of the contract, so that a refusal is deterministic): h = (double)radius (1 + 2^-20); a splat's cell
+ *        is floor(x / h), floor(y / h), floor(z / h) in float64, each clamped to [-2^62, 2^62]; candidates = the sum over participants
+ *        of the number of participants in the 27 cells around its own cell.  candidates > GSR_MAX_NEIGHBOR_CANDIDATES returns
+ *        GSR_ERR_INVALID with the masks unchanged (the message gives the count): a radius far too large for the cloud is a refused call,
+ *        not a kernel that runs for minutes.
+ *      Ordering: enqueued like gsr_splat_histogram (after every upload, edit and selection enqueued before it, before every frame
+ *        enqueued after it); it synchronises the host at most twice (the budget check and the stats): a click-time call.
+ *      Memory: scratch of GSR_NEIGHBOR_SCRATCH_BYTES_PER_SLOT bytes per slot of max_splats, plus 4 B per hash bucket (the least power
+ *        of two >= 2 max_splats: 8 to 16 B per slot) and the sort's look-back words, allocated by the first call and kept until
+ *        gsr_destroy; separate from the frame's buffers.  GSR_ERR_OOM keeps the state.
+ *      stats (may be NULL): participants, inside (participants inside), candidates; clusters and largest_cluster for CONNECTED and
+ *        SMALL_CLUSTERS, 0 otherwise.  Written only when the call succeeds.
+ *      GSR_ERR_INVALID, state kept, checked in this order: a NULL q; an unknown mode; a radius that is not finite or outside
+ *        [GSR_NEIGHBOR_MIN_RADIUS, GSR_NEIGHBOR_MAX_RADIUS] (so that r2 is a normal float: the grid's argument needs it); count = 0 for
+ *        SPARSE and SMALL_CLUSTERS; an unknown op; an instance outside the layout. ---- */
+#define GSR_NEIGHBOR_SPARSE 0           /* inside: fewer than `count` other participants within `radius` */
+#define GSR_NEIGHBOR_GROW 1             /* inside: selected, or a selected participant within `radius` */
+#define GSR_NEIGHBOR_CONNECTED 2        /* inside: in a cluster that holds a selected participant */
+#define GSR_NEIGHBOR_SMALL_CLUSTERS 3   /* inside: in a cluster of fewer than `count` participants */
+#define GSR_MAX_NEIGHBOR_CANDIDATES (1ull << 34)
+#define GSR_NEIGHBOR_MIN_RADIUS 0x1p-60f
+#define GSR_NEIGHBOR_MAX_RADIUS 0x1p+60f
+#define GSR_NEIGHBOR_SCRATCH_BYTES_PER_SLOT 32
+typedef struct gsr_neighborhood {
+    int32_t mode;       /* GSR_NEIGHBOR_* */
+    float radius;       /* source units; finite, in [GSR_NEIGHBOR_MIN_RADIUS, GSR_NEIGHBOR_MAX_RADIUS] */
+    uint32_t count;     /* SPARSE, SMALL_CLUSTERS: the threshold (>= 1); ignored otherwise */
+    int32_t instance;   /* -1: [0, n); k: instance k's source range intersected with [0, n) */
+} gsr_neighborhood;     /* 16 bytes */
+typedef struct gsr_neighborhood_stats {
+    uint64_t participants, inside, candidates;   /* candidates: the work measure above */
+    uint64_t clusters, largest_cluster;           /* CONNECTED / SMALL_CLUSTERS; 0 otherwise */
+} gsr_neighborhood_stats;                         /* 40 bytes */
+GSR_API int gsr_select_neighborhood(gsr_ctx *ctx, const gsr_neighborhood *q, int32_t op, gsr_neighborhood_stats *stats /* may be NULL */);
+
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
  *      num_tile_splats -- persistent across calls exactly like the reference's storage buffer.
