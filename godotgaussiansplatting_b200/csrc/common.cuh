@@ -391,6 +391,27 @@ int launch_duplicate_finish(uint64_t n, uint64_t S, uint32_t *hidden, uint32_t *
 // counts[0] = popcount of the selected bits below n
 int launch_count_selected(const uint32_t *selected, uint64_t n, unsigned long long *counts, cudaStream_t stream);
 
+// ---- splat export (gsr_export_ply; selection.cu) ----
+// The splats of [0, n) that are in scope (hidden == nullptr: the masks are not in use, every splat is kept and none selected) and not
+// vacant become 3DGS vertex rows of degree `degree`, in store order.  A counting pass gives their number; the writing pass places a
+// CTA's rows (one tile of COMPACT_TILE_WORDS mask words) at its prefix with the look-back of compact_store_kernel.
+__host__ __device__ constexpr uint32_t export_row_floats(int degree) { return 17u + 3u * (uint32_t)((degree + 1) * (degree + 1) - 1); }
+struct ExportArgs {
+    const float4 *soa;
+    uint64_t plane_stride;
+    uint64_t n;
+    const uint32_t *hidden, *selected;
+    uint32_t selected_only;            // GSR_EXPORT_SELECTED
+    int32_t degree;                    // d, 0 .. the stored degree
+    float *dst;                        // device memory: the rows, export_row_floats(degree) floats each
+    unsigned long long *lookback;      // compact_lookback_words(ceil(n / 32)) words, zeroed before the writing launch
+    unsigned long long *count;         // zeroed before the counting launch: the number of exported splats
+};
+// The dynamic shared memory of a writing CTA: its rows
+__host__ __device__ constexpr size_t export_shared_bytes(int degree) { return sizeof(float) * COMPACT_THREADS * export_row_floats(degree); }
+int launch_export_count(const ExportArgs &a, cudaStream_t stream);
+int launch_export_rows(const ExportArgs &a, int bands, bool sh_half, cudaStream_t stream);
+
 // ---- splat property selection (gsr_select_where, gsr_splat_histogram; selection.cu) ----
 // The planes a property reads beyond plane 0 (a size, volume or isotropy reads planes 1 and 2).  The kernels are templated on the union
 // of a filter set's bits, so each reads only the planes its set needs.

@@ -71,6 +71,8 @@ struct gsr_ctx {
         float4 *pos = nullptr;
         NeighborCounters *ctr = nullptr, *ctr_host = nullptr;
     } nb;
+    // gsr_export_ply: the exported count, then the look-back words of ceil(max_splats / 256) tiles and the ticket; first call
+    unsigned long long *export_words = nullptr;
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -369,6 +371,7 @@ void free_ctx(gsr_ctx *c) {
     if (c->masks.ids_ready) cudaEventDestroy(c->masks.ids_ready);
     if (c->store_ready) cudaEventDestroy(c->store_ready);
     cudaFree(c->hist);
+    cudaFree(c->export_words);
     free_neighbors(c->nb);
     if (c->hist_host) cudaFreeHost(c->hist_host);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
@@ -2278,6 +2281,73 @@ GSR_API int gsr_select_neighborhood(gsr_ctx *c, const gsr_neighborhood *q, int32
         stats->participants = k.n; stats->inside = k.inside; stats->candidates = k.candidates;
         stats->clusters = clusters ? k.clusters : 0ull; stats->largest_cluster = clusters ? k.largest : 0ull;
     }
+    return GSR_OK;
+}
+
+// ---- splat export: enqueued like gsr_splat_histogram; synchronises the host for the count, and once more for rows into host memory ----
+GSR_API int gsr_export_ply(gsr_ctx *c, int32_t scope, int32_t sh_degree, void *dst, uint64_t dst_rows, uint64_t *rows_out) {
+    static const char *where = "gsr_export_ply";
+    if (!c || !rows_out) { set_last_error("%s: NULL argument", where); return GSR_ERR_INVALID; }
+    if (scope != GSR_EXPORT_KEPT && scope != GSR_EXPORT_SELECTED) { set_last_error("%s: unknown scope %d", where, scope); return GSR_ERR_INVALID; }
+    if (sh_degree < -1 || sh_degree > c->sh_bands - 1) {
+        set_last_error("%s: sh_degree %d, need -1 .. the stored degree %d", where, sh_degree, c->sh_bands - 1);
+        return GSR_ERR_INVALID;
+    }
+    const int degree = sh_degree < 0 ? c->sh_bands - 1 : sh_degree;
+    const uint64_t row_bytes = sizeof(float) * export_row_floats(degree);
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    ExportArgs a;
+    memset(&a, 0, sizeof a);
+    a.soa = c->soa; a.plane_stride = c->plane_stride; a.n = c->num_splats;
+    a.hidden = c->masks.on ? c->masks.hidden : nullptr; a.selected = c->masks.on ? c->masks.selected : nullptr;
+    a.selected_only = scope == GSR_EXPORT_SELECTED;
+    a.degree = degree;
+    unsigned long long rows = 0ull;
+    cudaStream_t s = nullptr;
+    if (a.n && !(a.selected_only && !a.hidden)) {   // while the masks are not in use nothing is selected
+        if (!c->export_words) {
+            const size_t bytes = sizeof(unsigned long long) * (1ull + compact_lookback_words((uint32_t)((c->max_splats + 31ull) / 32ull)));
+            cudaError_t e = cudaMalloc((void **)&c->export_words, bytes);
+            if (e != cudaSuccess) {
+                c->export_words = nullptr;
+                set_last_error("%s: look-back words of %zu B -> %s", where, bytes, cudaGetErrorString(e));
+                return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+            }
+        }
+        a.count = c->export_words; a.lookback = c->export_words + 1;
+        if ((rc = store_stream(c, &s)) || (rc = launch_export_count(a, s))) return rc;
+        GSR_CUDA_TRY(cudaMemcpyAsync(&rows, a.count, sizeof rows, cudaMemcpyDeviceToHost, s));
+        GSR_CUDA_TRY(cudaStreamSynchronize(s));
+    }
+    *rows_out = rows;
+    if (!dst) return GSR_OK;
+    if (dst_rows < rows) {
+        set_last_error("%s: %llu exported rows, dst holds %llu", where, rows, (unsigned long long)dst_rows);
+        return GSR_ERR_INVALID;
+    }
+    if (!rows) return GSR_OK;
+    cudaPointerAttributes pa;
+    GSR_CUDA_TRY(cudaPointerGetAttributes(&pa, dst));
+    const bool device = pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged;
+    float *out = static_cast<float *>(dst);
+    if (!device) {   // host memory: rows x row_bytes of device staging, freed before the call returns
+        cudaError_t e = cudaMalloc((void **)&out, rows * row_bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            set_last_error("%s: staging of %llu B for host memory -> %s (export into device memory instead)", where,
+                           (unsigned long long)(rows * row_bytes), cudaGetErrorString(e));
+            return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+        }
+    }
+    a.dst = out;
+    rc = launch_export_rows(a, c->sh_bands, sh_half(c), s);
+    cudaError_t e = cudaSuccess;
+    if (!rc && !device) e = cudaMemcpyAsync(dst, out, rows * row_bytes, cudaMemcpyDeviceToHost, s);
+    if (!rc && e == cudaSuccess) e = cudaStreamSynchronize(s);
+    if (!device) cudaFree(out);
+    if (rc) return rc;
+    GSR_CUDA_TRY(e);
     return GSR_OK;
 }
 

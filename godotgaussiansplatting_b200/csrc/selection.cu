@@ -5,7 +5,8 @@
 // update is atomic, even for an instance range that starts inside a word.  The grid covers every word of [0, max_splats): SET clears the
 // splats outside the tested range.  The ID-plane operation scatters into a scratch mask with atomicOr (pixels share splats) and a
 // second kernel combines it.  Every kernel ends a word with selected &= ~hidden.  Delete and duplicate (compact_store_kernel) move whole
-// splats between indices with one chained scan over the mask words.  Property selection (select_where_kernel) has the region
+// splats between indices with one chained scan over the mask words; export (export_ply_kernel) places its PLY rows with the same scan and
+// decomposes each covariance in float64.  Property selection (select_where_kernel) has the region
 // operations' shape and tests the stored words; the property histogram (splat_histogram_kernel) is a grid-stride pass with the same reads.
 // The arithmetic follows the library's deterministic math (-fmad=false): one rounding per operator, in the order of include/gsr.h.
 #include "common.cuh"
@@ -475,10 +476,207 @@ __global__ void __launch_bounds__(SEL_THREADS) count_selected_kernel(const uint3
     if ((threadIdx.x & 31u) == 0u && ns) atomicAdd(counts, (unsigned long long)ns);
 }
 
-// ---- gsr_select_where / gsr_splat_histogram: per-splat properties of the stored words (include/gsr.h "Splat property selection") ----
 // A tested splat counts only if none of its plane-0 x, y, z is NaN (a vacant slot never counts).
 __device__ __forceinline__ bool splat_vacant(const float4 &p0) { return p0.x != p0.x || p0.y != p0.y || p0.z != p0.z; }
 
+// ---- gsr_export_ply: the exported splats of [0, n) as 3DGS vertex rows (include/gsr.h "Splat export") ----
+// The exported bits of mask word w (< ceil(n / 32)): lane l tests splat 32 w + l.  Plane 0 is read only for a splat in scope.
+__device__ __forceinline__ uint32_t export_bits(const ExportArgs &a, uint32_t w, uint32_t lane) {
+    const uint32_t valid = 32ull * (w + 1) <= a.n ? 0xffffffffu : (1u << (uint32_t)(a.n & 31ull)) - 1u;
+    const uint32_t scope = a.hidden ? (a.selected_only ? a.selected[w] : ~a.hidden[w]) & valid : valid;
+    bool in = (scope >> lane) & 1u;
+    if (in) in = !splat_vacant(__ldg(a.soa + 32ull * w + lane));
+    return __ballot_sync(0xffffffffu, in);
+}
+
+// *count += the exported splats: a warp per mask word (grid-stride), one atomic per warp
+__global__ void __launch_bounds__(SEL_THREADS) export_count_kernel(const __grid_constant__ ExportArgs a) {
+    const uint32_t lane = threadIdx.x & 31u, nw = (uint32_t)((a.n + 31ull) >> 5);
+    uint32_t c = 0u;
+    for (uint32_t w = blockIdx.x * SEL_WARPS + (threadIdx.x >> 5); w < nw; w += gridDim.x * SEL_WARPS) c += (uint32_t)__popc(export_bits(a, w, lane));
+    if (lane == 0u && c) atomicAdd(a.count, (unsigned long long)c);
+}
+
+// One cyclic-Jacobi rotation of the symmetric A in the plane (P, Q), accumulated into the columns of V (Numerical Recipes' jacobi):
+// A[P][Q] becomes exactly 0.  With `late` (after three sweeps) an element that is negligible beside both diagonal entries is zeroed
+// without a rotation.
+template <int P, int Q>
+__device__ __forceinline__ void jacobi_rotate(double (&A)[3][3], double (&V)[3][3], bool late) {
+    constexpr int R = 3 - P - Q;
+    const double apq = A[P][Q];
+    if (apq == 0.0) return;
+    const double g = 100.0 * fabs(apq);
+    if (late && fabs(A[P][P]) + g == fabs(A[P][P]) && fabs(A[Q][Q]) + g == fabs(A[Q][Q])) {
+        A[P][Q] = A[Q][P] = 0.0;
+        return;
+    }
+    const double theta = (A[Q][Q] - A[P][P]) / (2.0 * apq);
+    double t = 1.0 / (fabs(theta) + sqrt(theta * theta + 1.0));   // theta^2 = inf: t = 0, apq is negligible
+    if (theta < 0.0) t = -t;
+    const double c = 1.0 / sqrt(t * t + 1.0), s = t * c, tau = s / (1.0 + c);
+    A[P][P] -= t * apq;
+    A[Q][Q] += t * apq;
+    A[P][Q] = A[Q][P] = 0.0;
+    const double arp = A[R][P], arq = A[R][Q];
+    A[R][P] = A[P][R] = arp - s * (arq + arp * tau);
+    A[R][Q] = A[Q][R] = arq + s * (arp - arq * tau);
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        const double vp = V[r][P], vq = V[r][Q];
+        V[r][P] = vp - s * (vq + vp * tau);
+        V[r][Q] = vq + s * (vp - vq * tau);
+    }
+}
+
+// scale and rot of the covariance words (S00 S01 S02 S11 S12 S22) by the rule of include/gsr.h "Splat export"
+__device__ __forceinline__ void export_scale_rot(const float4 &p1, const float4 &p2, float *out) {
+    const float w6[6] = {p1.x, p1.y, p1.z, p1.w, p2.x, p2.y};
+    bool finite = true;
+#pragma unroll
+    for (int i = 0; i < 6; ++i) finite = finite && fabsf(w6[i]) <= 3.402823466e38f;
+    if (!finite) {
+        const float qnan = __uint_as_float(0x7FC00000u);
+        out[0] = out[1] = out[2] = qnan;
+        out[3] = 1.0f; out[4] = out[5] = out[6] = 0.0f;
+        return;
+    }
+    double A[3][3] = {{w6[0], w6[1], w6[2]}, {w6[1], w6[3], w6[4]}, {w6[2], w6[4], w6[5]}};
+    double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
+#pragma unroll 1
+    for (int sweep = 0; sweep < 16; ++sweep) {
+        if (A[0][1] == 0.0 && A[0][2] == 0.0 && A[1][2] == 0.0) break;
+        jacobi_rotate<0, 1>(A, V, sweep >= 3);
+        jacobi_rotate<0, 2>(A, V, sweep >= 3);
+        jacobi_rotate<1, 2>(A, V, sweep >= 3);
+    }
+    double l[3] = {A[0][0], A[1][1], A[2][2]};
+    // ascending eigenvalues with their columns: compare-exchange (0, 1), (1, 2), (0, 1)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const int i = k == 1 ? 1 : 0, j = i + 1;
+        if (l[j] < l[i]) {
+            const double t = l[i]; l[i] = l[j]; l[j] = t;
+#pragma unroll
+            for (int r = 0; r < 3; ++r) { const double v = V[r][i]; V[r][i] = V[r][j]; V[r][j] = v; }
+        }
+    }
+    const double det = V[0][0] * (V[1][1] * V[2][2] - V[1][2] * V[2][1]) - V[0][1] * (V[1][0] * V[2][2] - V[1][2] * V[2][0]) +
+                       V[0][2] * (V[1][0] * V[2][1] - V[1][1] * V[2][0]);
+    if (det < 0.0) { V[0][0] = -V[0][0]; V[1][0] = -V[1][0]; V[2][0] = -V[2][0]; }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) out[i] = (float)(0.5 * log(l[i] > 2.2250738585072014e-308 ? l[i] : 2.2250738585072014e-308));
+    // Shepperd: the largest of 4w^2 - 1 = tr, and 4x^2 - 1, 4y^2 - 1, 4z^2 - 1 (the diagonal entries), first on a tie
+    const double tr = (V[0][0] + V[1][1]) + V[2][2];
+    int k = 0;
+    double best = tr;
+#pragma unroll
+    for (int i = 0; i < 3; ++i) if (V[i][i] > best) { best = V[i][i]; k = i + 1; }
+    double q[4];
+    if (k == 0) {
+        const double w = 0.5 * sqrt(1.0 + tr), f = 0.25 / w;
+        q[0] = w; q[1] = (V[2][1] - V[1][2]) * f; q[2] = (V[0][2] - V[2][0]) * f; q[3] = (V[1][0] - V[0][1]) * f;
+    }
+#pragma unroll
+    for (int kk = 1; kk <= 3; ++kk) {   // unrolled, so that every index is a constant and V and q stay in registers
+        if (k != kk) continue;
+        const int a = kk - 1, b = kk % 3, c = (kk + 1) % 3;
+        const double v = 0.5 * sqrt(((1.0 + V[a][a]) - V[b][b]) - V[c][c]), f = 0.25 / v;
+        q[0] = (V[c][b] - V[b][c]) * f;
+        q[1 + a] = v; q[1 + b] = (V[b][a] + V[a][b]) * f; q[1 + c] = (V[c][a] + V[a][c]) * f;
+    }
+    const double norm = sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3]), sg = q[0] < 0.0 ? -1.0 : 1.0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) out[3 + i] = (float)(sg * (q[i] / norm));
+}
+
+// The writing pass.  A CTA owns COMPACT_TILE_WORDS consecutive mask words (one splat per thread, its tile from an atomic ticket like
+// compact_store_kernel), ranks its exported splats, publishes its count and looks back for its prefix excl (the pass only reads the
+// store, so it publishes its PREFIX right after).  Each exported splat reads planes 1, 2 and the SH planes of degree d and writes its
+// row into shared memory at its rank; the CTA's rows [excl, excl + agg) are one contiguous range of dst, stored with consecutive threads
+// on consecutive 4-byte words.
+#ifndef EXPORT_CTA_ROWS
+#ifndef GSR_CPU_EMU
+#define EXPORT_CTA_ROWS(name) extern __shared__ float name[]
+#else  // tests/kernel_emu, one CTA at a time: the largest row buffer
+#define EXPORT_CTA_ROWS(name) __shared__ float name[COMPACT_THREADS * export_row_floats(3)]
+#endif
+#endif
+template <int BANDS, bool HALF>
+__global__ void __launch_bounds__(COMPACT_THREADS) export_ply_kernel(const __grid_constant__ ExportArgs a) {
+    constexpr int K = sh_coeffs(BANDS), P = sh_planes(BANDS, HALF);
+    COMPACT_CTA_SHARED(CompactShared, sh);
+    EXPORT_CTA_ROWS(rows);
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    const uint32_t nw = (uint32_t)((a.n + 31ull) >> 5), tiles = (nw + COMPACT_TILE_WORDS - 1) / COMPACT_TILE_WORDS;
+    volatile unsigned long long *status = a.lookback;
+    if (tid == 0) sh.tile = (uint32_t)atomicAdd(a.lookback + tiles, 1ull);
+    __syncthreads();
+    const uint32_t tile = sh.tile, w = tile * COMPACT_TILE_WORDS + warp;
+    const uint32_t bits = w < nw ? export_bits(a, w, lane) : 0u;
+    if (lane == 0) sh.warp_count[warp] = (uint32_t)__popc(bits);
+    __syncthreads();
+    uint32_t rank = (uint32_t)__popc(bits & ((1u << lane) - 1u)), agg = 0u;
+#pragma unroll
+    for (uint32_t i = 0; i < COMPACT_TILE_WORDS; ++i) {
+        const uint32_t c = sh.warp_count[i];
+        rank += i < warp ? c : 0u;
+        agg += c;
+    }
+    if (tid == 0) status[tile] = CS_EARLY | agg;
+    if (warp == 0) {
+        const unsigned long long e = tile ? lookback_exclusive(status, tile, CS_EARLY | CS_AGG | CS_PREFIX) : 0ull;
+        if (lane == 0) {
+            sh.excl = e;
+            status[tile] = CS_PREFIX | (e + agg);
+        }
+    }
+    const uint32_t RW = export_row_floats(a.degree);
+    if ((bits >> lane) & 1u) {
+        const int Kd = (a.degree + 1) * (a.degree + 1), Pd = HALF ? (3 * Kd + 7) / 8 : (3 * Kd + 3) / 4;
+        const uint64_t s = 32ull * w + lane, st = a.plane_stride;
+        const float4 *src = a.soa + s;
+        const float4 p0 = __ldg(src), p1 = __ldg(src + st), p2 = __ldg(src + 2 * st);
+        float c[HALF ? 8 * P : 4 * P];
+#pragma unroll
+        for (int k = 0; k < P; ++k) {
+            float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            if (k < Pd) v = __ldg(src + (uint64_t)(3 + k) * st);
+            if constexpr (HALF) {
+                const uint32_t u[4] = {__float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w)};
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    c[8 * k + 2 * j] = half_bits_to_float(u[j] & 0xFFFFu);
+                    c[8 * k + 2 * j + 1] = half_bits_to_float(u[j] >> 16);
+                }
+            } else {
+                c[4 * k + 0] = v.x; c[4 * k + 1] = v.y; c[4 * k + 2] = v.z; c[4 * k + 3] = v.w;
+            }
+        }
+        float *r = rows + (size_t)rank * RW;
+        r[0] = p0.x; r[1] = p0.y; r[2] = p0.z;
+        r[3] = r[4] = r[5] = 0.0f;
+        r[6] = c[0]; r[7] = c[1]; r[8] = c[2];
+#pragma unroll
+        for (int k = 1; k < K; ++k) {
+            if (k < Kd) {
+#pragma unroll
+                for (int ch = 0; ch < 3; ++ch) r[9 + ch * (Kd - 1) + (k - 1)] = c[3 * k + ch];
+            }
+        }
+        float *t = r + 9 + 3 * (Kd - 1);
+        const double o = (double)p2.z;
+        double logit = log(o) - log1p(-o);
+        logit = logit != logit ? 0.0 : logit < -104.0 ? -104.0 : logit > 104.0 ? 104.0 : logit;
+        t[0] = (float)logit;
+        export_scale_rot(p1, p2, t + 1);
+    }
+    __syncthreads();
+    const unsigned long long excl = sh.excl;
+    float *dst = a.dst + excl * RW;
+    for (uint32_t i = tid; i < agg * RW; i += COMPACT_THREADS) dst[i] = rows[i];
+}
+
+// ---- gsr_select_where / gsr_splat_histogram: per-splat properties of the stored words (include/gsr.h "Splat property selection") ----
 // The planes of one splat beyond plane 0, each loaded the first time a property needs it, so a splat that failed an earlier filter
 // reads nothing more.  PL: the prop_planes bits of the filter set (a plane outside PL is never read); HALF: the SH format of plane 3.
 // Every value in float32, one rounding per operation, in the order of include/gsr.h.
@@ -862,6 +1060,47 @@ int launch_count_selected(const uint32_t *selected, uint64_t n, unsigned long lo
     return GSR_OK;
 }
 
+int launch_export_count(const ExportArgs &a, cudaStream_t stream) {
+    GSR_CUDA_TRY(cudaMemsetAsync(a.count, 0, sizeof(unsigned long long), stream));
+    const uint32_t words = (uint32_t)((a.n + 31ull) >> 5);
+    if (!words) return GSR_OK;
+    const uint32_t need = (words + SEL_WARPS - 1) / SEL_WARPS, blocks = need < 2048u ? need : 2048u;
+    export_count_kernel<<<blocks, SEL_THREADS, 0, stream>>>(a);
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
+namespace {
+template <int BANDS, bool HALF>
+int launch_export_variant(const ExportArgs &a, uint32_t blocks, cudaStream_t stream) {
+    const size_t smem = export_shared_bytes(a.degree);
+    if (smem > 48 * 1024) GSR_CUDA_TRY(cudaFuncSetAttribute(export_ply_kernel<BANDS, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    export_ply_kernel<BANDS, HALF><<<blocks, COMPACT_THREADS, smem, stream>>>(a);
+    return GSR_OK;
+}
+}  // namespace
+
+int launch_export_rows(const ExportArgs &a, int bands, bool sh_half, cudaStream_t stream) {
+    if (a.n == 0) return GSR_OK;
+    const uint32_t words = (uint32_t)((a.n + 31ull) >> 5);
+    const uint32_t blocks = (uint32_t)compact_lookback_words(words) - 1u;
+    GSR_CUDA_TRY(cudaMemsetAsync(a.lookback, 0, sizeof(unsigned long long) * compact_lookback_words(words), stream));
+    int rc;
+    switch (bands * 2 + (sh_half ? 1 : 0)) {
+        case 2: rc = launch_export_variant<1, false>(a, blocks, stream); break;
+        case 3: rc = launch_export_variant<1, true>(a, blocks, stream); break;
+        case 4: rc = launch_export_variant<2, false>(a, blocks, stream); break;
+        case 5: rc = launch_export_variant<2, true>(a, blocks, stream); break;
+        case 6: rc = launch_export_variant<3, false>(a, blocks, stream); break;
+        case 7: rc = launch_export_variant<3, true>(a, blocks, stream); break;
+        case 8: rc = launch_export_variant<4, false>(a, blocks, stream); break;
+        default: rc = launch_export_variant<4, true>(a, blocks, stream); break;
+    }
+    if (rc) return rc;
+    GSR_CUDA_TRY(cudaGetLastError());
+    return GSR_OK;
+}
+
 namespace {
 template <bool HALF, int PL>
 void launch_property_variant(const WhereArgs &a, uint32_t blocks, cudaStream_t stream) {
@@ -990,6 +1229,15 @@ int preload_selection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, delete_finish_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, duplicate_finish_kernel));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, count_selected_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_count_kernel));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<1, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<1, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<2, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<2, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<3, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<3, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<4, false>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, export_ply_kernel<4, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P2>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P1 | PROP_P2>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_P3>));

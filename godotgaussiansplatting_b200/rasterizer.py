@@ -473,6 +473,22 @@ class GaussianSplattingRasterizer:
         bands = self._sh_bands if self._sh_bands else 4
         return store_to_table(store, n, bands, bool(self._flags & _lib.GSR_FLAG_SH_HALF), hidden[:n])
 
+    def export_ply(self, scope: int = _lib.GSR_EXPORT_KEPT, sh_degree: int = -1) -> PlyFile:
+        """The edited cloud exported on the GPU (include/gsr.h "Splat export"): the splats of [0, num_splats) that are not hidden
+        (GSR_EXPORT_KEPT) or that are selected (GSR_EXPORT_SELECTED), vacant slots skipped, as the float32 rows of a 3DGS PLY of SH
+        degree sh_degree (-1: the stored degree), in store order, with their degree_properties names.  r.export_ply().save(path)
+        writes the file.  Synchronises twice (the count, then the rows)."""
+        from .ply_file import degree_properties
+        L, rows = _lib.lib(), C.c_uint64(0)
+        _lib.check(L.gsr_export_ply(self._ctx, int(scope), int(sh_degree), None, 0, C.byref(rows)), "gsr_export_ply")
+        degree = (self._sh_bands if self._sh_bands else 4) - 1 if int(sh_degree) < 0 else int(sh_degree)
+        names = degree_properties(degree)
+        table = np.empty((rows.value, len(names)), dtype=np.float32)
+        if rows.value:
+            _lib.check(L.gsr_export_ply(self._ctx, int(scope), int(sh_degree), C.c_void_p(table.ctypes.data), table.shape[0], C.byref(rows)),
+                       "gsr_export_ply")
+        return PlyFile.from_array(table, names)
+
     def _plane_stride(self) -> int:
         return (self._max_splats + 255) // 256 * 256
 

@@ -811,6 +811,46 @@ typedef struct gsr_neighborhood_stats {
 } gsr_neighborhood_stats;                         /* 40 bytes */
 GSR_API int gsr_select_neighborhood(gsr_ctx *ctx, const gsr_neighborhood *q, int32_t op, gsr_neighborhood_stats *stats /* may be NULL */);
 
+/* ---- Splat export: the edited cloud written back out as the vertex rows of a standard 3DGS PLY, on the GPU (the inverse of
+ *      gsr_upload_ply's ingest; no reference counterpart).  "Save" of an editor: the cleaned capture, or one object picked out of it.
+ *      Exported splats: every s of [0, n), n = gsr_stats.num_splats, none of whose plane-0 x, y, z is NaN (a vacant slot is never
+ *        exported: the rule of gsr_select_where) and that is in scope: GSR_EXPORT_KEPT its hidden bit is 0, GSR_EXPORT_SELECTED its
+ *        selected bit is 1.  While the masks are not in use KEPT is every splat and SELECTED none.  One row per exported splat, in
+ *        ascending store index.
+ *      Row: the vertex of a binary little-endian 3DGS PLY of SH degree d, in the trainer's property order
+ *        x y z nx ny nz f_dc_0..2 f_rest_0..(3((d+1)^2 - 1) - 1) opacity scale_0..2 rot_0..3: 17 + 3((d+1)^2 - 1) float32 values (17, 26,
+ *        41 or 62 for d = 0..3).  sh_degree = -1 exports the stored degree (sh_bands - 1); 0 .. the stored degree drops the bands above d.
+ *        The file a host writes is the header
+ *          ply / format binary_little_endian 1.0 / element vertex <rows> / property float <name>, one per column in the order above /
+ *          end_header
+ *        (one line each, '\n'-terminated), then the rows as they are.
+ *      Fields, per exported splat (source units: the stored position, before model_scale):
+ *        x y z      plane-0 x, y, z, bit for bit;  nx ny nz  +0
+ *        f_dc, f_rest  the stored coefficients bit for bit (a GSR_FLAG_SH_HALF half widened, which is exact); f_rest is channel-major as
+ *                   the trainer writes it: with K = (d+1)^2, column c (K - 1) + (k - 1) holds stored value 3k + c
+ *        opacity    the logit of o = plane-2 z in float64, log(o) - log1p(-o), clamped to [-104, 104], NaN replaced by +0, rounded to
+ *                   float32 once (within 1 float32 ulp of that value): o = 0 gives -104, o = 1 gives 104, o < 0, o > 1 or NaN give 0
+ *        scale, rot from S, the symmetric float64 matrix of the six covariance words: when any word is not finite the scales are the quiet
+ *                   NaN and rot = (1, 0, 0, 0).  Else float64 eigenvalues l0 <= l1 <= l2 and orthonormal eigenvectors V (cyclic Jacobi,
+ *                   |S - V diag(l) V^T|max <= 1e-12 max|S|), column 0 of V negated when det V < 0; scale_i = 0.5 log(max(l_i, DBL_MIN));
+ *                   rot = (w, x, y, z), the unit quaternion of V (Shepperd's method), normalised in float64, negated when w < 0.  Each
+ *                   value is rounded to float32 once.
+ *        A row depends only on the splat's stored words and on d: the same splat at another index, in another scope or call gives the
+ *        same bits.
+ *      dst: device memory, page-locked or pageable host memory of dst_rows rows.  Host memory is written through a temporary device
+ *        buffer of rows x row bytes, freed before the call returns; when it cannot be allocated the call returns GSR_ERR_OOM and writes
+ *        nothing (retry into device memory).  dst = NULL counts only.  *rows_out = the number of exported splats, also when dst_rows is
+ *        below it: then the call returns GSR_ERR_INVALID, writes nothing and names the count in gsr_last_error().
+ *      Ordering: enqueued like gsr_splat_histogram (after every upload, selection and edit enqueued before it, before every frame
+ *        enqueued after it); it synchronises the host (it returns the count): a save-time call.  It only reads: it does not put the
+ *        masks in use and is allowed on any context, sharded ones included.  Look-back words for ceil(max_splats / 256) tiles are
+ *        allocated by the first call and kept until gsr_destroy.
+ *      GSR_ERR_INVALID, nothing written: a NULL ctx or rows_out, an unknown scope, sh_degree < -1 or above the stored degree, the
+ *        capacity refusal above. ---- */
+#define GSR_EXPORT_KEPT 0       /* the splats whose hidden bit is 0 */
+#define GSR_EXPORT_SELECTED 1   /* the splats whose selected bit is 1 */
+GSR_API int gsr_export_ply(gsr_ctx *ctx, int32_t scope, int32_t sh_degree, void *dst, uint64_t dst_rows, uint64_t *rows_out);
+
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
  *      num_tile_splats -- persistent across calls exactly like the reference's storage buffer.
