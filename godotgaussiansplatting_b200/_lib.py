@@ -38,6 +38,8 @@ GSR_MAX_NEIGHBOR_CANDIDATES = 1 << 34
 GSR_NEIGHBOR_MIN_RADIUS, GSR_NEIGHBOR_MAX_RADIUS = 2.0 ** -60, 2.0 ** 60
 GSR_NEIGHBOR_SCRATCH_BYTES_PER_SLOT = 32
 GSR_EXPORT_KEPT, GSR_EXPORT_SELECTED = 0, 1
+GSR_COMPRESSED_CHUNK = 256
+GSR_COMPRESS_STORE_ORDER, GSR_COMPRESS_MORTON = 0, 1
 
 # every symbol include/gsr.h declares (tests/test_abi.py checks the header against this list and the .so)
 EXPORTS = [
@@ -49,7 +51,7 @@ EXPORTS = [
     "gsr_get_splat_masks", "gsr_set_splat_masks", "gsr_splat_mask_counts", "gsr_set_selection_style",
     "gsr_transform_selection", "gsr_splat_store_bytes", "gsr_copy_splat_store", "gsr_restore_splat_store", "gsr_recolor_selection",
     "gsr_delete_hidden", "gsr_duplicate_selection", "gsr_set_splat_count", "gsr_select_where", "gsr_splat_histogram",
-    "gsr_select_neighborhood", "gsr_export_ply",
+    "gsr_select_neighborhood", "gsr_export_ply", "gsr_export_compressed_ply", "gsr_upload_compressed_ply",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -92,6 +94,11 @@ class GsrNeighborhood(C.Structure):
 class GsrNeighborhoodStats(C.Structure):
     _fields_ = [("participants", C.c_uint64), ("inside", C.c_uint64), ("candidates", C.c_uint64), ("clusters", C.c_uint64),
                 ("largest_cluster", C.c_uint64)]
+
+
+class GsrCompressedPly(C.Structure):
+    _fields_ = [("chunks", C.c_void_p), ("packed", C.c_void_p), ("sh", C.c_void_p), ("rows", C.c_uint64), ("chunk_count", C.c_uint64),
+                ("sh_degree", C.c_uint32), ("chunk_floats", C.c_uint32)]
 
 
 class GsrSplatFilter(C.Structure):
@@ -196,6 +203,8 @@ def lib():
         L.gsr_splat_histogram.argtypes = [vp, C.POINTER(GsrSplatFilter), C.c_int32, C.c_int32, fp, u32, C.POINTER(u64), fp]
         L.gsr_select_neighborhood.argtypes = [vp, C.POINTER(GsrNeighborhood), C.c_int32, C.POINTER(GsrNeighborhoodStats)]
         L.gsr_export_ply.argtypes = [vp, C.c_int32, C.c_int32, vp, u64, C.POINTER(u64)]
+        L.gsr_export_compressed_ply.argtypes = [vp, C.c_int32, C.c_int32, C.c_int32, C.POINTER(GsrCompressedPly), C.POINTER(u64)]
+        L.gsr_upload_compressed_ply.argtypes = [vp, C.POINTER(GsrCompressedPly), u64, C.c_float]
         L.gsr_splat_store_bytes.argtypes = [vp]
         L.gsr_splat_store_bytes.restype = u64
         L.gsr_copy_splat_store.argtypes = [vp, vp]

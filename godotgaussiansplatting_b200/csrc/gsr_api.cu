@@ -73,6 +73,13 @@ struct gsr_ctx {
     } nb;
     // gsr_export_ply: the exported count, then the look-back words of ceil(max_splats / 256) tiles and the ticket; first call
     unsigned long long *export_words = nullptr;
+    // gsr_export_compressed_ply: a sort workspace of max_splats pairs, the pairs and their ping-pong halves (16 B per slot), and the
+    // bounds pass's result with its page-locked image; allocated by the first call and kept until gsr_destroy
+    struct Compressed {
+        SortWorkspace ws;
+        uint32_t *pairs = nullptr;   // keys | vals | alt keys | alt vals, max_splats each
+        CompressBounds *bounds = nullptr, *bounds_host = nullptr;
+    } cply;
     float4 *records = nullptr;  // 3 float4 per splat id; two tables (consecutive frames alternate: front / back overlap)
     float4 *records2 = nullptr;
     uint32_t *keys = nullptr;    // 3 * capacity: sort input of even frames | of odd frames | ping-pong partner (rasterizer.gd:88 has two halves)
@@ -348,6 +355,37 @@ int alloc_neighbors(gsr_ctx *c, const char *where) {
     return GSR_OK;
 }
 
+void free_compressed(gsr_ctx::Compressed &cp) {
+    sort_workspace_destroy(cp.ws);
+    cudaFree(cp.pairs); cudaFree(cp.bounds);
+    if (cp.bounds_host) cudaFreeHost(cp.bounds_host);
+    cp = gsr_ctx::Compressed();
+}
+
+// gsr_export_compressed_ply's scratch for max_splats slots; on failure nothing is left allocated
+int alloc_compressed(gsr_ctx *c, const char *where) {
+    gsr_ctx::Compressed &cp = c->cply;
+    if (cp.bounds_host) return GSR_OK;
+    const uint64_t m = c->max_splats;
+    int rc = sort_workspace_create(cp.ws, m, /*need_alt_buffers=*/false);
+    cudaError_t e = cudaSuccess;
+    if (!rc) {
+        e = cudaMalloc((void **)&cp.pairs, sizeof(uint32_t) * 4ull * m);
+        if (e == cudaSuccess) e = cudaMalloc((void **)&cp.bounds, sizeof(CompressBounds));
+        if (e == cudaSuccess) e = cudaMallocHost((void **)&cp.bounds_host, sizeof(CompressBounds));
+    }
+    if (rc || e != cudaSuccess) {
+        free_compressed(cp);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            set_last_error("%s: sort scratch for %llu slots -> %s", where, (unsigned long long)m, cudaGetErrorString(e));
+            rc = e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+        }
+        return rc;
+    }
+    return GSR_OK;
+}
+
 void free_ctx(gsr_ctx *c) {
     if (!c) return;
     cudaSetDevice(c->device);
@@ -372,6 +410,7 @@ void free_ctx(gsr_ctx *c) {
     if (c->store_ready) cudaEventDestroy(c->store_ready);
     cudaFree(c->hist);
     cudaFree(c->export_words);
+    free_compressed(c->cply);
     free_neighbors(c->nb);
     if (c->hist_host) cudaFreeHost(c->hist_host);
     if (c->inst.ring) cudaFreeHost(c->inst.ring);
@@ -513,7 +552,7 @@ GSR_API int gsr_create(const gsr_config *cfg, gsr_ctx **out) {
     // happen on the frame path (and would deadlock a group whose ranks share one process: a wait kernel spins meanwhile)
     if ((rc = preload_group_kernels()) || (rc = preload_projection_kernels()) || (rc = preload_sort_kernels()) || (rc = preload_ranges_kernels()) ||
         (rc = preload_ingest_kernels()) || (rc = preload_present_kernels()) || (rc = preload_composite_kernels()) || (rc = preload_selection_kernels()) ||
-        (rc = preload_neighbor_kernels()) || (sh_half(c) && (rc = preload_projection_half_kernels()))) { free_ctx(c); return rc; }
+        (rc = preload_neighbor_kernels()) || (rc = preload_compressed_kernels()) || (sh_half(c) && (rc = preload_projection_half_kernels()))) { free_ctx(c); return rc; }
     cudaError_t e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) { set_last_error("init sync -> %s", cudaGetErrorString(e)); free_ctx(c); return GSR_ERR_CUDA; }
     *out = c;
@@ -2348,6 +2387,159 @@ GSR_API int gsr_export_ply(gsr_ctx *c, int32_t scope, int32_t sh_degree, void *d
     if (!device) cudaFree(out);
     if (rc) return rc;
     GSR_CUDA_TRY(e);
+    return GSR_OK;
+}
+
+// ---- compressed PLY ----------------------------------------------------------------------------------------------------------------
+// The three element bodies of a compressed file of `rows` rows and SH degree d, and where each lives
+struct CplyBuffers {
+    void *ptr[3];
+    uint64_t bytes[3];
+    bool device[3];
+    uint64_t staged;   // bytes of device staging the host-memory buffers need (each part 16-byte aligned)
+};
+static int cply_buffers(CplyBuffers &b, const void *chunks, const void *packed, const void *sh, uint64_t rows, uint32_t chunk_floats,
+                        int degree) {
+    b.ptr[0] = const_cast<void *>(chunks); b.ptr[1] = const_cast<void *>(packed); b.ptr[2] = const_cast<void *>(sh);
+    b.bytes[0] = sizeof(float) * chunk_floats * ((rows + CPLY_CHUNK - 1) / CPLY_CHUNK);
+    b.bytes[1] = sizeof(uint32_t) * 4ull * rows;
+    b.bytes[2] = (uint64_t)cply_sh_bytes(degree) * rows;
+    b.staged = 0;
+    for (int i = 0; i < 3; ++i) {
+        b.device[i] = true;
+        if (!b.bytes[i]) continue;
+        cudaPointerAttributes pa;
+        GSR_CUDA_TRY(cudaPointerGetAttributes(&pa, b.ptr[i]));
+        b.device[i] = pa.type == cudaMemoryTypeDevice || pa.type == cudaMemoryTypeManaged;
+        if (!b.device[i]) b.staged += (b.bytes[i] + 15ull) & ~15ull;
+    }
+    return GSR_OK;
+}
+// Device staging for the host-memory buffers of b: dev[i] is where the kernels read or write part i.  GSR_ERR_OOM when it cannot be
+// allocated (*stage stays nullptr).
+static int cply_stage(CplyBuffers &b, void **stage, void *dev[3], const char *where) {
+    *stage = nullptr;
+    if (b.staged) {
+        cudaError_t e = cudaMalloc(stage, b.staged);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            *stage = nullptr;
+            set_last_error("%s: staging of %llu B for host memory -> %s (use device memory instead)", where, (unsigned long long)b.staged,
+                           cudaGetErrorString(e));
+            return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+        }
+    }
+    uint64_t off = 0;
+    for (int i = 0; i < 3; ++i) {
+        dev[i] = b.ptr[i];
+        if (!b.device[i]) { dev[i] = static_cast<char *>(*stage) + off; off += (b.bytes[i] + 15ull) & ~15ull; }
+    }
+    return GSR_OK;
+}
+
+// Enqueued like gsr_export_ply: synchronises the host for the count, and once more for the file
+GSR_API int gsr_export_compressed_ply(gsr_ctx *c, int32_t scope, int32_t sh_degree, int32_t order, gsr_compressed_ply *dst, uint64_t *rows_out) {
+    static const char *where = "gsr_export_compressed_ply";
+    if (!c || !rows_out) { set_last_error("%s: NULL argument", where); return GSR_ERR_INVALID; }
+    if (scope != GSR_EXPORT_KEPT && scope != GSR_EXPORT_SELECTED) { set_last_error("%s: unknown scope %d", where, scope); return GSR_ERR_INVALID; }
+    if (order != GSR_COMPRESS_STORE_ORDER && order != GSR_COMPRESS_MORTON) { set_last_error("%s: unknown order %d", where, order); return GSR_ERR_INVALID; }
+    if (sh_degree < -1 || sh_degree > c->sh_bands - 1) {
+        set_last_error("%s: sh_degree %d, need -1 .. the stored degree %d", where, sh_degree, c->sh_bands - 1);
+        return GSR_ERR_INVALID;
+    }
+    if (c->max_splats >= (1ull << 32)) { set_last_error("%s: the store index is 32-bit; max_splats %llu", where, (unsigned long long)c->max_splats); return GSR_ERR_INVALID; }
+    const int degree = sh_degree < 0 ? c->sh_bands - 1 : sh_degree;
+    if (dst && (!dst->chunks || !dst->packed || (degree > 0 && !dst->sh))) { set_last_error("%s: NULL buffer in dst", where); return GSR_ERR_INVALID; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    CompressArgs a;
+    memset(&a, 0, sizeof a);
+    a.soa = c->soa; a.plane_stride = c->plane_stride; a.n = c->num_splats;
+    a.hidden = c->masks.on ? c->masks.hidden : nullptr; a.selected = c->masks.on ? c->masks.selected : nullptr;
+    a.selected_only = scope == GSR_EXPORT_SELECTED;
+    a.morton = order == GSR_COMPRESS_MORTON;
+    a.degree = degree;
+    uint64_t rows = 0;
+    cudaStream_t s = nullptr;
+    gsr_ctx::Compressed &cp = c->cply;
+    if (a.n && !(a.selected_only && !a.hidden)) {   // while the masks are not in use nothing is selected
+        if ((rc = alloc_compressed(c, where))) return rc;
+        a.bounds = cp.bounds;
+        if ((rc = store_stream(c, &s)) || (rc = launch_compress_bounds(a, s))) return rc;
+        GSR_CUDA_TRY(cudaMemcpyAsync(cp.bounds_host, cp.bounds, sizeof(CompressBounds), cudaMemcpyDeviceToHost, s));
+        GSR_CUDA_TRY(cudaStreamSynchronize(s));
+        rows = cp.bounds_host->count;
+    }
+    *rows_out = rows;
+    if (!dst) return GSR_OK;
+    if (dst->rows < rows) {
+        set_last_error("%s: %llu exported rows, dst holds %llu", where, (unsigned long long)rows, (unsigned long long)dst->rows);
+        return GSR_ERR_INVALID;
+    }
+    if (rows) {
+        CplyBuffers b;
+        if ((rc = cply_buffers(b, dst->chunks, dst->packed, dst->sh, rows, CPLY_CHUNK_FLOATS, degree))) return rc;
+        void *stage = nullptr, *dev[3];
+        if ((rc = cply_stage(b, &stage, dev, where))) return rc;
+        const uint64_t m = c->max_splats;
+        a.keys = cp.pairs; a.vals = cp.pairs + m; a.sort_n = cp.ws.n_dev; a.rows = rows;
+        a.chunks = static_cast<float *>(dev[0]); a.packed = static_cast<uint32_t *>(dev[1]); a.sh = static_cast<uint8_t *>(dev[2]);
+        rc = launch_compress_keys(a, s);
+        if (!rc) rc = sort_pairs_device(cp.ws, a.keys, a.vals, a.sort_n, cp.pairs + 2 * m, cp.pairs + 3 * m, s, nullptr);
+        if (!rc) rc = launch_compress_chunks(a, c->sh_bands, sh_half(c), s);
+        cudaError_t e = cudaSuccess;
+        for (int i = 0; i < 3 && !rc && e == cudaSuccess; ++i)
+            if (!b.device[i] && b.bytes[i]) e = cudaMemcpyAsync(b.ptr[i], dev[i], b.bytes[i], cudaMemcpyDeviceToHost, s);
+        if (!rc && e == cudaSuccess) e = cudaStreamSynchronize(s);
+        if (stage) cudaFree(stage);
+        if (rc) return rc;
+        GSR_CUDA_TRY(e);
+    }
+    dst->rows = rows;
+    dst->chunk_count = (rows + CPLY_CHUNK - 1) / CPLY_CHUNK;
+    dst->sh_degree = (uint32_t)degree;
+    dst->chunk_floats = CPLY_CHUNK_FLOATS;
+    return GSR_OK;
+}
+
+// Synchronises like gsr_upload_ply: the caller may free or reuse src's buffers when it returns
+GSR_API int gsr_upload_compressed_ply(gsr_ctx *c, const gsr_compressed_ply *src, uint64_t first, float creation_time) {
+    static const char *where = "gsr_upload_compressed_ply";
+    if (!c || !src) { set_last_error("%s: NULL argument", where); return GSR_ERR_INVALID; }
+    if (src->chunk_floats != 12u && src->chunk_floats != 18u) { set_last_error("%s: chunk_floats %u, need 12 or 18", where, src->chunk_floats); return GSR_ERR_INVALID; }
+    if (src->sh_degree > 3u) { set_last_error("%s: sh_degree %u > 3", where, src->sh_degree); return GSR_ERR_INVALID; }
+    if (!src->chunks || !src->packed || (src->sh_degree > 0u && !src->sh)) { set_last_error("%s: NULL buffer in src", where); return GSR_ERR_INVALID; }
+    const uint64_t rows = src->rows;
+    if (src->chunk_count != (rows + CPLY_CHUNK - 1) / CPLY_CHUNK) {
+        set_last_error("%s: %llu chunks for %llu rows, need %llu", where, (unsigned long long)src->chunk_count, (unsigned long long)rows,
+                       (unsigned long long)((rows + CPLY_CHUNK - 1) / CPLY_CHUNK));
+        return GSR_ERR_INVALID;
+    }
+    if (rows > c->max_splats || first > c->max_splats - rows) {
+        set_last_error("%s: upload range [%llu,%llu) exceeds max_splats %llu", where, (unsigned long long)first, (unsigned long long)(first + rows),
+                       (unsigned long long)c->max_splats);
+        return GSR_ERR_INVALID;
+    }
+    int rc = use_device(c->device);
+    if (rc || !rows) return rc;
+    CplyBuffers b;
+    if ((rc = cply_buffers(b, src->chunks, src->packed, src->sh, rows, src->chunk_floats, (int)src->sh_degree))) return rc;
+    void *stage = nullptr, *dev[3];
+    if ((rc = cply_stage(b, &stage, dev, where))) return rc;
+    DecompressArgs a;
+    memset(&a, 0, sizeof a);
+    a.chunks = static_cast<const float *>(dev[0]); a.packed = static_cast<const uint32_t *>(dev[1]); a.sh = static_cast<const uint8_t *>(dev[2]);
+    a.rows = rows; a.chunk_floats = src->chunk_floats; a.degree = (int32_t)src->sh_degree; a.creation_time = creation_time;
+    a.soa = c->soa; a.plane_stride = c->plane_stride; a.first = first;
+    cudaError_t e = cudaStreamSynchronize(c->front_stream);   // a projection in flight reads the planes this call rewrites
+    for (int i = 0; i < 3 && e == cudaSuccess; ++i)
+        if (!b.device[i] && b.bytes[i]) e = cudaMemcpyAsync(dev[i], b.ptr[i], b.bytes[i], cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) rc = launch_compressed_to_soa(a, c->sh_bands, sh_half(c), c->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    if (stage) cudaFree(stage);
+    if (rc) return rc;
+    GSR_CUDA_TRY(e);
+    if (first + rows > c->num_splats) c->num_splats = first + rows;
     return GSR_OK;
 }
 

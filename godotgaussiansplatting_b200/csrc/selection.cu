@@ -497,98 +497,6 @@ __global__ void __launch_bounds__(SEL_THREADS) export_count_kernel(const __grid_
     if (lane == 0u && c) atomicAdd(a.count, (unsigned long long)c);
 }
 
-// One cyclic-Jacobi rotation of the symmetric A in the plane (P, Q), accumulated into the columns of V (Numerical Recipes' jacobi):
-// A[P][Q] becomes exactly 0.  With `late` (after three sweeps) an element that is negligible beside both diagonal entries is zeroed
-// without a rotation.
-template <int P, int Q>
-__device__ __forceinline__ void jacobi_rotate(double (&A)[3][3], double (&V)[3][3], bool late) {
-    constexpr int R = 3 - P - Q;
-    const double apq = A[P][Q];
-    if (apq == 0.0) return;
-    const double g = 100.0 * fabs(apq);
-    if (late && fabs(A[P][P]) + g == fabs(A[P][P]) && fabs(A[Q][Q]) + g == fabs(A[Q][Q])) {
-        A[P][Q] = A[Q][P] = 0.0;
-        return;
-    }
-    const double theta = (A[Q][Q] - A[P][P]) / (2.0 * apq);
-    double t = 1.0 / (fabs(theta) + sqrt(theta * theta + 1.0));   // theta^2 = inf: t = 0, apq is negligible
-    if (theta < 0.0) t = -t;
-    const double c = 1.0 / sqrt(t * t + 1.0), s = t * c, tau = s / (1.0 + c);
-    A[P][P] -= t * apq;
-    A[Q][Q] += t * apq;
-    A[P][Q] = A[Q][P] = 0.0;
-    const double arp = A[R][P], arq = A[R][Q];
-    A[R][P] = A[P][R] = arp - s * (arq + arp * tau);
-    A[R][Q] = A[Q][R] = arq + s * (arp - arq * tau);
-#pragma unroll
-    for (int r = 0; r < 3; ++r) {
-        const double vp = V[r][P], vq = V[r][Q];
-        V[r][P] = vp - s * (vq + vp * tau);
-        V[r][Q] = vq + s * (vp - vq * tau);
-    }
-}
-
-// scale and rot of the covariance words (S00 S01 S02 S11 S12 S22) by the rule of include/gsr.h "Splat export"
-__device__ __forceinline__ void export_scale_rot(const float4 &p1, const float4 &p2, float *out) {
-    const float w6[6] = {p1.x, p1.y, p1.z, p1.w, p2.x, p2.y};
-    bool finite = true;
-#pragma unroll
-    for (int i = 0; i < 6; ++i) finite = finite && fabsf(w6[i]) <= 3.402823466e38f;
-    if (!finite) {
-        const float qnan = __uint_as_float(0x7FC00000u);
-        out[0] = out[1] = out[2] = qnan;
-        out[3] = 1.0f; out[4] = out[5] = out[6] = 0.0f;
-        return;
-    }
-    double A[3][3] = {{w6[0], w6[1], w6[2]}, {w6[1], w6[3], w6[4]}, {w6[2], w6[4], w6[5]}};
-    double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
-#pragma unroll 1
-    for (int sweep = 0; sweep < 16; ++sweep) {
-        if (A[0][1] == 0.0 && A[0][2] == 0.0 && A[1][2] == 0.0) break;
-        jacobi_rotate<0, 1>(A, V, sweep >= 3);
-        jacobi_rotate<0, 2>(A, V, sweep >= 3);
-        jacobi_rotate<1, 2>(A, V, sweep >= 3);
-    }
-    double l[3] = {A[0][0], A[1][1], A[2][2]};
-    // ascending eigenvalues with their columns: compare-exchange (0, 1), (1, 2), (0, 1)
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const int i = k == 1 ? 1 : 0, j = i + 1;
-        if (l[j] < l[i]) {
-            const double t = l[i]; l[i] = l[j]; l[j] = t;
-#pragma unroll
-            for (int r = 0; r < 3; ++r) { const double v = V[r][i]; V[r][i] = V[r][j]; V[r][j] = v; }
-        }
-    }
-    const double det = V[0][0] * (V[1][1] * V[2][2] - V[1][2] * V[2][1]) - V[0][1] * (V[1][0] * V[2][2] - V[1][2] * V[2][0]) +
-                       V[0][2] * (V[1][0] * V[2][1] - V[1][1] * V[2][0]);
-    if (det < 0.0) { V[0][0] = -V[0][0]; V[1][0] = -V[1][0]; V[2][0] = -V[2][0]; }
-#pragma unroll
-    for (int i = 0; i < 3; ++i) out[i] = (float)(0.5 * log(l[i] > 2.2250738585072014e-308 ? l[i] : 2.2250738585072014e-308));
-    // Shepperd: the largest of 4w^2 - 1 = tr, and 4x^2 - 1, 4y^2 - 1, 4z^2 - 1 (the diagonal entries), first on a tie
-    const double tr = (V[0][0] + V[1][1]) + V[2][2];
-    int k = 0;
-    double best = tr;
-#pragma unroll
-    for (int i = 0; i < 3; ++i) if (V[i][i] > best) { best = V[i][i]; k = i + 1; }
-    double q[4];
-    if (k == 0) {
-        const double w = 0.5 * sqrt(1.0 + tr), f = 0.25 / w;
-        q[0] = w; q[1] = (V[2][1] - V[1][2]) * f; q[2] = (V[0][2] - V[2][0]) * f; q[3] = (V[1][0] - V[0][1]) * f;
-    }
-#pragma unroll
-    for (int kk = 1; kk <= 3; ++kk) {   // unrolled, so that every index is a constant and V and q stay in registers
-        if (k != kk) continue;
-        const int a = kk - 1, b = kk % 3, c = (kk + 1) % 3;
-        const double v = 0.5 * sqrt(((1.0 + V[a][a]) - V[b][b]) - V[c][c]), f = 0.25 / v;
-        q[0] = (V[c][b] - V[b][c]) * f;
-        q[1 + a] = v; q[1 + b] = (V[b][a] + V[a][b]) * f; q[1 + c] = (V[c][a] + V[a][c]) * f;
-    }
-    const double norm = sqrt(((q[0] * q[0] + q[1] * q[1]) + q[2] * q[2]) + q[3] * q[3]), sg = q[0] < 0.0 ? -1.0 : 1.0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) out[3 + i] = (float)(sg * (q[i] / norm));
-}
-
 // The writing pass.  A CTA owns COMPACT_TILE_WORDS consecutive mask words (one splat per thread, its tile from an atomic ticket like
 // compact_store_kernel), ranks its exported splats, publishes its count and looks back for its prefix excl (the pass only reads the
 // store, so it publishes its PREFIX right after).  Each exported splat reads planes 1, 2 and the SH planes of degree d and writes its

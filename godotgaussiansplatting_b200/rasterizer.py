@@ -19,6 +19,7 @@ import numpy as np
 
 from . import _lib
 from .camera import Camera3D, pack_camera_push_constants, transform_to_projection
+from .compressed_ply import CompressedPlyFile
 from .ply_file import PlyFile, PlyLayout, load_gaussian_splats
 
 TILE_SIZE = 16            # rasterizer.gd:4
@@ -67,11 +68,16 @@ class GaussianSplattingRasterizer:
         self.loaded_callbacks = []  # signal `loaded`
         self._ctx = C.c_void_p(None)
         self._device, self._flags, self._factor = device, flags | (_lib.GSR_FLAG_SH_HALF if sh_half else 0), dup_capacity_factor
-        try:
-            self._layout = point_cloud.layout()
-        except ValueError:
-            self._layout = None   # not a named 3DGS layout: the standard 62-property order, as the reference reads it
-        self._sh_bands = int(sh_bands) if sh_bands is not None else (self._layout.sh_degree + 1 if self._layout else 0)
+        self._compressed = isinstance(point_cloud, CompressedPlyFile)   # loaded through the device decode (upload_compressed_ply)
+        if self._compressed:
+            self._layout = None
+        else:
+            try:
+                self._layout = point_cloud.layout()
+            except ValueError:
+                self._layout = None   # not a named 3DGS layout: the standard 62-property order, as the reference reads it
+        default_bands = point_cloud.sh_degree + 1 if self._compressed else (self._layout.sh_degree + 1 if self._layout else 0)
+        self._sh_bands = int(sh_bands) if sh_bands is not None else default_bands
         has_filter_3d = self._layout is not None and self._layout.filter_3d >= 0
         self._antialiasing = float(antialiasing) if antialiasing is not None else (0.1 if has_filter_3d else 0.0)
         self._depth_order = int(depth_order)
@@ -135,6 +141,10 @@ class GaussianSplattingRasterizer:
         self.should_terminate_thread[0] = False
         self.num_splats_loaded[0] = 0
         if not load:
+            return
+        if self._compressed:   # a compressed PLY is decoded on the device in one call
+            self.upload_compressed_ply(self.point_cloud, 0, self.ticks())
+            self._emit_loaded()
             return
         # the reference starts a loader thread (:114); here the load runs inline, chunk by chunk
         stride = max(1, self.point_cloud.size // 1000)
@@ -488,6 +498,38 @@ class GaussianSplattingRasterizer:
             _lib.check(L.gsr_export_ply(self._ctx, int(scope), int(sh_degree), C.c_void_p(table.ctypes.data), table.shape[0], C.byref(rows)),
                        "gsr_export_ply")
         return PlyFile.from_array(table, names)
+
+    def export_compressed_ply(self, scope: int = _lib.GSR_EXPORT_KEPT, sh_degree: int = -1,
+                              order: int = _lib.GSR_COMPRESS_MORTON) -> CompressedPlyFile:
+        """The edited cloud exported on the GPU as a SuperSplat compressed PLY (include/gsr.h "Compressed PLY"): the splats of export_ply's
+        scope with a finite position, in Morton order (GSR_COMPRESS_MORTON, the smaller chunk ranges) or store order
+        (GSR_COMPRESS_STORE_ORDER, the rows of export_ply), SH degree sh_degree (-1: the stored degree).  r.export_compressed_ply().save(path)
+        writes the file.  Synchronises twice (the count, then the file)."""
+        L, rows = _lib.lib(), C.c_uint64(0)
+        _lib.check(L.gsr_export_compressed_ply(self._ctx, int(scope), int(sh_degree), int(order), None, C.byref(rows)), "gsr_export_compressed_ply")
+        degree = (self._sh_bands if self._sh_bands else 4) - 1 if int(sh_degree) < 0 else int(sh_degree)
+        n = rows.value
+        chunks = np.empty(((n + _lib.GSR_COMPRESSED_CHUNK - 1) // _lib.GSR_COMPRESSED_CHUNK, 18), dtype=np.float32)
+        packed = np.empty((n, 4), dtype=np.uint32)
+        sh = np.empty((n, 3 * ((degree + 1) ** 2 - 1)), dtype=np.uint8) if degree > 0 else None
+        if n:
+            dst = _lib.GsrCompressedPly(chunks.ctypes.data, packed.ctypes.data, sh.ctypes.data if sh is not None else None, n, chunks.shape[0],
+                                        degree, 18)
+            _lib.check(L.gsr_export_compressed_ply(self._ctx, int(scope), int(sh_degree), int(order), C.byref(dst), C.byref(rows)),
+                       "gsr_export_compressed_ply")
+        return CompressedPlyFile.from_arrays(chunks, packed, sh, degree)
+
+    def upload_compressed_ply(self, cply: CompressedPlyFile, first: int = 0, creation_time: float = 0.0) -> None:
+        """Device decode of a compressed PLY into splats [first, first + cply.size) (include/gsr.h gsr_upload_compressed_ply)."""
+        if not self._ctx:
+            raise RuntimeError("init_gpu() first")
+        chunks = np.ascontiguousarray(cply.chunks, dtype=np.float32)
+        packed = np.ascontiguousarray(cply.packed, dtype=np.uint32)
+        sh = np.ascontiguousarray(cply.sh, dtype=np.uint8) if cply.sh_degree > 0 else None
+        src = _lib.GsrCompressedPly(chunks.ctypes.data, packed.ctypes.data, sh.ctypes.data if sh is not None else None, cply.size,
+                                    chunks.shape[0], cply.sh_degree, chunks.shape[1])
+        _lib.check(_lib.lib().gsr_upload_compressed_ply(self._ctx, C.byref(src), int(first), float(creation_time)), "gsr_upload_compressed_ply")
+        self.num_splats_loaded[0] = max(self.num_splats_loaded[0], int(first) + cply.size)
 
     def _plane_stride(self) -> int:
         return (self._max_splats + 255) // 256 * 256

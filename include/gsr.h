@@ -851,6 +851,82 @@ GSR_API int gsr_select_neighborhood(gsr_ctx *ctx, const gsr_neighborhood *q, int
 #define GSR_EXPORT_SELECTED 1   /* the splats whose selected bit is 1 */
 GSR_API int gsr_export_ply(gsr_ctx *ctx, int32_t scope, int32_t sh_degree, void *dst, uint64_t dst_rows, uint64_t *rows_out);
 
+/* ---- Compressed PLY: the SuperSplat / PlayCanvas `compressed.ply` layout, written and read on the GPU.  About 61 B per degree-3 splat
+ *      (16 B at degree 0) instead of the 248 B of a float 3DGS PLY.  The library fills or reads the three element bodies; the host writes
+ *      or parses the header:
+ *        ply / format binary_little_endian 1.0 /
+ *        element chunk <ceil(rows / 256)> / property float <name>, one line each for min_x min_y min_z max_x max_y max_z min_scale_x
+ *          min_scale_y min_scale_z max_scale_x max_scale_y max_scale_z min_r min_g min_b max_r max_g max_b /
+ *        element vertex <rows> / property uint packed_position / property uint packed_rotation / property uint packed_scale /
+ *          property uint packed_color /
+ *        element sh <rows> / property uchar f_rest_0 .. f_rest_<3((d+1)^2 - 1) - 1>   (only for d > 0) /
+ *        end_header
+ *      ('\n'-terminated lines; `comment` lines may appear anywhere in the header), then the chunk floats, the packed words and the SH
+ *      bytes as they are.  Row r belongs to chunk r / 256; the last chunk may be partial.  Older files have 12-float chunks (no colour
+ *      range); they are accepted on upload.  The layout and the quantisation follow the public description of SuperSplat's format; no
+ *      file written by another tool has been checked against this library, and other decoders may reconstruct bin edges slightly
+ *      differently.  Bit-exactness is a property of this library's own rule below.
+ *
+ *      Export rule.  Every value in float64 from float32 inputs, one rounding per operation (the library is built with -fmad=false).
+ *        Exported splats: those of gsr_export_ply's rule (scope, vacant slots skipped) whose plane-0 x, y, z are also finite (an infinite
+ *          position cannot be quantised and is not exported).
+ *        Per row: position = plane-0 x, y, z; log-scales s0..s2 and quaternion (w x y z) = the scale and rot gsr_export_ply writes for
+ *          the splat, bit for bit; colour c_k = (float)(f_dc_k * 0.28209479177387814 + 0.5); alpha o = plane-2 z (the stored sigmoid);
+ *          SH = the stored coefficients 1 .. (d+1)^2 - 1, channel-major as in a degree-d 3DGS PLY.
+ *        Sanitised before the chunk statistics: log-scales clamped to [-20, 20], NaN -> -20; colours clamped to [-64, 64], NaN -> 0.5;
+ *          alpha clamped to [0, 1], NaN -> 0.
+ *        Chunk: the exact float32 minimum and maximum over the chunk's rows of x, y, z, s0..s2 and c0..c2 (18 floats, ordered as in the
+ *          header; -0 orders below +0).
+ *        norm(x, lo, hi) = 0 if x <= lo, 1 if x >= hi, 0 if hi - lo < 1e-5, else (x - lo) / (hi - lo).
+ *        unorm(v, b) = min(t, max(0, floor(v t + 0.5))), t = 2^b - 1.
+ *        packed_position, packed_scale = unorm(nx, 11) << 21 | unorm(ny, 10) << 11 | unorm(nz, 11) (n = norm over the chunk's range).
+ *        packed_color = unorm(nr, 8) << 24 | unorm(ng, 8) << 16 | unorm(nb, 8) << 8 | unorm(o, 8).
+ *        packed_rotation: i = the index of the largest |q_k| (the first on a tie); q negated when q_i < 0; the other three components in
+ *          ascending index, each unorm(q_k sqrt(0.5) + 0.5, 10); i << 30 | a << 20 | b << 10 | c.
+ *        SH byte = min(255, max(0, trunc((v / 8 + 0.5) 256))), NaN -> 128.
+ *        Row order: GSR_COMPRESS_STORE_ORDER ascending store index (the rows and order of gsr_export_ply).  GSR_COMPRESS_MORTON: lo, hi =
+ *          the float32 bounds of the exported positions; per axis cell = min(1023, floor((p - lo) / (hi - lo) 1024)), 0 when hi == lo;
+ *          key = part1by2(z) << 2 | part1by2(y) << 1 | part1by2(x) (30 bits); ascending key, ties in ascending store index.
+ *      Decode rule (upload).  float32, one IEEE operation at a time.  u(v, b) = v / (2^b - 1); lerp(lo, hi, u) = lo + (hi - lo) u.
+ *        Position and log-scale: lerp over the chunk's range.  Colour: lerp over the chunk's range (a 12-float chunk: u(v, 8) itself),
+ *          f_dc = (c - 0.5f) / 0.28209479177387814f.  Quaternion: a, b, c = (u(field, 10) - 0.5f) 1.41421356f,
+ *          m = sqrt(max(0, 1 - ((a a + b b) + c c))) at index i, a, b, c at the other indices in ascending order.  SH: (q + 0.5f) 0.03125f
+ *          - 4.0f (the bin's midpoint).
+ *        The store then holds what gsr_upload_ply stores for the decoded float rows (x y z f_dc f_rest opacity scale rot), except plane-2
+ *          z = u(alpha, 8) itself (no logit and sigmoid).  Coefficients above the file's degree are stored as 0, those above the store's
+ *          bands are dropped.
+ *
+ *      gsr_export_compressed_ply(ctx, scope, sh_degree, order, dst, rows_out): scope GSR_EXPORT_KEPT / _SELECTED, sh_degree -1 (the
+ *        stored degree) or 0 .. the stored degree, order GSR_COMPRESS_*.  dst->rows is the capacity in rows: dst->chunks holds
+ *        ceil(dst->rows / 256) x 18 floats, dst->packed dst->rows x 4 words, dst->sh dst->rows x 3((d+1)^2 - 1) bytes (unused for d = 0).
+ *        The three may be device, page-locked or pageable memory (host memory goes through temporary device staging, freed before the
+ *        call returns).  dst = NULL counts only.  *rows_out = the exported count, also when it exceeds dst->rows: then GSR_ERR_INVALID and
+ *        nothing is written.  On success dst->rows, dst->chunk_count, dst->sh_degree and dst->chunk_floats (18) describe the file written,
+ *        so dst can be passed to gsr_upload_compressed_ply as it is.  Ordered like gsr_export_ply; it only reads the store, does not put
+ *        the masks in use and is allowed on sharded contexts.  Scratch of 16 B per slot plus a sort workspace is allocated by the first
+ *        call and kept until gsr_destroy (GSR_ERR_OOM, nothing kept, when it cannot be).  GSR_ERR_INVALID: a NULL ctx or rows_out, an
+ *        unknown scope or order, a bad sh_degree, a NULL buffer in dst (sh only with d > 0), the capacity refusal, max_splats >= 2^32.
+ *      gsr_upload_compressed_ply(ctx, src, first, creation_time): rows [0, src->rows) become splats [first, first + rows).  src's buffers
+ *        may be device or host memory.  A chunk-aligned piece of a file (rows from a multiple of 256, its chunks from that chunk on) is a
+ *        file itself, so a load may be split into pieces.  Synchronises like gsr_upload_ply.  GSR_ERR_INVALID, nothing written: NULL ctx,
+ *        src or buffer (sh == NULL with d > 0), chunk_floats not 12 or 18, sh_degree > 3, chunk_count != ceil(rows / 256),
+ *        [first, first + rows) beyond max_splats. ---- */
+#define GSR_COMPRESSED_CHUNK 256
+#define GSR_COMPRESS_STORE_ORDER 0   /* ascending store index: the rows of gsr_export_ply */
+#define GSR_COMPRESS_MORTON 1        /* 30-bit Morton order over the exported bounds (SuperSplat's; the smaller chunk ranges) */
+typedef struct gsr_compressed_ply {
+    float *chunks;          /* chunk_count x chunk_floats */
+    uint32_t *packed;       /* rows x 4: position, rotation, scale, color */
+    uint8_t *sh;            /* rows x 3((d+1)^2 - 1); may be NULL iff sh_degree 0 */
+    uint64_t rows;
+    uint64_t chunk_count;   /* ceil(rows / 256) */
+    uint32_t sh_degree;     /* 0..3 */
+    uint32_t chunk_floats;  /* 18; 12 accepted on upload */
+} gsr_compressed_ply;       /* 48 bytes */
+GSR_API int gsr_export_compressed_ply(gsr_ctx *ctx, int32_t scope, int32_t sh_degree, int32_t order, gsr_compressed_ply *dst /* NULL: count */,
+                                      uint64_t *rows_out);
+GSR_API int gsr_upload_compressed_ply(gsr_ctx *ctx, const gsr_compressed_ply *src, uint64_t first, float creation_time);
+
 /* ---- get_splat_position() (rasterizer.gd:162-171): re-dispatches the compositor for `tile_id` and reads the
  *      16-byte tile_splat_pos buffer (gsplat_render.glsl:33-36,105-110).  out_xyzn = splat_pos.xyz,
  *      num_tile_splats -- persistent across calls exactly like the reference's storage buffer.
