@@ -30,6 +30,7 @@ GSR_NO_ID = 0xFFFFFFFF              # gsr_set_splat_ids: no splat / no instance
 GSR_MAX_SELECT_VERTICES = 64
 GSR_SELECT_SET, GSR_SELECT_ADD, GSR_SELECT_SUBTRACT, GSR_SELECT_TOGGLE = range(4)
 GSR_PROP_OPACITY, GSR_PROP_SIZE, GSR_PROP_VOLUME, GSR_PROP_ISOTROPY, GSR_PROP_COLOR_DISTANCE = range(5)
+GSR_PROP_CONTRIBUTION, GSR_PROP_PEAK_CONTRIBUTION, GSR_PROP_VIEWS, GSR_PROP_CONTRIBUTING_PIXELS = range(16, 20)   # gsr_set_splat_contribution
 GSR_MAX_SPLAT_FILTERS = 8
 GSR_MAX_HISTOGRAM_BINS = 1024
 GSR_HISTOGRAM_KEPT, GSR_HISTOGRAM_SELECTED = 0, 1
@@ -51,7 +52,7 @@ EXPORTS = [
     "gsr_get_splat_masks", "gsr_set_splat_masks", "gsr_splat_mask_counts", "gsr_set_selection_style",
     "gsr_transform_selection", "gsr_splat_store_bytes", "gsr_copy_splat_store", "gsr_restore_splat_store", "gsr_recolor_selection",
     "gsr_delete_hidden", "gsr_duplicate_selection", "gsr_set_splat_count", "gsr_select_where", "gsr_splat_histogram",
-    "gsr_select_neighborhood", "gsr_export_ply", "gsr_export_compressed_ply", "gsr_upload_compressed_ply",
+    "gsr_select_neighborhood", "gsr_set_splat_contribution", "gsr_reset_splat_contribution", "gsr_splat_contribution_frames", "gsr_export_ply", "gsr_export_compressed_ply", "gsr_upload_compressed_ply",
     "gsr_get_stats", "gsr_get_frame_history", "gsr_debug_copy", "gsr_debug_enable_trace", "gsr_debug_compositor_config", "gsr_debug_pipeline", "gsr_debug_keep_unsorted", "gsr_sorter_create", "gsr_sorter_destroy",
     "gsr_sorter_sort_device", "gsr_sort_pairs_host", "gsr_sorter_last_ms", "gsr_error_string", "gsr_last_error",
     "gsr_device_count", "gsr_version",
@@ -103,6 +104,11 @@ class GsrCompressedPly(C.Structure):
 
 class GsrSplatFilter(C.Structure):
     _fields_ = [("property", C.c_int32), ("lo", C.c_float), ("hi", C.c_float), ("rgb", C.c_float * 3)]
+
+
+class GsrSplatContribution(C.Structure):
+    _fields_ = [("weight", C.c_uint64), ("pixels", C.c_uint64), ("peak", C.c_float), ("views", C.c_uint32), ("last_frame", C.c_uint32),
+                ("pad", C.c_uint32)]
 
 
 class GsrCutout(C.Structure):
@@ -175,6 +181,9 @@ def lib():
         L.gsr_set_motion_vectors.argtypes = [vp, vp]
         L.gsr_reset_motion.argtypes = [vp]
         L.gsr_set_splat_ids.argtypes = [vp, vp]
+        L.gsr_set_splat_contribution.argtypes = [vp, vp, C.c_uint64]
+        L.gsr_reset_splat_contribution.argtypes = [vp]
+        L.gsr_splat_contribution_frames.argtypes = [vp, C.POINTER(C.c_uint32)]
         L.gsr_set_instances.argtypes = [vp, C.POINTER(GsrInstance), u32]
         L.gsr_set_instance_appearance.argtypes = [vp, C.POINTER(GsrInstanceAppearance), u32]
         L.gsr_set_sh_degree.argtypes = [vp, C.c_int32]

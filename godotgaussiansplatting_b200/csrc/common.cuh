@@ -555,10 +555,14 @@ int launch_compressed_to_soa(const DecompressArgs &a, int bands, bool sh_half, c
 // ---- splat property selection (gsr_select_where, gsr_splat_histogram; selection.cu) ----
 // The planes a property reads beyond plane 0 (a size, volume or isotropy reads planes 1 and 2).  The kernels are templated on the union
 // of a filter set's bits, so each reads only the planes its set needs.
-enum PropPlanes : int { PROP_P1 = 1, PROP_P2 = 2, PROP_P3 = 4 };
+enum PropPlanes : int { PROP_P1 = 1, PROP_P2 = 2, PROP_P3 = 4, PROP_PC = 16 };   // (8: the binary16 bit of the variant tables)
 __host__ __device__ constexpr int prop_planes(int32_t p) {
     return p == GSR_PROP_OPACITY ? PROP_P2 : p == GSR_PROP_COLOR_DISTANCE ? PROP_P3 : PROP_P1 | PROP_P2;
 }
+// The contribution properties (GSR_PROP_CONTRIBUTION ..) read the contribution buffer (PROP_PC) and no plane; the kernels that can
+// meet them test for them before prop_planes.
+__host__ __device__ constexpr bool prop_is_contrib(int32_t p) { return p >= GSR_PROP_CONTRIBUTION && p <= GSR_PROP_CONTRIBUTING_PIXELS; }
+__host__ __device__ constexpr int prop_sources(int32_t p) { return prop_is_contrib(p) ? PROP_PC : prop_planes(p); }
 // inside(s) for the splats s of [first, first + count) (the caller bounds it by the cloud's n), combined into the selected mask by `op`
 // over every word, then selected &= ~hidden.
 struct WhereArgs {
@@ -570,8 +574,9 @@ struct WhereArgs {
     uint64_t plane_stride;
     uint32_t n;                                   // filters
     gsr_splat_filter f[GSR_MAX_SPLAT_FILTERS];
+    const gsr_splat_contribution *contrib;        // PROP_PC only: the contribution buffer (gsr_set_splat_contribution)
 };
-// planes: the union of prop_planes over the set; sh_half: the store's SH format (read only when the set reads plane 3)
+// planes: the union of prop_sources over the set; sh_half: the store's SH format (read only when the set reads plane 3)
 int launch_select_where(const WhereArgs &a, int planes, bool sh_half, cudaStream_t stream);
 // The histogram's device buffer: the counters, then the min / max keys, then the edges.  The keys are kept as ints so that one
 // atomicMax serves both: keys[0] = max of hist_signed_key(~ord(v)) (the least ord(v)), keys[1] = max of hist_signed_key(ord(v)) (the
@@ -591,6 +596,7 @@ struct HistArgs {
     unsigned long long *counts;                   // bins + 3, zeroed
     int32_t *keys;                                // INT32_MIN, INT32_MIN on entry: the least and greatest ord(v), as above
     const float *edges;                           // bins + 1
+    const gsr_splat_contribution *contrib;        // PROP_PC only: the contribution buffer (gsr_set_splat_contribution)
 };
 int launch_splat_histogram(const HistArgs &a, int planes, bool sh_half, int sm_count, cudaStream_t stream);
 
@@ -785,7 +791,18 @@ struct SplatIdArgs {
     uint32_t *ids_out;          // W*H uint2 (v, k); (NO_ID, NO_ID) where no splat has t - t' > 0
     const uint32_t *warp_inst;  // instance of every drawn warp; nullptr: no instances, k = NO_ID
 };
-int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion = nullptr, const SplatIdArgs *ids = nullptr);
+// Splat contribution (gsr_set_splat_contribution, with depth compositing only, without motion vectors and IDs): the second
+// __grid_constant__ parameter of composite_contrib_kernel.  Every (in-image pixel, blended splat) with w = t - t' > 0 adds
+// q(w) = __float2uint_rn(w * 2^24), 1, max(peak, w) to the record of the splat's source slot, and the frame once to its views.
+struct ContribArgs {
+    gsr_splat_contribution *accum;   // max_splats records, indexed by source slot
+    const uint32_t *warp_inst;       // instance of every drawn warp; nullptr: no instances, the slot is the drawn id
+    const InstanceDesc *desc;        // slot = desc[k].first + (v - 32 desc[k].warp0) for k = warp_inst[v >> 5]
+    uint32_t *frames;                // +1 per frame that did not overflow the duplicate capacity
+    uint32_t epoch;                  // the frame's: non-zero, the same for gsr_render's re-render of an overflowed frame
+};
+int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion = nullptr, const SplatIdArgs *ids = nullptr,
+                     const ContribArgs *contrib = nullptr);
 int composite_max_ctas_per_sm(int *out);
 // order[0 .. num_tiles) = owned-tile indices sorted by descending expected chain length: the chunk count the tile consumed in the
 // previous frame (hint[k] with bit 31 set; the bit is cleared here) or, without a hint, its list length in chunks capped at

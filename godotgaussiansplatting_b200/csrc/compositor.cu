@@ -38,6 +38,11 @@
 // (t' = t * (1 - alpha), the value the blend stores), replaced only by a strictly larger w.  The compare and selects sit beside the
 // transmittance chain, not on it.  The output is (v, warp_inst[v >> 5]) per pixel, (NO_ID, NO_ID) where no w was > 0.  Its pointers
 // travel in the second parameter too.
+// Splat contribution (composite_contrib_kernel, CONTRIB = true, gsr_set_splat_contribution; with DEPTH, without MOTION and IDS): the
+// drawn id is staged as for IDS, and per staged splat every warp reduces the w = t - t' > 0 of its in-image pixels -- the sum of
+// q(w) = rn(w * 2^24), the hit count and the largest w -- into its own slice of shared memory (a warp-uniform skip when no lane has
+// a hit).  At the end of each chunk a thread sums the four warps' slices of its two staged splats in 64 bits and adds them to the
+// splat's source-slot record with one global atomic each, plus an exchange of the frame's epoch that counts the frame once per slot.
 #include <stdlib.h>
 #include <string.h>
 
@@ -103,9 +108,17 @@ template <> struct PendingT<false, true> { using type = IdPending; };
 template <bool MOTION, bool IDS = false> using Pending = typename PendingT<MOTION, IDS>::type;
 // IDS: the second parameter is the motion one (or the placeholder) extended by the ID pointers, so the motion code reads it unchanged
 template <bool MOTION> struct WithIds : MotionParam<MOTION> { SplatIdArgs ids; };
-template <bool MOTION, bool IDS> struct SecondParamT { using type = MotionParam<MOTION>; };
-template <bool MOTION> struct SecondParamT<MOTION, true> { using type = WithIds<MOTION>; };
-template <bool MOTION, bool IDS> using SecondParam = typename SecondParamT<MOTION, IDS>::type;
+template <bool MOTION, bool IDS, bool CONTRIB> struct SecondParamT { using type = MotionParam<MOTION>; };
+template <bool MOTION> struct SecondParamT<MOTION, true, false> { using type = WithIds<MOTION>; };
+// CONTRIB (depth compositing alone): the contribution constants
+template <> struct SecondParamT<false, false, true> { using type = ContribArgs; };
+template <bool MOTION, bool IDS, bool CONTRIB = false> using SecondParam = typename SecondParamT<MOTION, IDS, CONTRIB>::type;
+
+// gather's motion constants: the second parameter of a MOTION variant, nothing for the others
+template <bool MOTION, class SP> __device__ __forceinline__ const MotionParam<MOTION> *motion_param(const SP &mo) {
+    if constexpr (MOTION) return &mo;
+    else return nullptr;
+}
 
 // vz = (V[2], V[6], V[10], V[14]): the view-matrix row of the depth (DEPTH only)
 template <bool DEPTH, bool MOTION = false, bool IDS = false>
@@ -269,11 +282,15 @@ struct IdState {   // IDS: the two pixels' largest w and its drawn id
 template <bool IDS> struct IdStateT { using type = NoMotion; };
 template <> struct IdStateT<true> { using type = IdState; };
 template <bool IDS> using IdStateOf = typename IdStateT<IDS>::type;
-template <bool CONTRACT, bool DEPTH, bool MOTION = false, bool IDS = false>
+//      CONTRIB: the warp's reductions of the pixels' w > 0 (in-image pixels only: in0 / in1) for staged splat j + u go to its slice
+//      cw: cw[j + u] = the sum of q(w), cw[CW_HITS + j + u] = the hit count, cw[CW_PEAK + j + u] = the bits of the largest w.  Only a
+//      splat with a hit is written: the hit count of the others stays the 0 of the staging.
+constexpr int CW_HITS = (THREADS / 32) * CHUNK, CW_PEAK = 2 * CW_HITS;
+template <bool CONTRACT, bool DEPTH, bool MOTION = false, bool IDS = false, bool CONTRIB = false>
 __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, const float *s_d, int j, const F2 al2[GU], const F2 om2[GU], F2 &cr2,
                                         F2 &cg2, F2 &cb2, float &t0, float &t1, bool &alive_mid, float z0, float z1, bool &o0, bool &o1, F2 &dd2,
                                         const float2 *s_m = nullptr, F2 *mx2 = nullptr, F2 *my2 = nullptr, const uint32_t *s_v = nullptr,
-                                        IdStateOf<IDS> *ids = nullptr) {
+                                        IdStateOf<IDS> *ids = nullptr, uint32_t *cw = nullptr, bool in0 = false, bool in1 = false) {
 #pragma unroll
     for (int u = 0; u < GU; ++u) {
         const float cbl = s_c[j + u];
@@ -323,6 +340,18 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, co
             ids->best0 = b0 ? w0 : ids->best0; ids->id0 = b0 ? vj : ids->id0;
             ids->best1 = b1 ? w1 : ids->best1; ids->id1 = b1 ? vj : ids->id1;
         }
+        if constexpr (CONTRIB) {
+            const float w0 = __fsub_rn(t0, pl), w1 = __fsub_rn(t1, ph);
+            const bool h0 = a0 && in0 && w0 > 0.0f, h1 = a1 && in1 && w1 > 0.0f;
+            if (__any_sync(0xffffffffu, h0 || h1)) {   // warp-uniform
+                const uint32_t q = (h0 ? __float2uint_rn(w0 * 16777216.0f) : 0u) + (h1 ? __float2uint_rn(w1 * 16777216.0f) : 0u);
+                const uint32_t qs = __reduce_add_sync(0xffffffffu, q);   // <= 64 * 2^24
+                const uint32_t hits = (uint32_t)(__popc(__ballot_sync(0xffffffffu, h0)) + __popc(__ballot_sync(0xffffffffu, h1)));
+                const uint32_t b0 = h0 ? __float_as_uint(w0) : 0u, b1 = h1 ? __float_as_uint(w1) : 0u;   // w > 0: the bits order as the floats
+                const int pk = __reduce_max_sync(0xffffffffu, (int)(b0 > b1 ? b0 : b1));
+                if ((threadIdx.x & 31u) == 0u) { cw[j + u] = qs; cw[CW_HITS + j + u] = hits; cw[CW_PEAK + j + u] = (uint32_t)pk; }
+            }
+        }
         t0 = a0 ? pl : t0;
         t1 = a1 ? ph : t1;
     }
@@ -338,20 +367,29 @@ __device__ __forceinline__ void phase_b(const float4 B[GU], const float *s_c, co
 // code as when this body was its own).
 // MOTION (gsr_set_motion_vectors, with DEPTH only): the motion constants in `mo`; the other variants take an empty placeholder.
 // IDS (gsr_set_splat_ids, with DEPTH only): `mo` also carries the ID pointers (mo.ids).
-template <bool CONTRACT, bool DEPTH, bool MOTION, bool IDS>
-__device__ __forceinline__ void composite_tiles(const CompositeArgs p, const SecondParam<MOTION, IDS> &mo) {
+// CONTRIB (gsr_set_splat_contribution, with DEPTH only, without MOTION and IDS): `mo` is the ContribArgs.
+template <bool CONTRACT, bool DEPTH, bool MOTION, bool IDS, bool CONTRIB = false>
+__device__ __forceinline__ void composite_tiles(const CompositeArgs p, const SecondParam<MOTION, IDS, CONTRIB> &mo) {
     static_assert(!MOTION || DEPTH, "motion vectors are a companion of depth compositing");
     static_assert(!IDS || DEPTH, "splat IDs are a companion of depth compositing");
+    static_assert(!CONTRIB || (DEPTH && !MOTION && !IDS), "splat contribution is a companion of depth compositing alone");
+    constexpr bool VID = IDS || CONTRIB;   // the drawn id of the staged splats is needed
     __shared__ float4 s_a[CHUNK];
     __shared__ float4 s_b[CHUNK];
     __shared__ float s_c[CHUNK];
     __shared__ float s_d[DEPTH ? CHUNK : 1];   // view depth of the staged splats
     __shared__ float2 s_m[MOTION ? CHUNK : 1]; // MOTION: screen motion of the staged splats
-    __shared__ uint32_t s_v[IDS ? CHUNK : 1];  // IDS: drawn id of the staged splats
+    __shared__ uint32_t s_v[VID ? CHUNK : 1];  // IDS, CONTRIB: drawn id of the staged splats
+    __shared__ uint32_t s_cw[CONTRIB ? 3 * CW_HITS : 1];   // CONTRIB: [sum q | hits | peak bits][warp][staged splat]
     __shared__ uint32_t s_vote[THREADS / 32];
     __shared__ uint32_t s_tile;
 
     const uint32_t tid = threadIdx.x, lane = tid & 31u, warp = tid >> 5;
+    bool accumulate = false;   // CONTRIB: the frame's pairs did not overflow the duplicate capacity
+    if constexpr (CONTRIB) {
+        accumulate = p.frame->overflow == 0u;
+        if (accumulate && blockIdx.x == 0 && tid == 0 && mo.frames) atomicAdd(mo.frames, 1u);
+    }
     {   // sparse frame: only the first `comp_cta_limit` CTAs (one per SM: the block scheduler deals a fresh grid breadth-first) work
         const uint32_t limit = p.frame->comp_cta_limit;
         if (limit && blockIdx.x >= limit) return;
@@ -391,6 +429,7 @@ __device__ __forceinline__ void composite_tiles(const CompositeArgs p, const Sec
         IdStateOf<IDS> ids;                              // IDS: largest w so far (0: none) and its drawn id
         if constexpr (IDS) ids = IdState{0.f, 0.f, NO_ID, NO_ID};
         float z0 = __uint_as_float(0x7f800000u), z1 = z0; // DEPTH: scene depth (+inf: nothing occludes; also outside the image)
+        const bool in0 = py < p.height && px0 < p.width, in1 = py < p.height && px0 + 1 < p.width;   // CONTRIB: inside the image
         if (DEPTH && p.scene_depth && py < p.height) {
             const float *zrow = p.scene_depth + (uint64_t)py * (uint64_t)p.width;
             if (px0 < p.width) z0 = zrow[px0];
@@ -398,12 +437,12 @@ __device__ __forceinline__ void composite_tiles(const CompositeArgs p, const Sec
         }
 
         Staged n0 = null_splat(), n1 = null_splat();
-        Pending<MOTION, IDS> q0, q1;   // MOTION: the gathered splats' pending motion loads; IDS: their drawn ids
+        Pending<MOTION, VID> q0, q1;   // MOTION: the gathered splats' pending motion loads; IDS, CONTRIB: their drawn ids
         if constexpr (MOTION) { q0 = null_motion(); q1 = null_motion(); }
-        else if constexpr (IDS) { q0.v = NO_ID; q1.v = NO_ID; }
+        else if constexpr (VID) { q0.v = NO_ID; q1.v = NO_ID; }
         if (num_iterations > 0) {
-            if ((int)tid < num_splats) n0 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + tid, vz, &q0, &mo);
-            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + tid + THREADS, vz, &q1, &mo);
+            if ((int)tid < num_splats) n0 = gather<DEPTH, MOTION, VID>(p.records, p.values, bounds.x + tid, vz, &q0, motion_param<MOTION>(mo));
+            if ((int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION, VID>(p.records, p.values, bounds.x + tid + THREADS, vz, &q1, motion_param<MOTION>(mo));
         }
 
         int consumed = 0;  // chunks blended before the stop rule fired (next frame's scheduling hint)
@@ -416,16 +455,20 @@ __device__ __forceinline__ void composite_tiles(const CompositeArgs p, const Sec
             s_a[tid + THREADS] = n1.a; s_b[tid + THREADS] = n1.b; s_c[tid + THREADS] = n1.c;
             if constexpr (DEPTH) { s_d[tid] = n0.d; s_d[tid + THREADS] = n1.d; }
             if constexpr (MOTION) { s_m[tid] = motion_of(mo, q0); s_m[tid + THREADS] = motion_of(mo, q1); }
-            if constexpr (IDS) { s_v[tid] = q0.v; s_v[tid + THREADS] = q1.v; }   // (a null splat: alpha 0, w = 0, never the pixel's)
+            if constexpr (VID) { s_v[tid] = q0.v; s_v[tid + THREADS] = q1.v; }   // (a null splat: alpha 0, w = 0, never the pixel's)
+            if constexpr (CONTRIB) {   // no hits yet: a warp that leaves the chunk early adds nothing
+#pragma unroll
+                for (int w = 0; w < THREADS / 32; ++w) { s_cw[CW_HITS + w * CHUNK + tid] = 0u; s_cw[CW_HITS + w * CHUNK + tid + THREADS] = 0u; }
+            }
             __syncthreads();
             // prefetch the next chunk's records while this one is blended (slots past the list end become null splats)
             n0 = null_splat(); n1 = null_splat();
             if constexpr (MOTION) { q0 = null_motion(); q1 = null_motion(); }
-            else if constexpr (IDS) { q0.v = NO_ID; q1.v = NO_ID; }
+            else if constexpr (VID) { q0.v = NO_ID; q1.v = NO_ID; }
             if (i + 1 < num_iterations) {
                 const int nb = sort_offset + CHUNK;
-                if (nb + (int)tid < num_splats) n0 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz, &q0, &mo);
-                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION, IDS>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz, &q1, &mo);
+                if (nb + (int)tid < num_splats) n0 = gather<DEPTH, MOTION, VID>(p.records, p.values, bounds.x + (uint32_t)nb + tid, vz, &q0, motion_param<MOTION>(mo));
+                if (nb + (int)tid + THREADS < num_splats) n1 = gather<DEPTH, MOTION, VID>(p.records, p.values, bounds.x + (uint32_t)nb + tid + THREADS, vz, &q1, motion_param<MOTION>(mo));
             }
 
             // :79-91, GU splats per iteration; `chunk` rounded up to GU reads null splats (opacity 0 => exact no-op).  Software-pipelined:
@@ -448,8 +491,8 @@ __device__ __forceinline__ void composite_tiles(const CompositeArgs p, const Sec
 #pragma unroll
                 for (int u = 0; u < GU; ++u) { A[u] = s_a[jn + u]; B[u] = s_b[jn + u]; }
                 bool alive_mid = true;
-                phase_b<CONTRACT, DEPTH, MOTION, IDS>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2, s_m, &mx2, &my2,
-                                                      s_v, &ids);
+                phase_b<CONTRACT, DEPTH, MOTION, IDS, CONTRIB>(Bc, s_c, s_d, j, al2, om2, cr2, cg2, cb2, t0, t1, alive_mid, z0, z1, o0, o1, dd2, s_m,
+                                                               &mx2, &my2, s_v, &ids, s_cw + warp * CHUNK, in0, in1);
                 go = __any_sync(0xffffffffu, alive_mid);
             }
 
@@ -462,6 +505,33 @@ __device__ __forceinline__ void composite_tiles(const CompositeArgs p, const Sec
             uint32_t shared_t = 0;
 #pragma unroll
             for (int w = 0; w < THREADS / 32; ++w) shared_t += s_vote[w];
+            if constexpr (CONTRIB) {   // the chunk's hits -> the source-slot records (this thread staged splats tid and tid + THREADS)
+                for (int h = (int)tid; accumulate && h < chunk; h += THREADS) {
+                    unsigned long long qsum = 0ull;
+                    uint32_t hits = 0u, peak = 0u;
+#pragma unroll
+                    for (int w = 0; w < THREADS / 32; ++w) {
+                        const uint32_t n = s_cw[CW_HITS + w * CHUNK + h];   // 0: the warp had no hit (its other words are stale)
+                        hits += n;
+                        qsum += n ? (unsigned long long)s_cw[w * CHUNK + h] : 0ull;
+                        const uint32_t pw = n ? s_cw[CW_PEAK + w * CHUNK + h] : 0u;
+                        peak = pw > peak ? pw : peak;
+                    }
+                    if (hits) {
+                        const uint32_t v = s_v[h];
+                        uint64_t slot = v;
+                        if (mo.warp_inst) {
+                            const InstanceDesc d = mo.desc[__ldg(mo.warp_inst + (v >> 5))];
+                            slot = d.first + (v - 32u * d.warp0);
+                        }
+                        gsr_splat_contribution *r = mo.accum + slot;
+                        atomicAdd(reinterpret_cast<unsigned long long *>(&r->weight), qsum);
+                        atomicAdd(reinterpret_cast<unsigned long long *>(&r->pixels), (unsigned long long)hits);
+                        atomicMax(reinterpret_cast<int *>(&r->peak), (int)peak);
+                        if (atomicExch(&r->last_frame, mo.epoch) != mo.epoch) atomicAdd(&r->views, 1u);
+                    }
+                }
+            }
             if (!(shared_t > 255u)) break;
         }
 
@@ -537,6 +607,14 @@ __global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_ids_ke
     composite_tiles<CONTRACT, true, MOTION, true>(p, mo);
 }
 
+// Splat contribution (gsr_set_splat_contribution): the depth-compositing frame plus the accumulation into the contribution buffer.  A
+// kernel of its own like composite_ids_kernel.
+template <bool CONTRACT>
+__global__ void __launch_bounds__(THREADS, GSR_COMP_MIN_BLOCKS) composite_contrib_kernel(const __grid_constant__ CompositeArgs p,
+                                                                                         const __grid_constant__ ContribArgs mo) {
+    composite_tiles<CONTRACT, true, false, false, true>(p, mo);
+}
+
 }  // namespace
 
 #ifndef GSR_CPU_EMU
@@ -552,11 +630,13 @@ int preload_composite_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<false, false>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<true, true>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_ids_kernel<false, true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_contrib_kernel<true>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, composite_contrib_kernel<false>));
     return GSR_OK;
 }
 
 int composite_max_ctas_per_sm(int *out) {
-    int a = 0, b = 0, c = 0, d = 0, e = 0, f = 0, g = 0, h = 0, i = 0, j = 0;
+    int a = 0, b = 0, c = 0, d = 0, e = 0, f = 0, g = 0, h = 0, i = 0, j = 0, k = 0, l = 0;
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, composite_kernel<true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, composite_kernel<false>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, composite_kernel<true, true>, THREADS, 0));
@@ -567,6 +647,8 @@ int composite_max_ctas_per_sm(int *out) {
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&h, composite_ids_kernel<false, false>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&i, composite_ids_kernel<true, true>, THREADS, 0));
     GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&j, composite_ids_kernel<false, true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&k, composite_contrib_kernel<true>, THREADS, 0));
+    GSR_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&l, composite_contrib_kernel<false>, THREADS, 0));
     if (c < a) a = c;
     if (d < b) b = d;
     if (e < a) a = e;
@@ -575,16 +657,21 @@ int composite_max_ctas_per_sm(int *out) {
     if (h < b) b = h;
     if (i < a) a = i;
     if (j < b) b = j;
+    if (k < a) a = k;
+    if (l < b) b = l;
     *out = a < b ? a : b;
     if (*out < 1) *out = 1;
     return GSR_OK;
 }
 
-int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion, const SplatIdArgs *ids) {
+int launch_composite(const CompositeArgs &a, cudaStream_t stream, const MotionArgs *motion, const SplatIdArgs *ids, const ContribArgs *contrib) {
     if (a.num_tiles <= 0) return GSR_OK;
     const int per_sm = a.ctas_per_sm > 0 ? a.ctas_per_sm : 1;
     const int grid = a.num_tiles < a.sm_count * per_sm ? a.num_tiles : a.sm_count * per_sm;
-    if (a.depth_out && ids && motion) {   // splat IDs and motion vectors (gsr_set_splat_ids + gsr_set_motion_vectors)
+    if (a.depth_out && contrib) {   // splat contribution (gsr_set_splat_contribution; never with motion vectors or IDs)
+        if (a.contract) composite_contrib_kernel<true><<<grid, THREADS, 0, stream>>>(a, *contrib);
+        else composite_contrib_kernel<false><<<grid, THREADS, 0, stream>>>(a, *contrib);
+    } else if (a.depth_out && ids && motion) {   // splat IDs and motion vectors (gsr_set_splat_ids + gsr_set_motion_vectors)
         WithIds<true> x;
         static_cast<MotionArgs &>(x) = *motion;
         x.ids = *ids;

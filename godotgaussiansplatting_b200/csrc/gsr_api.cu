@@ -114,6 +114,11 @@ struct gsr_ctx {
     float *motion_out = nullptr;
     // splat IDs (gsr_set_splat_ids, with depth compositing): caller-owned W*H uint32 pair plane; nullptr = off
     uint32_t *ids_out = nullptr;
+    // splat contribution (gsr_set_splat_contribution, with depth compositing): caller-owned max_splats records; nullptr = off.  The
+    // device frame counter is allocated by the first set; contrib_epoch is the epoch of the last frame enqueued (0: none yet).
+    gsr_splat_contribution *contrib = nullptr;
+    uint32_t *contrib_frames = nullptr;
+    uint32_t contrib_epoch = 0;
     // The camera and instance transforms of a frame, recorded for every frame enqueued by gsr_render* (motion on or off): `mot_last` is
     // the last enqueued frame's, the previous state of the next frame; `mot_used` is the previous state the last frame was enqueued
     // with (gsr_render's re-render of an overflowed frame uses it again).  valid == false: no previous frame (first frame, gsr_resize,
@@ -410,6 +415,7 @@ void free_ctx(gsr_ctx *c) {
     if (c->store_ready) cudaEventDestroy(c->store_ready);
     cudaFree(c->hist);
     cudaFree(c->export_words);
+    cudaFree(c->contrib_frames);
     free_compressed(c->cply);
     free_neighbors(c->nb);
     if (c->hist_host) cudaFreeHost(c->hist_host);
@@ -692,6 +698,7 @@ GSR_API int gsr_resize(gsr_ctx *c, int32_t width, int32_t height) {
     c->scene_depth = nullptr; c->depth_out = nullptr;   // the caller's depth planes have the old size: depth compositing is off
     c->motion_out = nullptr; c->mot_last.valid = false;   // so are motion vectors, and the next frame has no previous one
     c->ids_out = nullptr;                                  // and splat IDs
+    c->contrib = nullptr;                                  // and splat contribution
     cudaFree(c->pick_strip); c->pick_strip = nullptr;
     GSR_CUDA_TRY(cudaMalloc((void **)&c->bounds, sizeof(uint2) * (size_t)tx * ty));
     GSR_CUDA_TRY(cudaMalloc((void **)&c->comp_order, sizeof(uint32_t) * (size_t)tx * ty));
@@ -900,6 +907,9 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     const gsr_ctx::MotionState &prev = same_frame ? c->mot_used : c->mot_last;
     // splat IDs (gsr_set_splat_ids), read here as well
     const bool ids = c->ids_out && c->depth_out;
+    // splat contribution (gsr_set_splat_contribution), and the frame's epoch (a re-render keeps its frame's)
+    const bool contrib = c->contrib && c->depth_out;
+    if (contrib && !same_frame) c->contrib_epoch = c->contrib_epoch + 1u ? c->contrib_epoch + 1u : 1u;
     {
         uint32_t links = projection_num_blocks((uint32_t)(inst ? c->inst.drawn : c->max_splats));
         if (gf) {
@@ -1121,7 +1131,12 @@ static int render_enqueue(gsr_ctx *c, const float *view_proj, const void *unifor
     SplatIdArgs sa;
     sa.ids_out = c->ids_out;
     sa.warp_inst = inst ? c->inst.warps : nullptr;
-    if ((rc = launch_composite(ca, s, motion ? &ma : nullptr, ids ? &sa : nullptr))) return rc;
+    ContribArgs cb;
+    cb.accum = c->contrib;
+    cb.warp_inst = inst ? c->inst.warps : nullptr; cb.desc = c->inst.desc;
+    cb.frames = c->contrib_frames;
+    cb.epoch = c->contrib_epoch;
+    if ((rc = launch_composite(ca, s, motion ? &ma : nullptr, ids ? &sa : nullptr, contrib ? &cb : nullptr))) return rc;
     launches += ca.num_tiles > 0 ? 1 : 0;
     if (gf && !gf->rows_local) {   // rows have landed in the presenting rank's frame: tell it (system-scope flag store after the kernel boundary)
         if ((rc = launch_group_signal_done(group_peers(c, gf->parity), 0, c->grp.rank, gf->seq, s))) return rc;
@@ -1522,6 +1537,7 @@ GSR_API int gsr_set_depth_compositing(gsr_ctx *c, const float *scene_depth_devic
         c->scene_depth = nullptr; c->depth_out = nullptr;
         c->motion_out = nullptr;   // motion vectors are a companion of the mode
         c->ids_out = nullptr;      // and so are splat IDs
+        c->contrib = nullptr;      // and splat contribution
         return GSR_OK;
     }
     if (c->width == 0) { set_last_error("gsr_set_depth_compositing before gsr_resize"); return GSR_ERR_STATE; }
@@ -1534,6 +1550,7 @@ GSR_API int gsr_set_motion_vectors(gsr_ctx *c, float *motion_out_device) {
     if (!c) return GSR_ERR_INVALID;
     if (!motion_out_device) { c->motion_out = nullptr; return GSR_OK; }
     if (!c->depth_out) { set_last_error("gsr_set_motion_vectors: depth compositing is off"); return GSR_ERR_STATE; }
+    if (c->contrib) { set_last_error("gsr_set_motion_vectors: splat contribution is on"); return GSR_ERR_STATE; }
     if (motion_out_device == c->depth_out || motion_out_device == c->scene_depth) {
         set_last_error("gsr_set_motion_vectors: the motion plane is the depth output or the scene depth");
         return GSR_ERR_INVALID;
@@ -1550,12 +1567,76 @@ GSR_API int gsr_set_splat_ids(gsr_ctx *c, uint32_t *ids_out_device) {
     if (!c) return GSR_ERR_INVALID;
     if (!ids_out_device) { c->ids_out = nullptr; return GSR_OK; }
     if (!c->depth_out) { set_last_error("gsr_set_splat_ids: depth compositing is off"); return GSR_ERR_STATE; }
+    if (c->contrib) { set_last_error("gsr_set_splat_ids: splat contribution is on"); return GSR_ERR_STATE; }
     const void *p = ids_out_device;
     if (p == (const void *)c->depth_out || p == (const void *)c->scene_depth || p == (const void *)c->motion_out) {
         set_last_error("gsr_set_splat_ids: the ID plane is the depth output, the scene depth or the motion plane");
         return GSR_ERR_INVALID;
     }
     c->ids_out = ids_out_device;   // read by the next render_enqueue: frames already enqueued keep their plane
+    return GSR_OK;
+}
+
+// ---- splat contribution (gsr_set_splat_contribution): the buffer is read when a frame is enqueued; the reset and the frame counter
+// are ordered on the render stream, where every frame's compositor runs
+static bool bytes_overlap(const void *a, size_t na, const void *b, size_t nb) {
+    const char *x = static_cast<const char *>(a), *y = static_cast<const char *>(b);
+    return a && b && x < y + nb && y < x + na;
+}
+
+GSR_API int gsr_set_splat_contribution(gsr_ctx *c, gsr_splat_contribution *accum_device, uint64_t slots) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!accum_device) { c->contrib = nullptr; return GSR_OK; }
+    if (slots != c->max_splats) {
+        set_last_error("gsr_set_splat_contribution: %llu slots, the context has max_splats %llu", (unsigned long long)slots,
+                       (unsigned long long)c->max_splats);
+        return GSR_ERR_INVALID;
+    }
+    if (!c->depth_out) { set_last_error("gsr_set_splat_contribution: depth compositing is off"); return GSR_ERR_STATE; }
+    const size_t bytes = sizeof(gsr_splat_contribution) * slots, pixels = (size_t)c->width * c->height;
+    if (bytes_overlap(accum_device, bytes, c->depth_out, sizeof(float) * pixels) ||
+        bytes_overlap(accum_device, bytes, c->scene_depth, sizeof(float) * pixels) ||
+        bytes_overlap(accum_device, bytes, c->motion_out, 2 * sizeof(float) * pixels) ||
+        bytes_overlap(accum_device, bytes, c->ids_out, 2 * sizeof(uint32_t) * pixels)) {
+        set_last_error("gsr_set_splat_contribution: the buffer overlaps the depth output, the scene depth, the motion or the ID plane");
+        return GSR_ERR_INVALID;
+    }
+    if (c->motion_out || c->ids_out) {
+        set_last_error("gsr_set_splat_contribution: motion vectors or splat IDs are on");
+        return GSR_ERR_STATE;
+    }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    if (!c->contrib_frames) {
+        cudaError_t e = cudaMalloc((void **)&c->contrib_frames, sizeof(uint32_t));
+        if (e != cudaSuccess) {
+            c->contrib_frames = nullptr;
+            set_last_error("gsr_set_splat_contribution: frame counter -> %s", cudaGetErrorString(e));
+            return e == cudaErrorMemoryAllocation ? GSR_ERR_OOM : GSR_ERR_CUDA;
+        }
+    }
+    GSR_CUDA_TRY(cudaMemsetAsync(c->contrib_frames, 0, sizeof(uint32_t), c->stream));
+    c->contrib = accum_device;   // read by the next render_enqueue: frames already enqueued keep their buffer
+    return GSR_OK;
+}
+
+GSR_API int gsr_reset_splat_contribution(gsr_ctx *c) {
+    if (!c) return GSR_ERR_INVALID;
+    if (!c->contrib) { set_last_error("gsr_reset_splat_contribution: no contribution buffer is set"); return GSR_ERR_STATE; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    GSR_CUDA_TRY(cudaMemsetAsync(c->contrib, 0, sizeof(gsr_splat_contribution) * c->max_splats, c->stream));
+    GSR_CUDA_TRY(cudaMemsetAsync(c->contrib_frames, 0, sizeof(uint32_t), c->stream));
+    return GSR_OK;
+}
+
+GSR_API int gsr_splat_contribution_frames(gsr_ctx *c, uint32_t *frames) {
+    if (!c || !frames) { set_last_error("gsr_splat_contribution_frames: NULL argument"); return GSR_ERR_INVALID; }
+    if (!c->contrib) { set_last_error("gsr_splat_contribution_frames: no contribution buffer is set"); return GSR_ERR_STATE; }
+    int rc = use_device(c->device);
+    if (rc) return rc;
+    GSR_CUDA_TRY(cudaMemcpyAsync(frames, c->contrib_frames, sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
+    GSR_CUDA_TRY(cudaStreamSynchronize(c->stream));
     return GSR_OK;
 }
 
@@ -2160,7 +2241,10 @@ GSR_API int gsr_set_splat_count(gsr_ctx *c, uint64_t n) {
 
 // ---- splat property selection: gsr_select_where is enqueued like the selections, gsr_splat_histogram like the store edits ----------
 static int check_property(const gsr_splat_filter &f, const char *where, uint32_t i) {
-    if (f.property < GSR_PROP_OPACITY || f.property > GSR_PROP_COLOR_DISTANCE) { set_last_error("%s: filter %u: unknown property %d", where, i, f.property); return GSR_ERR_INVALID; }
+    if ((f.property < GSR_PROP_OPACITY || f.property > GSR_PROP_COLOR_DISTANCE) && !prop_is_contrib(f.property)) {
+        set_last_error("%s: filter %u: unknown property %d", where, i, f.property);
+        return GSR_ERR_INVALID;
+    }
     if (f.property != GSR_PROP_COLOR_DISTANCE) return GSR_OK;   // rgb is ignored
     for (int k = 0; k < 3; ++k) {
         if (!(fabsf(f.rgb[k]) <= 3.402823466e38f)) { set_last_error("%s: filter %u: non-finite rgb[%d]", where, i, k); return GSR_ERR_INVALID; }
@@ -2186,9 +2270,10 @@ GSR_API int gsr_select_where(gsr_ctx *c, const gsr_splat_filter *filters, uint32
     for (uint32_t i = 0; i < n; ++i) {
         if ((rc = check_property(filters[i], "gsr_select_where", i))) return rc;
         if (filters[i].lo != filters[i].lo || filters[i].hi != filters[i].hi) { set_last_error("gsr_select_where: filter %u: NaN bound", i); return GSR_ERR_INVALID; }
-        planes |= prop_planes(filters[i].property);
+        planes |= prop_sources(filters[i].property);
     }
     if (!select_op_valid(op)) { set_last_error("gsr_select_where: unknown op %d", op); return GSR_ERR_INVALID; }
+    if ((planes & PROP_PC) && !c->contrib) { set_last_error("gsr_select_where: a contribution property, and no contribution buffer is set"); return GSR_ERR_STATE; }
     WhereArgs a;
     memset(&a, 0, sizeof a);
     if ((rc = property_range(c, "gsr_select_where", instance, a.first, a.count))) return rc;
@@ -2197,7 +2282,11 @@ GSR_API int gsr_select_where(gsr_ctx *c, const gsr_splat_filter *filters, uint32
     a.soa = c->soa; a.plane_stride = c->plane_stride;
     a.n = n;
     memcpy(a.f, filters, sizeof(gsr_splat_filter) * n);
-    return launch_select_where(a, planes, sh_half(c), mask_stream(c));
+    a.contrib = c->contrib;
+    cudaStream_t s = mask_stream(c);
+    // the contribution buffer is written by the compositor of every earlier frame, on the render stream
+    if ((planes & PROP_PC) && (rc = store_stream(c, &s))) return rc;
+    return launch_select_where(a, planes, sh_half(c), s);
 }
 
 // ord (gsr_set_depth_order) back to the float
@@ -2214,6 +2303,10 @@ GSR_API int gsr_splat_histogram(gsr_ctx *c, const gsr_splat_filter *property, in
     int rc = check_property(*property, "gsr_splat_histogram", 0);
     if (rc) return rc;
     if (scope != GSR_HISTOGRAM_KEPT && scope != GSR_HISTOGRAM_SELECTED) { set_last_error("gsr_splat_histogram: unknown scope %d", scope); return GSR_ERR_INVALID; }
+    if (prop_is_contrib(property->property) && !c->contrib) {
+        set_last_error("gsr_splat_histogram: a contribution property, and no contribution buffer is set");
+        return GSR_ERR_STATE;
+    }
     HistArgs a;
     memset(&a, 0, sizeof a);
     if ((rc = property_range(c, "gsr_splat_histogram", instance, a.first, a.count))) return rc;
@@ -2253,7 +2346,8 @@ GSR_API int gsr_splat_histogram(gsr_ctx *c, const gsr_splat_filter *property, in
         a.counts = reinterpret_cast<unsigned long long *>(buf);
         a.keys = reinterpret_cast<int32_t *>(buf + HIST_KEYS_OFFSET);
         a.edges = reinterpret_cast<const float *>(buf + HIST_EDGES_OFFSET);
-        if ((rc = launch_splat_histogram(a, prop_planes(property->property), sh_half(c), c->sm_count, s))) return rc;
+        a.contrib = c->contrib;
+        if ((rc = launch_splat_histogram(a, prop_sources(property->property), sh_half(c), c->sm_count, s))) return rc;
         GSR_CUDA_TRY(cudaMemcpyAsync(img, buf, HIST_EDGES_OFFSET, cudaMemcpyDeviceToHost, s));
         GSR_CUDA_TRY(cudaStreamSynchronize(s));
         got = reinterpret_cast<unsigned long long *>(img);

@@ -587,9 +587,12 @@ __global__ void __launch_bounds__(COMPACT_THREADS) export_ply_kernel(const __gri
 // ---- gsr_select_where / gsr_splat_histogram: per-splat properties of the stored words (include/gsr.h "Splat property selection") ----
 // The planes of one splat beyond plane 0, each loaded the first time a property needs it, so a splat that failed an earlier filter
 // reads nothing more.  PL: the prop_planes bits of the filter set (a plane outside PL is never read); HALF: the SH format of plane 3.
-// Every value in float32, one rounding per operation, in the order of include/gsr.h.
+// Every value in float32, one rounding per operation, in the order of include/gsr.h.  PROP_PC in PL: the contribution properties are
+// read from the splat's record `rec` of the contribution buffer.
+template <bool PC> struct ContribRec {};
+template <> struct ContribRec<true> { const gsr_splat_contribution *rec = nullptr; };
 template <bool HALF, int PL>
-struct SplatProps {
+struct SplatProps : ContribRec<(PL & PROP_PC) != 0> {
     const float4 *src;   // plane 0 of the splat
     uint64_t st;
     float4 p1 = make_float4(0.0f, 0.0f, 0.0f, 0.0f), p2 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
@@ -598,6 +601,13 @@ struct SplatProps {
     __device__ __forceinline__ SplatProps(const float4 *s, uint64_t stride) : src(s), st(stride) {}
 
     __device__ __forceinline__ float value(const gsr_splat_filter &f) {
+        if constexpr ((PL & PROP_PC) != 0) {
+            const int32_t p = f.property;
+            if (p == GSR_PROP_CONTRIBUTION) return __fmul_rn((float)__ldg(reinterpret_cast<const unsigned long long *>(&this->rec->weight)), 0x1p-24f);
+            if (p == GSR_PROP_PEAK_CONTRIBUTION) return __ldg(&this->rec->peak);
+            if (p == GSR_PROP_VIEWS) return (float)__ldg(&this->rec->views);
+            if (p == GSR_PROP_CONTRIBUTING_PIXELS) return (float)__ldg(reinterpret_cast<const unsigned long long *>(&this->rec->pixels));
+        }
         const int need = prop_planes(f.property) & ~have;
         if constexpr ((PL & PROP_P1) != 0) if (need & PROP_P1) p1 = __ldg(src + st);
         if constexpr ((PL & PROP_P2) != 0) if (need & PROP_P2) p2 = __ldg(src + 2 * st);
@@ -649,6 +659,7 @@ __global__ void __launch_bounds__(SEL_THREADS) select_where_kernel(const __grid_
         const float4 *src = a.soa + s;
         in = !splat_vacant(__ldg(src));
         SplatProps<HALF, PL> sp(src, a.plane_stride);
+        if constexpr ((PL & PROP_PC) != 0) sp.rec = a.contrib + s;
 #pragma unroll 1
         for (uint32_t i = 0; in && i < a.n; ++i) {
             const float v = sp.value(a.f[i]);
@@ -693,6 +704,7 @@ __global__ void __launch_bounds__(PROP_HIST_THREADS) splat_histogram_kernel(cons
         const float4 *src = a.soa + s;
         if (splat_vacant(__ldg(src))) continue;
         SplatProps<HALF, PL> sp(src, a.plane_stride);
+        if constexpr ((PL & PROP_PC) != 0) sp.rec = a.contrib + s;
         const float v = sp.value(a.prop);
         uint32_t k = 0u;
         for (uint32_t step = a.top; step; step >>= 1) {
@@ -1020,8 +1032,18 @@ void launch_property_variant(const HistArgs &a, uint32_t blocks, cudaStream_t st
 }
 
 // The variants: the plane sets a filter set can need (plane 1 always comes with plane 2), and the SH format only where plane 3 is read.
+// A set that reads the contribution buffer takes the contribution-only variant, or with other properties the variant that can read
+// every plane (a plane is still loaded only when a filter needs it).
+constexpr int PROP_ALL = PROP_P1 | PROP_P2 | PROP_P3 | PROP_PC;
 template <class Args>
 int launch_property(const Args &a, int planes, bool sh_half, uint32_t blocks, cudaStream_t stream) {
+    if (planes & PROP_PC) {
+        if (planes == PROP_PC) launch_property_variant<false, PROP_PC>(a, blocks, stream);
+        else if (sh_half) launch_property_variant<true, PROP_ALL>(a, blocks, stream);
+        else launch_property_variant<false, PROP_ALL>(a, blocks, stream);
+        GSR_CUDA_TRY(cudaGetLastError());
+        return GSR_OK;
+    }
     switch (planes | (sh_half && (planes & PROP_P3) ? 8 : 0)) {
         case PROP_P2: launch_property_variant<false, PROP_P2>(a, blocks, stream); break;
         case PROP_P1 | PROP_P2: launch_property_variant<false, PROP_P1 | PROP_P2>(a, blocks, stream); break;
@@ -1162,6 +1184,12 @@ int preload_selection_kernels() {
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_P3>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_P2 | PROP_P3>));
     GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_P1 | PROP_P2 | PROP_P3>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_PC>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<false, PROP_ALL>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, select_where_kernel<true, PROP_ALL>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_PC>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<false, PROP_ALL>));
+    GSR_CUDA_TRY(cudaFuncGetAttributes(&fa, splat_histogram_kernel<true, PROP_ALL>));
     return GSR_OK;
 }
 #endif  // GSR_CPU_EMU

@@ -271,6 +271,25 @@ class GaussianSplattingRasterizer:
         compositing (set_depth_compositing first).  splat_sources maps the array to source splat indices."""
         _lib.check(_lib.lib().gsr_set_splat_ids(self._ctx, C.c_void_p(ids_out_ptr or None)), "gsr_set_splat_ids")
 
+    def set_splat_contribution(self, accum_ptr: int | None) -> None:
+        """Accumulate every splat's blend weight over the frames rendered from now on (include/gsr.h gsr_set_splat_contribution):
+        accum_ptr = a zeroed device array of max_splats 32-byte gsr_splat_contribution records (e.g. a torch uint8 tensor of
+        32 * max_splats bytes), one per source slot; None switches it off.  Needs depth compositing (set_depth_compositing first), and
+        neither motion vectors nor splat IDs.  read_splat_contribution decodes a downloaded copy; the GSR_PROP_CONTRIBUTION ..
+        properties select and histogram by it."""
+        _lib.check(_lib.lib().gsr_set_splat_contribution(self._ctx, C.c_void_p(accum_ptr or None), self._max_splats if accum_ptr else 0),
+                   "gsr_set_splat_contribution")
+
+    def reset_splat_contribution(self) -> None:
+        """Zero the contribution buffer and the frame counter, ordered between the frames enqueued before and after the call."""
+        _lib.check(_lib.lib().gsr_reset_splat_contribution(self._ctx), "gsr_reset_splat_contribution")
+
+    def splat_contribution_frames(self) -> int:
+        """The frames accumulated since the last set or reset; a frame that overflowed the duplicate capacity is not (synchronises)."""
+        n = C.c_uint32(0)
+        _lib.check(_lib.lib().gsr_splat_contribution_frames(self._ctx, C.byref(n)), "gsr_splat_contribution_frames")
+        return int(n.value)
+
     def splat_sources(self, ids: np.ndarray) -> np.ndarray:
         """The source splat index of every pixel of an (h, w, 2) array read back from set_splat_ids' plane, under the current instance
         layout (set_instances): GSR_NO_ID where the pixel has no splat.  Valid for frames rendered with that layout."""
@@ -758,9 +777,25 @@ def unpack_mask(words: np.ndarray, n: int) -> np.ndarray:
     return np.unpackbits(np.ascontiguousarray(words, dtype="<u4").view(np.uint8), bitorder="little")[:n].astype(bool)
 
 
+CONTRIBUTION_DTYPE = np.dtype([("weight", "<u8"), ("pixels", "<u8"), ("peak", "<f4"), ("views", "<u4"), ("last_frame", "<u4"),
+                               ("pad", "<u4")])   # gsr_splat_contribution
+
+
+def read_splat_contribution(buf) -> dict:
+    """Decode a contribution buffer (gsr_set_splat_contribution) downloaded to the host -- bytes, a uint8 array or a torch tensor on any
+    device -- into numpy arrays over the slots: weight (float64, the sum of q(w) / 2^24), pixels, peak and views."""
+    if hasattr(buf, "detach"):   # a torch tensor
+        buf = buf.detach().cpu().contiguous().view(-1).numpy()
+    raw = np.frombuffer(buf, dtype=np.uint8) if isinstance(buf, (bytes, bytearray, memoryview)) else np.ascontiguousarray(buf).view(np.uint8)
+    rec = raw.view(CONTRIBUTION_DTYPE)
+    return {"weight": rec["weight"].astype(np.float64) * 2.0 ** -24, "pixels": rec["pixels"].copy(), "peak": rec["peak"].copy(),
+            "views": rec["views"].copy()}
+
+
 def splat_filter(property: int, lo: float = -np.inf, hi: float = np.inf, rgb=None) -> _lib.GsrSplatFilter:
     """One gsr_splat_filter: the property (GSR_PROP_*) passes iff lo <= value <= hi; rgb is the reference colour of
-    GSR_PROP_COLOR_DISTANCE (default black; ignored by the other properties)."""
+    GSR_PROP_COLOR_DISTANCE (default black; ignored by the other properties).  GSR_PROP_CONTRIBUTION, _PEAK_CONTRIBUTION, _VIEWS
+    and _CONTRIBUTING_PIXELS read the contribution buffer of set_splat_contribution."""
     f = _lib.GsrSplatFilter()
     f.property, f.lo, f.hi = int(property), float(lo), float(hi)
     f.rgb[:] = [float(x) for x in (rgb if rgb is not None else (0.0, 0.0, 0.0))]

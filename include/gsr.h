@@ -745,6 +745,11 @@ GSR_API int gsr_set_splat_count(gsr_ctx *ctx, uint64_t n);
 #define GSR_PROP_VOLUME 2
 #define GSR_PROP_ISOTROPY 3
 #define GSR_PROP_COLOR_DISTANCE 4
+/* read from the contribution buffer, not from the stored words: see "Splat contribution" below (5 .. 15 stay unknown) */
+#define GSR_PROP_CONTRIBUTION 16
+#define GSR_PROP_PEAK_CONTRIBUTION 17
+#define GSR_PROP_VIEWS 18
+#define GSR_PROP_CONTRIBUTING_PIXELS 19
 #define GSR_MAX_SPLAT_FILTERS 8
 typedef struct gsr_splat_filter {
     int32_t property;   /* GSR_PROP_* */
@@ -757,6 +762,52 @@ GSR_API int gsr_select_where(gsr_ctx *ctx, const gsr_splat_filter *filters, uint
 #define GSR_HISTOGRAM_SELECTED 1   /* only the selected ones */
 GSR_API int gsr_splat_histogram(gsr_ctx *ctx, const gsr_splat_filter *property, int32_t instance, int32_t scope, const float *edges,
                                 uint32_t bins, uint64_t *counts, float minmax[2]);
+
+/* ---- Splat contribution: how much every stored splat shows up in the rendered views, accumulated on the GPU over any number of
+ *      depth-composited frames, so a host can select and prune the splats that contribute least (no reference counterpart).
+ *      accum_device: caller-owned device array of `slots` records, one per source slot [0, max_splats); `slots` must equal max_splats
+ *      (GSR_ERR_INVALID otherwise).  NULL switches the mode off.  The call does not zero the buffer: the host zeroes it, or calls
+ *      gsr_reset_splat_contribution.  The mode rules are those of gsr_set_splat_ids: GSR_ERR_STATE while depth compositing is off (a
+ *      NULL scene depth is enough); gsr_set_depth_compositing(ctx, NULL, NULL) and gsr_resize switch it off; its single-context rules
+ *      are those of depth compositing; the pointer is read when a frame is enqueued; gsr_pick does not accumulate.
+ *      GSR_ERR_INVALID, previous state kept: a buffer that aliases depth_out, scene_depth, motion_out or the ID plane.  GSR_ERR_STATE,
+ *      previous state kept: motion vectors or splat IDs are on (gsr_set_motion_vectors and gsr_set_splat_ids likewise refuse while the
+ * mode is on).  The call never synchronises; the first one allocates a 4-byte frame counter.
+ *      Rule: a frame enqueued with the mode on adds, for every pixel inside the image and every splat that the pixel's depth-composited
+ *      blend blends (the splats of the ID rule of gsr_set_splat_ids: same scene-depth stop, dead-pixel rule t > 1/255, sorted order and
+ *      tile-stop vote), with w = t - t' exactly the float32 w of the ID rule (the context's contraction mode), to the record of the
+ *      splat's SOURCE slot (the drawn id v without instances, first_k + (v - 32 w_k) with them) if w > 0:
+ *        weight += q(w) = __float2uint_rn(w * 2^24);  pixels += 1;  peak = max(peak, w);
+ *        views += 1 once per frame and slot, however many tiles, pixels and instances touch it.
+ *      Integer sums, a max and a once-per-frame count: every field is order-independent and bit-exact.  weight cannot overflow before
+ *      2^40 full-weight pixel hits.  Hidden splats, hidden instances and splats past an instance's draw_count are never blended.
+ *      A frame whose pairs overflowed the duplicate capacity adds nothing: gsr_render's re-render of an overflowed frame adds that frame
+ *      exactly once, and an asynchronous overflowed frame, or an overflowed frame under GSR_FLAG_STATIC_CAPACITY, adds nothing.  rgba
+ *      and depth_out are bit-identical to the same frame without the mode.
+ *      gsr_reset_splat_contribution: enqueues a zeroing of the buffer and of the frame counter, ordered after every frame enqueued before
+ *      it and before every later one; it never synchronises.  GSR_ERR_STATE if no buffer is set.
+ *      gsr_splat_contribution_frames: synchronises the context and returns the frames added since the last set or reset (the overflowed
+ *      ones are not).  GSR_ERR_STATE if no buffer is set.
+ *      Store edits do not touch the buffer, which is indexed by slot: after gsr_delete_hidden or gsr_duplicate_selection its
+ *      statistics are stale until a reset (the rank rule of gsr_delete_hidden lets a host remap them).
+ *      Properties for gsr_select_where and gsr_splat_histogram, read from the buffer, combinable with the others in one filter set:
+ *        GSR_PROP_CONTRIBUTION         (float)weight * 2^-24 (a round to nearest, then an exact scale)
+ *        GSR_PROP_PEAK_CONTRIBUTION    peak
+ *        GSR_PROP_VIEWS                (float)views
+ *        GSR_PROP_CONTRIBUTING_PIXELS  (float)pixels
+ *      They refuse with GSR_ERR_STATE while no buffer is set, and are ordered after the compositor of every frame enqueued before the
+ *      call. ---- */
+typedef struct gsr_splat_contribution {
+    uint64_t weight;      /* sum of q(w) over every blended (pixel, frame, drawn copy) with w > 0 */
+    uint64_t pixels;      /* number of those (pixel, frame, drawn copy) triples */
+    float peak;           /* the largest w, +0 if none */
+    uint32_t views;       /* accumulated frames in which the splat had some w > 0 */
+    uint32_t last_frame;  /* library-owned (the views rule); hosts do not interpret it */
+    uint32_t pad;
+} gsr_splat_contribution; /* 32 bytes */
+GSR_API int gsr_set_splat_contribution(gsr_ctx *ctx, gsr_splat_contribution *accum_device, uint64_t slots);
+GSR_API int gsr_reset_splat_contribution(gsr_ctx *ctx);
+GSR_API int gsr_splat_contribution_frames(gsr_ctx *ctx, uint32_t *frames);
 
 /* ---- Splat neighbourhood selection: select splats by the splats around them -- isolated floaters, one step of "select more", the
  *      object under a clicked splat, every small clump (no reference counterpart).  Queries run on a spatial grid on the GPU.
